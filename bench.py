@@ -2,7 +2,7 @@
 """bench.py -- rays/s of the FruitNeRF hot path (fused field + compositing, forward + backward) on
 synthetic 4096-ray x 192-sample batches (BASELINE.json metric), N GPUs of one node.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--variant small|big] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--variant small|big] [--impl ours|reference] [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over one batch: render forward (hash encode -> MLPs ->
 composite), MSE + BCE loss, backward into the flat gradient buffer (and, for N > 1, one NCCL
@@ -31,6 +31,7 @@ NUM_IMAGES = 100
 CPU_BUDGET_S = 40.0  # wall-clock budget of the CPU arm inside the default run
 HASH_BYTES_PER_POINT_FWD = 16 * 8 * 2 * 4  # L levels x 8 corners x F=2 x fp32 (SURVEY.md 8d)
 HASH_BYTES_PER_POINT_BWD = 2 * HASH_BYTES_PER_POINT_FWD  # read-modify-write scatter
+DUMP_MAX_ELEMS = 1 << 20  # --dump-outputs: larger arrays are written as a fixed seeded sample of this many elements
 
 
 def _peaks():
@@ -38,13 +39,12 @@ def _peaks():
     if p.exists():
         j = json.loads(p.read_text())
         return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 class ClockSampler:
-    """SM clock / throttle-reason sampling during the timed region (B200_PROFILING.md clocks line),
-    through NVML in-process (an `nvidia-smi -lms` poller next to the 256 MiB L2-flush fills stalled
-    the GPU for ~10 ms per step on this pool; NVML queries from a thread do not)."""
+    """SM clock / throttle-reason sampling during the timed region, through NVML in-process (an
+    `nvidia-smi -lms` poller next to the 256 MiB L2-flush fills stalls the GPU; NVML queries from a thread do not)."""
 
     def __init__(self, index: int, period_s: float = 0.02):
         self.index, self.period = index, period_s
@@ -127,7 +127,7 @@ def step_fn(field, batch, world, impl_id):
     return out, loss
 
 
-DTYPE = "f32 (parameters, gather, compositing and accumulators fp32; MLP products on tcgen05 as bf16 hi/lo splits, 3 MMAs per product, ~2^-16)"
+DTYPE = "f32 (parameters, gather, compositing, scatter and accumulators fp32; MLP products of forward and backward on wgmma as bf16 hi/lo splits, 4 MMAs per product, ~2^-17)"
 
 
 def _ncu_traffic(kernel: str):
@@ -143,9 +143,7 @@ def _ncu_traffic(kernel: str):
 def kernel_names(variant: str, kernel: str):
     if kernel == "simt":
         return "simt_field_forward_kernel + simt_composite_kernel", "simt_field_backward_kernel"
-    if variant == "small":
-        return "tc_render_forward_ws_kernel", "tc_field_backward_kernel"
-    return "tc_render_forward_big_kernel", "tc_big_backward_chain_kernel + tc_big_dw_kernel"
+    return "simt_field_forward_kernel<wgmma> + simt_composite_kernel", "simt_field_backward_kernel<wgmma>"  # auto / tcgen05
 
 
 def _stage(msg: str) -> None:
@@ -153,7 +151,28 @@ def _stage(msg: str) -> None:
         print(f"[bench {time.strftime('%H:%M:%S')}] {msg}", file=sys.stderr, flush=True)
 
 
-def measure_variant(variant: str, steps: int, warmup: int, args, world: int, rank: int, dev, impl_id, with_e2e: bool = True):
+def dump_step(step, field, out_dir: str) -> None:
+    """Write what the last replayed training step returned to its caller -- the loss, the render outputs and the parameter
+    gradients -- as float32 <name>.npy files.  Arrays above DUMP_MAX_ELEMS elements are written as the elements at a fixed
+    seeded set of flat indices (the same set for every run with the same arguments)."""
+    import numpy as np
+
+    names = {id(p): n for n, p in field.named_parameters()}
+    arrays = {"loss": step.loss}
+    arrays.update({k: v for k, v in step.outputs.items()})
+    arrays.update({f"grad.{names.get(id(p), i)}": p.grad for i, p in enumerate(step.params) if p.grad is not None})
+    out = Path(out_dir)
+    out.mkdir(parents=True, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy().reshape(-1)
+        if a.size > DUMP_MAX_ELEMS:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, DUMP_MAX_ELEMS, replace=False))
+            a = a[idx]
+        np.save(out / f"{name}.npy", a.astype(np.float32))
+
+
+def measure_variant(variant: str, steps: int, warmup: int, args, world: int, rank: int, dev, impl_id, with_e2e: bool = True,
+                    dump_dir=None):
     """Device-timed step / forward / backward and (optionally) the end-to-end loop of one field variant."""
     from fruitnerf_b200 import _lib as L
     from fruitnerf_b200 import ops
@@ -166,7 +185,7 @@ def measure_variant(variant: str, steps: int, warmup: int, args, world: int, ran
     o, d, s, e, cam = syn.ray_batch(R_RAYS, S_SAMPLES, salt=rank, num_images=NUM_IMAGES)
     img, mask = syn.targets(R_RAYS, salt=rank)
     host = [t.pin_memory() for t in (o, d, s, e, cam.to(torch.int32), img, mask)]
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)  # > 50 MB L2 of the H100
 
     # the public training-step API: render fwd + loss + bwd captured in one CUDA graph
     exchange = None
@@ -217,6 +236,8 @@ def measure_variant(variant: str, steps: int, warmup: int, args, world: int, ran
 
         dist.barrier()
     clocks = sampler.stop() if sampler else None
+    if dump_dir is not None:
+        dump_step(step, field, dump_dir)
     step_ms = [ev[0].elapsed_time(ev[1]) for ev in evs]
     if os.environ.get("FNR_BENCH_DEBUG"):
         print(f"rank {rank} {variant} step_ms " + " ".join(f"{v:.3f}" for v in step_ms), file=sys.stderr)
@@ -451,7 +472,7 @@ def measure_export(dev, n: int = 512, batch: int = 32768):
     return {"workload": f"uniform {n}^3 volume sample of the fruit_nerf field, {batch} rays x {n} samples per launch, deterministic grid",
             "ms": ms, "points": total, "points_per_s": total / (ms * 1e-3), "counts": counts, "thresholds": thr,
             "keys_unique_and_nested": bool(ok), "gpu_launches": launches,
-            "roofline": {"kernel": "tc_render_forward_ws_kernel<export>", "bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s",
+            "roofline": {"kernel": "simt_export_kernel<wgmma>", "bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s",
                          "frac": ach / peak, "algorithmic_bytes": total * HASH_BYTES_PER_POINT_FWD}}
 
 
@@ -474,7 +495,8 @@ def run_ours(args):
         dist.init_process_group("nccl", device_id=dev)
     impl_id = {"auto": L.FNR_IMPL_AUTO, "simt": L.FNR_IMPL_SIMT, "tcgen05": L.FNR_IMPL_TCGEN05}[args.kernel]
     warm = max(args.warmup, 3)
-    head = measure_variant(args.variant, args.steps, warm, args, world, rank, dev, impl_id)
+    head = measure_variant(args.variant, args.steps, warm, args, world, rank, dev, impl_id,
+                           dump_dir=args.dump_outputs if rank == 0 else None)
     variants = {}
     if args.variant == "small" and not args.no_variants:
         # BASELINE.json configs[2] / [3]: fruit_nerf_big, same batch shape, same timing rules (fewer timed steps)
@@ -694,6 +716,9 @@ def main():
     ap.add_argument("--no-graph", action="store_true", help="diagnostic: eager step instead of the CUDA-graph step")
     ap.add_argument("--no-flush", action="store_true", help="diagnostic: skip the L2 flush between timed steps")
     ap.add_argument("--no-clocks", action="store_true", help="diagnostic: do not sample nvidia-smi during the timed region")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the loss, render outputs and gradients of the last step as DIR/<name>.npy "
+                         "(float32; arrays above 2^20 elements as a fixed seeded sample)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

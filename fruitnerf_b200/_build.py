@@ -1,4 +1,7 @@
-"""In-tree build of libfruitnerf_b200.so (sm_100a) with nvcc.  Used by __graft_entry__.build()."""
+"""In-tree build of libfruitnerf_b200.so (sm_90a, H100) with nvcc.  Used by __graft_entry__.build().
+
+The tensor-core path (impl = tcgen05 / auto) is the wgmma instantiation of the kernels in fnr_simt.cu (fnr_wgmma.cuh,
+dispatch in fnr_tc.cu).  The fused Blackwell kernels are kept outside the library under design/blackwell/."""
 from __future__ import annotations
 
 import os
@@ -8,9 +11,10 @@ from pathlib import Path
 
 CSRC = Path(__file__).resolve().parent / "csrc"
 LIB = CSRC / "libfruitnerf_b200.so"
-SOURCES = ["fnr_api.cu", "fnr_simt.cu", "fnr_tc.cu", "fnr_tc_ws.cu", "fnr_tc_big.cu", "fnr_tc_big_bwd.cu", "fnr_tc_bwd.cu", "fnr_proposal.cu", "fnr_optim.cu", "fnr_glue.cu", "fnr_nvls.cu"]
+STAMP = CSRC / "libfruitnerf_b200.recipe"  # flags and sources LIB was built from
+SOURCES = ["fnr_api.cu", "fnr_simt.cu", "fnr_tc.cu", "fnr_proposal.cu", "fnr_optim.cu", "fnr_glue.cu", "fnr_nvls.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-O2",
 ]
@@ -31,6 +35,10 @@ def _stale(target: Path, deps) -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
+    # objects built with other flags or sources (an older architecture, say) are stale whatever their mtimes
+    recipe = " ".join([*NVCC_FLAGS, *SOURCES])
+    if not STAMP.exists() or STAMP.read_text() != recipe:
+        force = True
     headers = list(CSRC.glob("*.cuh")) + list(CSRC.glob("*.h")) + [CSRC.parent.parent / "include" / "fruitnerf_b200.h"]
     objs = []
     procs = []
@@ -53,6 +61,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}{r.stderr}")
+        STAMP.write_text(recipe)
     return LIB
 
 

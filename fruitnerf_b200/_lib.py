@@ -215,7 +215,7 @@ def load() -> C.CDLL:
     if not path.exists():
         raise FruitNerfNativeError(
             f"{path} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a).  fruitnerf_b200 has no CPU / PyTorch fallback."
+            "(nvcc, sm_90a).  fruitnerf_b200 has no CPU / PyTorch fallback."
         )
     lib = C.CDLL(str(path))
     lib.fnr_version.restype = C.c_int

@@ -1,7 +1,6 @@
 // extern "C" entry points of libfruitnerf_b200.so: argument validation, conversion of the plain-C
-// structs of include/fruitnerf_b200.h into kernel arguments, dispatch between the fused tcgen05
-// kernels and the fp32 simt kernels.  No host synchronisation, no allocation (the one exception: the cuBLAS handle the
-// big-family backward creates at its first call, fnr_tc_big_bwd.cu).
+// structs of include/fruitnerf_b200.h into kernel arguments, dispatch between the tensor-core
+// (wgmma) and the fp32 simt instantiations of the kernels (fnr_tc.cu).  No host synchronisation, no allocation.
 #include <atomic>
 #include <cstdarg>
 #include <cstdio>
@@ -206,13 +205,7 @@ int fnr_render_forward(const fnr_field_desc* desc, const fnr_field_params* param
 
   int impl = desc->impl;
   if (impl == FNR_IMPL_AUTO) impl = tc_supported(fam, F, Rr) ? FNR_IMPL_TCGEN05 : FNR_IMPL_SIMT;
-  if (impl == FNR_IMPL_TCGEN05) {
-    if (!tc_supported(fam, F, Rr)) {
-      set_error("tcgen05 render kernel does not support this shape (R=%d S=%d)", Rr.R, Rr.S);
-      return FNR_ERR_UNSUPPORTED;
-    }
-    return launch_tc_render_forward(fam, F, P, Rr, O, Cm, st);
-  }
+  if (impl == FNR_IMPL_TCGEN05) return launch_tc_render_forward(fam, F, P, Rr, O, Cm, st);
   if (impl != FNR_IMPL_SIMT) {
     set_error("invalid impl %d", impl);
     return FNR_ERR_INVALID_ARGUMENT;
@@ -234,8 +227,6 @@ int fnr_render_backward_scratch_bytes(const fnr_field_desc* desc, int32_t num_ra
     return FNR_ERR_INVALID_ARGUMENT;
   }
   *bytes = (size_t)num_rays * num_samples * 5 * sizeof(float) + 256;
-  // the big-family tensor-core backward stages every layer's X / dY for the cuBLAS weight-gradient GEMMs (fnr_tc_big_bwd.cu)
-  if (classify(desc) == kFamilyBig && desc->impl != FNR_IMPL_SIMT) *bytes += tc_big_backward_scratch_bytes((long long)num_rays * num_samples) + 256;
   return FNR_OK;
 }
 
@@ -290,17 +281,8 @@ int fnr_render_backward(const fnr_field_desc* desc, const fnr_field_params* para
   KFieldBwd FB{point_grads, saved->stash_encoding, saved->sample_rgb, scratch_bytes > used ? extra : nullptr,
                scratch_bytes > used ? scratch_bytes - used : 0};
   int impl = desc->impl;
-  const bool big_tc = fam == kFamilyBig && FB.extra_bytes >= tc_big_backward_scratch_bytes((long long)Rr.R * Rr.S) + 256 &&
-                      tc_big_backward_supported(F, FB);
-  if (impl == FNR_IMPL_AUTO) impl = (big_tc || tc_backward_supported(fam, F, Rr, FB)) ? FNR_IMPL_TCGEN05 : FNR_IMPL_SIMT;
-  if (impl == FNR_IMPL_TCGEN05) {
-    if (big_tc) return launch_tc_big_field_backward(F, P, G, Rr, FB, st);
-    if (!tc_backward_supported(fam, F, Rr, FB)) {
-      set_error("tcgen05 backward kernel does not support this configuration");
-      return FNR_ERR_UNSUPPORTED;
-    }
-    return launch_tc_field_backward(fam, F, P, G, Rr, FB, st);
-  }
+  if (impl == FNR_IMPL_AUTO) impl = tc_backward_supported(fam, F, Rr, FB) ? FNR_IMPL_TCGEN05 : FNR_IMPL_SIMT;
+  if (impl == FNR_IMPL_TCGEN05) return launch_tc_field_backward(fam, F, P, G, Rr, FB, st);
   return launch_simt_field_backward(fam, F, P, G, Rr, FB, st);
 }
 

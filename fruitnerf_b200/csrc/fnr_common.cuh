@@ -1,4 +1,4 @@
-// Shared device helpers of the FruitNeRF B200 hot path.
+// Shared device helpers of the FruitNeRF hot path.
 //
 // Index-defining arithmetic (sample position -> [0,1]^3 -> per-level cell -> hash row) is written
 // with explicit round-to-nearest intrinsics in the op order of the reference
@@ -145,13 +145,6 @@ __device__ __forceinline__ float nan_to_num(float v) {
   if (v != v) return 0.0f;
   if (isinf(v)) return v > 0.0f ? 3.4028234663852886e38f : -3.4028234663852886e38f;
   return v;
-}
-
-// 256-bit global store (STG.E.ENL2.256, sm_100+): one whole 32-byte sector per lane; dst must be 32-byte aligned
-__device__ __forceinline__ void st_global_v8(float* dst, float a0, float a1, float a2, float a3, float a4, float a5, float a6, float a7) {
-  asm volatile("st.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(dst), "f"(a0), "f"(a1), "f"(a2), "f"(a3), "f"(a4), "f"(a5), "f"(a6),
-               "f"(a7)
-               : "memory");
 }
 
 __device__ __forceinline__ float sigmoidf_(float v) { return 1.0f / (1.0f + expf(-v)); }

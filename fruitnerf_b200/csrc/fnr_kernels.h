@@ -223,25 +223,19 @@ int launch_simt_field_backward(Family fam, const KField& F, const KParams& P, co
 int launch_simt_export(Family fam, const KField& F, const KParams& P, const KExport& E, cudaStream_t st);
 int launch_hash_indices(const KField& F, const KRays& Rr, int32_t* rows, float* positions, cudaStream_t st);
 
-// fused tcgen05 forward (fnr_tc.cu).  Returns FNR_ERR_UNSUPPORTED when the shape is not covered.
+// tensor-core (wgmma, sm_90a) instantiations of the field forward / export kernels (fnr_simt.cu, fnr_wgmma.cuh)
+int launch_wgmma_field_forward(Family fam, const KField& F, const KParams& P, const KRays& Rr, const KFieldOut& O, cudaStream_t st);
+int launch_wgmma_export(Family fam, const KField& F, const KParams& P, const KExport& E, cudaStream_t st);
+int launch_wgmma_field_backward(Family fam, const KField& F, const KParams& P, const KParams& G, const KRays& Rr, const KFieldBwd& B,
+                                cudaStream_t st);
+
+// impl = tcgen05 / auto dispatch (fnr_tc.cu): the wgmma kernels above for the shipped families.
 bool tc_supported(Family fam, const KField& F, const KRays& Rr);
 bool tc_export_supported(Family fam, const KExport& E);
-bool tc_big_supported(int S);
-size_t tc_big_backward_scratch_bytes(long long num_points);
-bool tc_big_backward_supported(const KField& F, const KFieldBwd& B);
-int launch_tc_big_field_backward(const KField& F, const KParams& P, const KParams& G, const KRays& Rr, const KFieldBwd& B, cudaStream_t st);
-int launch_tc_render_forward_big(const KField& F, const KParams& P, const KRays& Rr, const KFieldOut& O, const KComposite& Cm, cudaStream_t st);
-int launch_tc_export_big(const KField& F, const KParams& P, const KExport& E, cudaStream_t st);
-// warp-specialised small-family forward / export (fnr_tc_ws.cu)
-bool tc_ws_supported(int S);
-int launch_tc_render_forward_ws(const KField& F, const KParams& P, const KRays& Rr, const KFieldOut& O, const KComposite& Cm, cudaStream_t st);
-int launch_tc_export_ws(const KField& F, const KParams& P, const KExport& E, cudaStream_t st);
-int launch_tc_export(Family fam, const KField& F, const KParams& P, const KExport& E, cudaStream_t st);
+bool tc_backward_supported(Family fam, const KField& F, const KRays& Rr, const KFieldBwd& B);
 int launch_tc_render_forward(Family fam, const KField& F, const KParams& P, const KRays& Rr, const KFieldOut& O,
                              const KComposite& Cm, cudaStream_t st);
-
-// tensor-core field backward (fnr_tc_bwd.cu)
-bool tc_backward_supported(Family fam, const KField& F, const KRays& Rr, const KFieldBwd& B);
+int launch_tc_export(Family fam, const KField& F, const KParams& P, const KExport& E, cudaStream_t st);
 int launch_tc_field_backward(Family fam, const KField& F, const KParams& P, const KParams& G, const KRays& Rr, const KFieldBwd& B,
                              cudaStream_t st);
 

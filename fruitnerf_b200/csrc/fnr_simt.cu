@@ -9,6 +9,7 @@
 // Reference semantics: fruit_nerf/fruit_field.py:168-301, fruit_nerf/fruit_nerf.py:251-269,316-357.
 #include "fnr_common.cuh"
 #include "fnr_kernels.h"
+#include "fnr_wgmma.cuh"
 
 namespace fnr {
 
@@ -141,6 +142,28 @@ __device__ __forceinline__ void hash_encode(const float2* __restrict__ table, co
 // ------------------------------------------------------------------------------------------
 // Field evaluation of one point.  Keeps the activations the backward needs when KEEP.
 // ------------------------------------------------------------------------------------------
+// How field_mlps evaluates a Linear layer: per thread in fp32 on the CUDA cores (the exact device reference), or
+// block-wide on the tensor cores (fnr_wgmma.cuh; every thread of the 128-thread CTA must take part).
+struct SimtLinear {
+  template <int K, int N, bool RELU>
+  static __device__ __forceinline__ void fwd(const float* __restrict__ W, const float* __restrict__ b, const float (&x)[K], float (&y)[N]) {
+    linear_fwd<K, N, RELU>(W, b, x, y);
+  }
+};
+template <class C>
+struct WgmmaLinear {
+  static constexpr int kSmemBytes = wg::Smem<C::MAXW, C::MAXW>::kBytes;
+  template <int K, int N, bool RELU>
+  static __device__ __forceinline__ void fwd(const float* __restrict__ W, const float* __restrict__ b, const float (&x)[K], float (&y)[N]) {
+    if constexpr (N < 8) {  // the 1- and 3-wide output heads: 64 MACs per point, exact fp32 on the CUDA cores
+      linear_fwd<K, N, RELU>(W, b, x, y);
+    } else {
+      extern __shared__ __align__(128) uint8_t wg_smem[];
+      wg::linear<C::MAXW, C::MAXW, K, N, RELU>(wg_smem, W, b, x, y);
+    }
+  }
+};
+
 template <class C>
 struct Acts {
   float h1[C::BASE_H];      // relu(base0)
@@ -154,24 +177,24 @@ struct Acts {
   float logit;
 };
 
-template <class C>
+template <class C, class Lin = SimtLinear>
 __device__ __forceinline__ void field_mlps(const KParams& P, const float (&enc)[C::ENC], const float* __restrict__ dir,
                                            const float* __restrict__ app, Acts<C>& a) {
-  linear_fwd<C::ENC, C::BASE_H, true>(P.base_w[0], P.base_b[0], enc, a.h1);
-  linear_fwd<C::BASE_H, C::BASE_OUT, false>(P.base_w[1], P.base_b[1], a.h1, a.out);
+  Lin::template fwd<C::ENC, C::BASE_H, true>(P.base_w[0], P.base_b[0], enc, a.h1);
+  Lin::template fwd<C::BASE_H, C::BASE_OUT, false>(P.base_w[1], P.base_b[1], a.h1, a.out);
   // semantic branch: mlp_semantics(detach(geo)) -> Linear head (fruit_field.py:263-268)
   float geo[C::GEO];
 #pragma unroll
   for (int i = 0; i < C::GEO; ++i) geo[i] = a.out[1 + i];
-  linear_fwd<C::GEO, C::SEM_H, true>(P.sem_w[0], P.sem_b[0], geo, a.z1);
+  Lin::template fwd<C::GEO, C::SEM_H, true>(P.sem_w[0], P.sem_b[0], geo, a.z1);
   if constexpr (C::SEM_LAYERS == 3) {
-    linear_fwd<C::SEM_H, C::SEM_H, true>(P.sem_w[1], P.sem_b[1], a.z1, a.z2);
-    linear_fwd<C::SEM_H, C::SEM_OUT, false>(P.sem_w[2], P.sem_b[2], a.z2, a.zo);
+    Lin::template fwd<C::SEM_H, C::SEM_H, true>(P.sem_w[1], P.sem_b[1], a.z1, a.z2);
+    Lin::template fwd<C::SEM_H, C::SEM_OUT, false>(P.sem_w[2], P.sem_b[2], a.z2, a.zo);
   } else {
-    linear_fwd<C::SEM_H, C::SEM_OUT, false>(P.sem_w[1], P.sem_b[1], a.z1, a.zo);
+    Lin::template fwd<C::SEM_H, C::SEM_OUT, false>(P.sem_w[1], P.sem_b[1], a.z1, a.zo);
   }
   float lg[1];
-  linear_fwd<C::SEM_OUT, 1, false>(P.head_w, P.head_b, a.zo, lg);
+  Lin::template fwd<C::SEM_OUT, 1, false>(P.head_w, P.head_b, a.zo, lg);
   a.logit = lg[0];
   // colour branch: cat[SH(dir), geo, appearance] -> MLP -> sigmoid (fruit_field.py:270-278)
   sh_degree4(dir[0], dir[1], dir[2], a.cin);
@@ -179,10 +202,10 @@ __device__ __forceinline__ void field_mlps(const KParams& P, const float (&enc)[
   for (int i = 0; i < C::GEO; ++i) a.cin[C::SH + i] = geo[i];
 #pragma unroll
   for (int i = 0; i < C::APP; ++i) a.cin[C::SH + C::GEO + i] = app[i];
-  linear_fwd<C::COL_IN, C::COL_H, true>(P.col_w[0], P.col_b[0], a.cin, a.c1);
-  linear_fwd<C::COL_H, C::COL_H, true>(P.col_w[1], P.col_b[1], a.c1, a.c2);
+  Lin::template fwd<C::COL_IN, C::COL_H, true>(P.col_w[0], P.col_b[0], a.cin, a.c1);
+  Lin::template fwd<C::COL_H, C::COL_H, true>(P.col_w[1], P.col_b[1], a.c1, a.c2);
   float o3[3];
-  linear_fwd<C::COL_H, 3, false>(P.col_w[2], P.col_b[2], a.c2, o3);
+  Lin::template fwd<C::COL_H, 3, false>(P.col_w[2], P.col_b[2], a.c2, o3);
 #pragma unroll
   for (int i = 0; i < 3; ++i) a.rgb[i] = sigmoidf_(o3[i]);
 }
@@ -204,12 +227,16 @@ __device__ __forceinline__ void block_mean_embedding(const KParams& P, int num_i
 // ------------------------------------------------------------------------------------------
 // K1: per-point field forward.
 // ------------------------------------------------------------------------------------------
-template <class C>
+// The loop runs whole 128-point tiles per CTA (threads past N compute a clamped point and store nothing), so that the
+// block-wide tensor-core layers of WgmmaLinear see every thread.
+template <class C, class Lin = SimtLinear>
 __global__ void __launch_bounds__(kThreads) simt_field_forward_kernel(KField F, KParams P, KRays Rr, KFieldOut O) {
   __shared__ float s_app[C::APP];
   block_mean_embedding(P, F.num_images, C::APP, F.appearance_mode, s_app);
   const long long N = (long long)Rr.R * Rr.S;
-  for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < N; p += (long long)gridDim.x * blockDim.x) {
+  for (long long p0 = (long long)blockIdx.x * blockDim.x; p0 < N; p0 += (long long)gridDim.x * blockDim.x) {
+    const bool valid = p0 + threadIdx.x < N;
+    const long long p = valid ? p0 + threadIdx.x : N - 1;
     const int r = (int)(p / Rr.S);
     const float* o = Rr.origins + 3 * (size_t)r;
     const float* d = Rr.directions + 3 * (size_t)r;
@@ -217,7 +244,7 @@ __global__ void __launch_bounds__(kThreads) simt_field_forward_kernel(KField F, 
     const Vec3 pos = field_position(o, d, Rr.starts[p], Rr.ends[p], F.position_mode, F.aabb, sel);
     float enc[C::ENC];
     hash_encode<C::L>(reinterpret_cast<const float2*>(P.hash_table), F.scalings, F.log2T, pos, enc);
-    if (O.stash_encoding) {
+    if (O.stash_encoding && valid) {
       float4* st = reinterpret_cast<float4*>(O.stash_encoding + (size_t)p * C::ENC);
 #pragma unroll
       for (int i = 0; i < C::ENC / 4; ++i) st[i] = make_float4(enc[4 * i], enc[4 * i + 1], enc[4 * i + 2], enc[4 * i + 3]);
@@ -229,7 +256,8 @@ __global__ void __launch_bounds__(kThreads) simt_field_forward_kernel(KField F, 
 #pragma unroll
     for (int i = 0; i < C::APP; ++i) appv[i] = (F.appearance_mode == FNR_APP_PER_CAMERA) ? __ldg(app + i) : app[i];
     Acts<C> a;
-    field_mlps<C>(P, enc, d, appv, a);
+    field_mlps<C, Lin>(P, enc, d, appv, a);
+    if (!valid) continue;
     const float density = sel ? expf(a.out[0]) : 0.f;
     if (O.sample_density) O.sample_density[p] = density;
     if (O.sample_semantics) O.sample_semantics[p] = a.logit;
@@ -509,7 +537,49 @@ __device__ __forceinline__ void tile_weight_grad(float* __restrict__ sX, float* 
   }
 }
 
+// How the backward evaluates a layer: recompute, input gradient dx = W^T dy and weight gradient dW = dY^T X per tile, either
+// in fp32 on the CUDA cores (the exact device reference) or block-wide on the tensor cores (fnr_wgmma.cuh).  The 1- and
+// 3-wide output heads stay in fp32 on both.
+struct SimtBackward {
+  using Lin = SimtLinear;
+  static constexpr int kSmemBytes(int maxw) { return 2 * kThreads * (((maxw + 3) & ~3) + 4) * 4; }
+  template <int K, int N>
+  static __device__ __forceinline__ void dx(const float* __restrict__ W, const float (&dy)[N], float (&dxv)[K]) {
+    linear_bwd_input<K, N>(W, dy, dxv);
+  }
+  template <int K, int N>
+  static __device__ __forceinline__ void dw(float* sX, float* sY, const float (&x)[K], const float (&dy)[N], float* gW, float* gb) {
+    tile_weight_grad<K, N>(sX, sY, x, dy, gW, gb);
+  }
+};
 template <class C>
+struct WgmmaBackward {
+  using Lin = WgmmaLinear<C>;
+  static constexpr int cmax(int a, int b) { return a > b ? a : b; }
+  static constexpr int kSmemBytes(int maxw) {
+    return cmax(cmax(WgmmaLinear<C>::kSmemBytes, wg::DwSmem<C::MAXW, C::MAXW>::kBytes), SimtBackward::kSmemBytes(maxw));
+  }
+  template <int K, int N>
+  static __device__ __forceinline__ void dx(const float* __restrict__ W, const float (&dy)[N], float (&dxv)[K]) {
+    if constexpr (N < 8) {
+      linear_bwd_input<K, N>(W, dy, dxv);
+    } else {
+      extern __shared__ __align__(128) uint8_t wg_smem[];
+      wg::linear_dx<C::MAXW, C::MAXW, K, N>(wg_smem, W, dy, dxv);
+    }
+  }
+  template <int K, int N>
+  static __device__ __forceinline__ void dw(float* sX, float* sY, const float (&x)[K], const float (&dy)[N], float* gW, float* gb) {
+    if constexpr (N < 8) {
+      tile_weight_grad<K, N>(sX, sY, x, dy, gW, gb);
+    } else {
+      extern __shared__ __align__(128) uint8_t wg_smem[];
+      wg::weight_grad<K, N>(wg_smem, x, dy, gW, gb);
+    }
+  }
+};
+
+template <class C, class Bw = SimtBackward>
 __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F, KParams P, KParams G, KRays Rr,
                                                                       KFieldBwd B) {
   extern __shared__ __align__(16) float smem[];
@@ -550,7 +620,7 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
     for (int i = 0; i < C::APP; ++i)
       appv[i] = (F.appearance_mode == FNR_APP_PER_CAMERA) ? __ldg(P.app_embedding + (size_t)cam * C::APP + i) : s_app[i];
     Acts<C> a;
-    field_mlps<C>(P, enc, d, appv, a);
+    field_mlps<C, typename Bw::Lin>(P, enc, d, appv, a);
 
     // upstream per-point grads (zero for padding threads)
     const float* pg = B.point_grads + 5 * (size_t)pc;
@@ -567,30 +637,30 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
     {
       float dlg[1] = {d_logit};
       float dzo[C::SEM_OUT];
-      linear_bwd_input<C::SEM_OUT, 1>(P.head_w, dlg, dzo);
-      tile_weight_grad<C::SEM_OUT, 1>(sX, sY, a.zo, dlg, G.head_w, G.head_b);
+      Bw::template dx<C::SEM_OUT, 1>(P.head_w, dlg, dzo);
+      Bw::template dw<C::SEM_OUT, 1>(sX, sY, a.zo, dlg, G.head_w, G.head_b);
       float geo[C::GEO];
 #pragma unroll
       for (int i = 0; i < C::GEO; ++i) geo[i] = a.out[1 + i];
       float dz1[C::SEM_H];
       if constexpr (C::SEM_LAYERS == 3) {
         float dz2[C::SEM_H];
-        linear_bwd_input<C::SEM_H, C::SEM_OUT>(P.sem_w[2], dzo, dz2);
-        tile_weight_grad<C::SEM_H, C::SEM_OUT>(sX, sY, a.z2, dzo, G.sem_w[2], G.sem_b[2]);
+        Bw::template dx<C::SEM_H, C::SEM_OUT>(P.sem_w[2], dzo, dz2);
+        Bw::template dw<C::SEM_H, C::SEM_OUT>(sX, sY, a.z2, dzo, G.sem_w[2], G.sem_b[2]);
 #pragma unroll
         for (int i = 0; i < C::SEM_H; ++i) dz2[i] = a.z2[i] > 0.f ? dz2[i] : 0.f;
-        linear_bwd_input<C::SEM_H, C::SEM_H>(P.sem_w[1], dz2, dz1);
-        tile_weight_grad<C::SEM_H, C::SEM_H>(sX, sY, a.z1, dz2, G.sem_w[1], G.sem_b[1]);
+        Bw::template dx<C::SEM_H, C::SEM_H>(P.sem_w[1], dz2, dz1);
+        Bw::template dw<C::SEM_H, C::SEM_H>(sX, sY, a.z1, dz2, G.sem_w[1], G.sem_b[1]);
       } else {
-        linear_bwd_input<C::SEM_H, C::SEM_OUT>(P.sem_w[1], dzo, dz1);
-        tile_weight_grad<C::SEM_H, C::SEM_OUT>(sX, sY, a.z1, dzo, G.sem_w[1], G.sem_b[1]);
+        Bw::template dx<C::SEM_H, C::SEM_OUT>(P.sem_w[1], dzo, dz1);
+        Bw::template dw<C::SEM_H, C::SEM_OUT>(sX, sY, a.z1, dzo, G.sem_w[1], G.sem_b[1]);
       }
 #pragma unroll
       for (int i = 0; i < C::SEM_H; ++i) dz1[i] = a.z1[i] > 0.f ? dz1[i] : 0.f;
-      tile_weight_grad<C::GEO, C::SEM_H>(sX, sY, geo, dz1, G.sem_w[0], G.sem_b[0]);
+      Bw::template dw<C::GEO, C::SEM_H>(sX, sY, geo, dz1, G.sem_w[0], G.sem_b[0]);
       if (F.pass_semantic_gradients) {
         float dg[C::GEO];
-        linear_bwd_input<C::GEO, C::SEM_H>(P.sem_w[0], dz1, dg);
+        Bw::template dx<C::GEO, C::SEM_H>(P.sem_w[0], dz1, dg);
 #pragma unroll
         for (int i = 0; i < C::GEO; ++i) d_geo[i] += dg[i];
       }
@@ -601,16 +671,16 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
 #pragma unroll
       for (int i = 0; i < 3; ++i) do3[i] = d_rgb[i] * a.rgb[i] * (1.0f - a.rgb[i]);
       float dc2[C::COL_H], dc1[C::COL_H], dcin[C::COL_IN];
-      linear_bwd_input<C::COL_H, 3>(P.col_w[2], do3, dc2);
-      tile_weight_grad<C::COL_H, 3>(sX, sY, a.c2, do3, G.col_w[2], G.col_b[2]);
+      Bw::template dx<C::COL_H, 3>(P.col_w[2], do3, dc2);
+      Bw::template dw<C::COL_H, 3>(sX, sY, a.c2, do3, G.col_w[2], G.col_b[2]);
 #pragma unroll
       for (int i = 0; i < C::COL_H; ++i) dc2[i] = a.c2[i] > 0.f ? dc2[i] : 0.f;
-      linear_bwd_input<C::COL_H, C::COL_H>(P.col_w[1], dc2, dc1);
-      tile_weight_grad<C::COL_H, C::COL_H>(sX, sY, a.c1, dc2, G.col_w[1], G.col_b[1]);
+      Bw::template dx<C::COL_H, C::COL_H>(P.col_w[1], dc2, dc1);
+      Bw::template dw<C::COL_H, C::COL_H>(sX, sY, a.c1, dc2, G.col_w[1], G.col_b[1]);
 #pragma unroll
       for (int i = 0; i < C::COL_H; ++i) dc1[i] = a.c1[i] > 0.f ? dc1[i] : 0.f;
-      linear_bwd_input<C::COL_IN, C::COL_H>(P.col_w[0], dc1, dcin);
-      tile_weight_grad<C::COL_IN, C::COL_H>(sX, sY, a.cin, dc1, G.col_w[0], G.col_b[0]);
+      Bw::template dx<C::COL_IN, C::COL_H>(P.col_w[0], dc1, dcin);
+      Bw::template dw<C::COL_IN, C::COL_H>(sX, sY, a.cin, dc1, G.col_w[0], G.col_b[0]);
 #pragma unroll
       for (int i = 0; i < C::GEO; ++i) d_geo[i] += dcin[C::SH + i];
       // appearance-embedding gradient (only the per-camera rows are parameters of the graph;
@@ -646,12 +716,12 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
 #pragma unroll
       for (int i = 0; i < C::GEO; ++i) dout[1 + i] = d_geo[i];
       float dh1[C::BASE_H];
-      linear_bwd_input<C::BASE_H, C::BASE_OUT>(P.base_w[1], dout, dh1);
-      tile_weight_grad<C::BASE_H, C::BASE_OUT>(sX, sY, a.h1, dout, G.base_w[1], G.base_b[1]);
+      Bw::template dx<C::BASE_H, C::BASE_OUT>(P.base_w[1], dout, dh1);
+      Bw::template dw<C::BASE_H, C::BASE_OUT>(sX, sY, a.h1, dout, G.base_w[1], G.base_b[1]);
 #pragma unroll
       for (int i = 0; i < C::BASE_H; ++i) dh1[i] = a.h1[i] > 0.f ? dh1[i] : 0.f;
-      linear_bwd_input<C::ENC, C::BASE_H>(P.base_w[0], dh1, denc);
-      tile_weight_grad<C::ENC, C::BASE_H>(sX, sY, enc, dh1, G.base_w[0], G.base_b[0]);
+      Bw::template dx<C::ENC, C::BASE_H>(P.base_w[0], dh1, denc);
+      Bw::template dw<C::ENC, C::BASE_H>(sX, sY, enc, dh1, G.base_w[0], G.base_b[0]);
     }
     // ---- hash-table scatter -----------------------------------------------------------------
     if (valid) {
@@ -689,14 +759,15 @@ __device__ __forceinline__ int warp_claim(int* counter, bool pred, int lane, int
   return basev;
 }
 
-template <class C>
+template <class C, class Lin = SimtLinear>
 __global__ void __launch_bounds__(kThreads) simt_export_kernel(KField F, KParams P, KExport E) {
   __shared__ float s_app[C::APP];
   block_mean_embedding(P, F.num_images, C::APP, FNR_APP_MEAN, s_app);
   const int lane = threadIdx.x & 31;
   const long long N = (long long)E.B * E.S;
-  const long long Npad = (N + 31) / 32 * 32;
-  for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < Npad; p += (long long)gridDim.x * blockDim.x) {
+  // whole 128-point tiles per CTA (see simt_field_forward_kernel): warp-converged row claims, block-wide MLP layers
+  for (long long p0 = (long long)blockIdx.x * blockDim.x; p0 < N; p0 += (long long)gridDim.x * blockDim.x) {
+    const long long p = p0 + threadIdx.x;
     const bool valid = p < N;
     const long long pc = valid ? p : N - 1;
     const int r = (int)(pc / E.S), s = (int)(pc % E.S);
@@ -716,7 +787,7 @@ __global__ void __launch_bounds__(kThreads) simt_export_kernel(KField F, KParams
 #pragma unroll
     for (int i = 0; i < C::APP; ++i) appv[i] = s_app[i];
     Acts<C> a;
-    field_mlps<C>(P, enc, E.normal, appv, a);
+    field_mlps<C, Lin>(P, enc, E.normal, appv, a);
     const float density = sel ? expf(a.out[0]) : 0.f;
     const float sg = sigmoidf_(a.logit);
     // heaviside(sigmoid(logit) - thr, 0): 1 iff sigmoid - thr > 0
@@ -803,7 +874,7 @@ int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;  // H100 SXM
   }
   return n;
 }
@@ -834,27 +905,33 @@ int launch_simt_composite_backward(const KRays& Rr, const KCompositeBwd& B, cuda
   return check_launch("simt_composite_backward_kernel");
 }
 
-template <class C>
-static int launch_bwd(const KField& F, const KParams& P, const KParams& G, const KRays& Rr, const KFieldBwd& B,
-                      cudaStream_t st) {
-  constexpr int TP = ((C::MAXW + 3) & ~3) + 4;
-  const size_t smem = 2 * (size_t)kThreads * TP * sizeof(float);
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(simt_field_backward_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute(simt_field_backward_kernel)");
-    configured = true;
-  }
+template <class C, class Bw>
+static int launch_bwd(const KField& F, const KParams& P, const KParams& G, const KRays& Rr, const KFieldBwd& B, cudaStream_t st) {
+  constexpr int smem = Bw::kSmemBytes(C::MAXW);
+  auto kernel = simt_field_backward_kernel<C, Bw>;
+  // per device: set on every call (cheap), so that a process driving several GPUs opts in on each of them
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute(simt_field_backward_kernel)");
+  int per_sm = 0;
+  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, smem);
+  if (e != cudaSuccess) return check_cuda(e, "cudaOccupancyMaxActiveBlocksPerMultiprocessor");
   const long long N = (long long)Rr.R * Rr.S;
-  const int grid = grid_for(N, kThreads, sm_count() * 2);
-  simt_field_backward_kernel<C><<<grid, kThreads, smem, st>>>(F, P, G, Rr, B);
+  const int grid = grid_for(N, kThreads, sm_count() * (per_sm > 0 ? per_sm : 1));
+  kernel<<<grid, kThreads, smem, st>>>(F, P, G, Rr, B);
   return check_launch("simt_field_backward_kernel");
 }
 
 int launch_simt_field_backward(Family fam, const KField& F, const KParams& P, const KParams& G, const KRays& Rr,
                                const KFieldBwd& B, cudaStream_t st) {
   if ((long long)Rr.R * Rr.S == 0) return FNR_OK;
-  return fam == kFamilySmall ? launch_bwd<CfgSmall>(F, P, G, Rr, B, st) : launch_bwd<CfgBig>(F, P, G, Rr, B, st);
+  return fam == kFamilySmall ? launch_bwd<CfgSmall, SimtBackward>(F, P, G, Rr, B, st) : launch_bwd<CfgBig, SimtBackward>(F, P, G, Rr, B, st);
+}
+
+int launch_wgmma_field_backward(Family fam, const KField& F, const KParams& P, const KParams& G, const KRays& Rr, const KFieldBwd& B,
+                                cudaStream_t st) {
+  if ((long long)Rr.R * Rr.S == 0) return FNR_OK;
+  return fam == kFamilySmall ? launch_bwd<CfgSmall, WgmmaBackward<CfgSmall>>(F, P, G, Rr, B, st)
+                             : launch_bwd<CfgBig, WgmmaBackward<CfgBig>>(F, P, G, Rr, B, st);
 }
 
 int launch_simt_export(Family fam, const KField& F, const KParams& P, const KExport& E, cudaStream_t st) {
@@ -866,6 +943,48 @@ int launch_simt_export(Family fam, const KField& F, const KParams& P, const KExp
   else
     simt_export_kernel<CfgBig><<<grid, kThreads, 0, st>>>(F, P, E);
   return check_launch("simt_export_kernel");
+}
+
+// Tensor-core (wgmma) instantiations of the forward and export kernels: one 128-thread CTA (one warpgroup) per SM slot
+// the shared-memory plan of WgmmaLinear allows.
+template <class K, class C>
+static int wgmma_grid(K kernel, long long N, int& grid) {
+  // per device: set on every call (cheap), so that a process driving several GPUs opts in on each of them
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WgmmaLinear<C>::kSmemBytes);
+  if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute(wgmma field kernel)");
+  int per_sm = 0;
+  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, WgmmaLinear<C>::kSmemBytes);
+  if (e != cudaSuccess) return check_cuda(e, "cudaOccupancyMaxActiveBlocksPerMultiprocessor");
+  grid = grid_for(N, kThreads, sm_count() * (per_sm > 0 ? per_sm : 1));
+  return FNR_OK;
+}
+
+template <class C>
+static int launch_wgmma_forward_c(const KField& F, const KParams& P, const KRays& Rr, const KFieldOut& O, cudaStream_t st) {
+  auto kernel = simt_field_forward_kernel<C, WgmmaLinear<C>>;
+  int grid = 0, rc = wgmma_grid<decltype(kernel), C>(kernel, (long long)Rr.R * Rr.S, grid);
+  if (rc) return rc;
+  kernel<<<grid, kThreads, WgmmaLinear<C>::kSmemBytes, st>>>(F, P, Rr, O);
+  return check_launch("simt_field_forward_kernel<wgmma>");
+}
+
+int launch_wgmma_field_forward(Family fam, const KField& F, const KParams& P, const KRays& Rr, const KFieldOut& O, cudaStream_t st) {
+  if ((long long)Rr.R * Rr.S == 0) return FNR_OK;
+  return fam == kFamilySmall ? launch_wgmma_forward_c<CfgSmall>(F, P, Rr, O, st) : launch_wgmma_forward_c<CfgBig>(F, P, Rr, O, st);
+}
+
+template <class C>
+static int launch_wgmma_export_c(const KField& F, const KParams& P, const KExport& E, cudaStream_t st) {
+  auto kernel = simt_export_kernel<C, WgmmaLinear<C>>;
+  int grid = 0, rc = wgmma_grid<decltype(kernel), C>(kernel, (long long)E.B * E.S, grid);
+  if (rc) return rc;
+  kernel<<<grid, kThreads, WgmmaLinear<C>::kSmemBytes, st>>>(F, P, E);
+  return check_launch("simt_export_kernel<wgmma>");
+}
+
+int launch_wgmma_export(Family fam, const KField& F, const KParams& P, const KExport& E, cudaStream_t st) {
+  if ((long long)E.B * E.S == 0) return FNR_OK;
+  return fam == kFamilySmall ? launch_wgmma_export_c<CfgSmall>(F, P, E, st) : launch_wgmma_export_c<CfgBig>(F, P, E, st);
 }
 
 int launch_hash_indices(const KField& F, const KRays& Rr, int32_t* rows, float* positions, cudaStream_t st) {

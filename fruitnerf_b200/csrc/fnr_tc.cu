@@ -1,47 +1,42 @@
-// Dispatch of the tensor-core render / export forward (fnr_render_forward, fnr_export_forward with impl = tcgen05 / auto):
-//   fruit_nerf family (geo 15, semantic 15-64-64, colour 63-64-64-3)           -> fnr_tc_ws.cu  (warp-specialised: cp.async gather
-//                                                                                 warps, TMEM-resident MLP chains, per-group compositing)
-//   fruit_nerf_big / _huge (geo 30, semantic 30-128-128-64, colour 78-64-64-3)  -> fnr_tc_big.cu
-// everything else is served by the simt kernels (tc_supported() == false).
-// (The round-1 kernel of this file -- gather and MLP chain in the same 16 warps, activations in shared memory -- was replaced by
-// fnr_tc_ws.cu in round 2: 0.529 -> 0.284 ms on the 4096 x 192 bench batch.)
+// Dispatch of impl = tcgen05 (the tensor-core implementation) on sm_90a.
+//
+// The field MLPs of render / export forward and of the field backward run on the Hopper tensor cores: fnr_simt.cu's
+// kernels instantiated with WgmmaLinear / WgmmaBackward (fnr_wgmma.cuh: bf16 hi/lo split operands, wgmma, fp32
+// accumulation; the backward's dx = W^T dy and per-tile dW = dY^T X as well), followed by the compositing kernel for
+// render calls.  impl = auto takes them for both shipped families.  The name is the historical one: the fused Blackwell
+// (tcgen05 / tensor memory) kernels this impl first selected are kept as a design record under design/blackwell/ and are
+// not part of the library.
 #include "fnr_common.cuh"
 #include "fnr_kernels.h"
 
 namespace fnr {
 
-bool tc_supported(Family fam, const KField& F, const KRays& Rr) {
-  (void)F;
-  if (fam == kFamilyBig) return tc_big_supported(Rr.S);
-  return fam == kFamilySmall && tc_ws_supported(Rr.S);
-}
+// auto takes the tensor-core kernels for both shipped families (4096x192 bench batch on an H100: render forward 1.4 ms
+// against 3.7 ms on the simt kernels for fruit_nerf, 5.5 against 8.4 ms for fruit_nerf_big)
+static bool shipped(Family fam) { return fam == kFamilySmall || fam == kFamilyBig; }
+bool tc_supported(Family fam, const KField&, const KRays&) { return shipped(fam); }
+bool tc_export_supported(Family fam, const KExport&) { return shipped(fam); }
+bool tc_backward_supported(Family fam, const KField&, const KRays&, const KFieldBwd&) { return shipped(fam); }
 
-bool tc_export_supported(Family fam, const KExport& E) {
-  if (fam == kFamilyBig) return tc_big_supported(E.S);
-  return fam == kFamilySmall && tc_ws_supported(E.S);
-}
-
-int launch_tc_render_forward(Family fam, const KField& F, const KParams& P, const KRays& Rr, const KFieldOut& O,
-                             const KComposite& Cm, cudaStream_t st) {
-  if (!tc_supported(fam, F, Rr)) {
-    set_error("tcgen05 render kernel does not support this shape");
-    return FNR_ERR_UNSUPPORTED;
+int launch_tc_render_forward(Family fam, const KField& F, const KParams& P, const KRays& Rr, const KFieldOut& O, const KComposite& Cm,
+                             cudaStream_t st) {
+  const bool composite = Cm.rgb || Cm.accumulation || Cm.depth || Cm.depth_index || Cm.semantics || Cm.weights;
+  if (composite && !(O.sample_density && O.sample_rgb && O.sample_semantics)) {
+    set_error("tensor-core render: sample_density/sample_rgb/sample_semantics buffers are required when ray outputs are requested");
+    return FNR_ERR_INVALID_ARGUMENT;
   }
-  if (Rr.R == 0) return FNR_OK;
-  if (fam == kFamilyBig) return launch_tc_render_forward_big(F, P, Rr, O, Cm, st);
-  return launch_tc_render_forward_ws(F, P, Rr, O, Cm, st);
+  int rc = launch_wgmma_field_forward(fam, F, P, Rr, O, st);
+  if (rc || !composite) return rc;
+  return launch_simt_composite(Rr, Cm, st);
 }
 
-// The export path reuses the fused forward (AABB positions, mean appearance embedding) and replaces the
-// compositing stage by the three threshold selections + stream compaction.
 int launch_tc_export(Family fam, const KField& F, const KParams& P, const KExport& E, cudaStream_t st) {
-  if (!tc_export_supported(fam, E)) {
-    set_error("tcgen05 export kernel does not support this shape");
-    return FNR_ERR_UNSUPPORTED;
-  }
-  if (E.B == 0) return FNR_OK;
-  if (fam == kFamilyBig) return launch_tc_export_big(F, P, E, st);
-  return launch_tc_export_ws(F, P, E, st);
+  return launch_wgmma_export(fam, F, P, E, st);
+}
+
+int launch_tc_field_backward(Family fam, const KField& F, const KParams& P, const KParams& G, const KRays& Rr, const KFieldBwd& B,
+                             cudaStream_t st) {
+  return launch_wgmma_field_backward(fam, F, P, G, Rr, B, st);
 }
 
 }  // namespace fnr

@@ -1,9 +1,9 @@
 """CUDA-graph execution of the training hot step.
 
-One FruitNeRF training iteration on the hot path is a handful of kernels that together run for ~1-2 ms
-on a B200; enqueueing them op by op from Python costs more than executing them.  ``GraphedTrainStep``
+One FruitNeRF training iteration on the hot path is a handful of kernels that together run for a few
+milliseconds; enqueueing them op by op from Python costs a large share of that.  ``GraphedTrainStep``
 captures the body of ``FruitPipeline.get_train_loss_dict`` + ``backward`` for a fixed batch shape --
-fused render forward, MSE / BCE-with-logits loss (fruit_nerf/fruit_nerf.py:359-366), tensor-core
+fused render forward, MSE / BCE-with-logits loss (fruit_nerf/fruit_nerf.py:359-366), field
 backward into the flat gradient buffer -- into ONE CUDA graph and replays it per step.  Inputs live in
 static device buffers that ``load_batch`` refreshes (asynchronous H2D copies from pinned memory).
 """

@@ -1,5 +1,5 @@
 """FruitField -- the reference's field (fruit_nerf/fruit_field.py:43-301) as a parameter holder
-whose forward runs in the native sm_100a kernels.
+whose forward runs in the native sm_90a kernels.
 
 Constructor signature, attribute names and state-dict keys follow the reference under
 nerfstudio's torch path, so ``load_state_dict(strict=True)`` round-trips

@@ -1,6 +1,6 @@
 """FruitPipeline -- drop-in surface of fruit_nerf.fruit_pipeline.FruitPipeline (66-260).
 
-Differences that matter on B200: instead of wrapping the model in DDP (fruit_pipeline.py:117, NCCL
+Differences that matter on the GPU: instead of wrapping the model in DDP (fruit_pipeline.py:117, NCCL
 all-reduce of every parameter's .grad in 25 MiB buckets) the backward kernels accumulate into ONE
 flat fp32 gradient buffer (ops.flat_zero_grads) and ``sync_gradients`` all-reduces that buffer in a
 single NCCL collective over NVLink/NVSwitch (mean over ranks, the DDP semantics).

@@ -85,7 +85,7 @@ def _require_cuda(*ts: Optional[Tensor]) -> torch.device:
             continue
         if not t.is_cuda:
             raise L.FruitNerfNativeError(
-                "fruitnerf_b200 ops need CUDA tensors: the hot path is hand-written sm_100a CUDA with no CPU fallback"
+                "fruitnerf_b200 ops need CUDA tensors: the hot path is hand-written sm_90a CUDA with no CPU fallback"
             )
         dev = t.device
     return dev

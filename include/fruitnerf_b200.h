@@ -1,7 +1,7 @@
 /*
- * fruitnerf_b200 -- C ABI of the B200-native FruitNeRF hot path.
+ * fruitnerf_b200 -- C ABI of the H100-native FruitNeRF hot path.
  *
- * One shared library (libfruitnerf_b200.so, sm_100a) behind the reference's Nerfstudio plugin
+ * One shared library (libfruitnerf_b200.so, sm_90a) behind the reference's Nerfstudio plugin
  * surface.  Plain C: no C++ or torch types cross this boundary.  Every buffer is a raw DEVICE
  * pointer allocated and owned by the caller (PyTorch on the Python side); the library keeps no
  * global state besides a thread-local error string and, once the fruit_nerf_big backward has run, a cuBLAS
@@ -67,10 +67,10 @@ extern "C" {
 #define FNR_APP_MEAN 1       /* embedding.mean(0)        (inference/export, or use_average...) */
 #define FNR_APP_ZEROS 2      /* zeros                    (eval without average embedding) */
 
-/* implementation selector for the forward kernels */
-#define FNR_IMPL_AUTO 0    /* tcgen05 fused kernel when the shape is supported, else simt */
+/* implementation selector for the forward, export and backward kernels */
+#define FNR_IMPL_AUTO 0    /* tensor-core kernels for the shipped network shapes, else simt */
 #define FNR_IMPL_SIMT 1    /* fp32 CUDA-core kernels (exact-fp32 device reference) */
-#define FNR_IMPL_TCGEN05 2 /* fused tcgen05/TMEM kernel; FNR_ERR_UNSUPPORTED if shape unsupported */
+#define FNR_IMPL_TCGEN05 2 /* tensor-core kernels (wgmma on sm_90a; historical name); FNR_ERR_UNSUPPORTED if shape unsupported */
 
 /* One nn.Linear stack: n_layers Linear layers, ReLU between them (nerfstudio MLP torch path);
  * dims[0] = input width, dims[n_layers] = output width. */

@@ -212,7 +212,7 @@ def _safe_ray_weights(f, R):
     return ok
 
 
-@pytest.mark.parametrize("impl", [L.FNR_IMPL_SIMT, L.FNR_IMPL_AUTO], ids=["simt", "auto"])
+@pytest.mark.parametrize("impl", [L.FNR_IMPL_SIMT, L.FNR_IMPL_TCGEN05, L.FNR_IMPL_AUTO], ids=["simt", "tcgen05", "auto"])
 @pytest.mark.parametrize("name,R,S", [("small", 128, 48), ("big", 128, 48), ("small", 111, 50), ("big", 77, 37)])
 def test_backward_matches_oracle_autograd(native_lib, cuda_device, name, R, S, impl):
     """auto = fused tcgen05 forward + tensor-core backward where the shape is covered (small family),
@@ -250,7 +250,7 @@ def test_backward_matches_oracle_autograd(native_lib, cuda_device, name, R, S, i
         assert_rel(g, g_ref, rel=2e-3, floor=0.25, what=f"grad {key}")
 
 
-@pytest.mark.parametrize("impl", [L.FNR_IMPL_SIMT, L.FNR_IMPL_AUTO], ids=["simt", "auto"])
+@pytest.mark.parametrize("impl", [L.FNR_IMPL_SIMT, L.FNR_IMPL_TCGEN05, L.FNR_IMPL_AUTO], ids=["simt", "tcgen05", "auto"])
 def test_field_only_backward(native_lib, cuda_device, impl):
     """FruitField.forward users: gradients w.r.t. per-sample outputs flow to the parameters."""
     sd, spec = make_state("small", log2T=15)
