@@ -1,7 +1,7 @@
 """In-tree build of libfruitnerf_b200.so (sm_90a, H100) with nvcc.  Used by __graft_entry__.build().
 
 The tensor-core path (impl = tcgen05 / auto) is the wgmma instantiation of the kernels in fnr_simt.cu (fnr_wgmma.cuh,
-dispatch in fnr_tc.cu).  The fused Blackwell kernels are kept outside the library under design/blackwell/."""
+dispatch in fnr_api.cu).  The fused Blackwell kernels are kept outside the library under design/blackwell/."""
 from __future__ import annotations
 
 import os
@@ -12,7 +12,7 @@ from pathlib import Path
 CSRC = Path(__file__).resolve().parent / "csrc"
 LIB = CSRC / "libfruitnerf_b200.so"
 STAMP = CSRC / "libfruitnerf_b200.recipe"  # flags and sources LIB was built from
-SOURCES = ["fnr_api.cu", "fnr_simt.cu", "fnr_tc.cu", "fnr_proposal.cu", "fnr_optim.cu", "fnr_glue.cu", "fnr_nvls.cu"]
+SOURCES = ["fnr_api.cu", "fnr_simt.cu", "fnr_proposal.cu", "fnr_optim.cu", "fnr_glue.cu", "fnr_nvls.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr",

@@ -209,15 +209,12 @@ def load() -> C.CDLL:
     global _lib
     if _lib is not None:
         return _lib
-    import os
-
-    path = Path(os.environ.get("FNR_LIB") or LIB_PATH)  # FNR_LIB: load an experimental build of the same ABI (tools/ only)
-    if not path.exists():
+    if not LIB_PATH.exists():
         raise FruitNerfNativeError(
-            f"{path} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
+            f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
             "(nvcc, sm_90a).  fruitnerf_b200 has no CPU / PyTorch fallback."
         )
-    lib = C.CDLL(str(path))
+    lib = C.CDLL(str(LIB_PATH))
     lib.fnr_version.restype = C.c_int
     lib.fnr_nvls_allreduce_mean.restype = C.c_int
     lib.fnr_nvls_allreduce_mean.argtypes = [C.POINTER(NvlsDesc), C.c_size_t, C.c_int32, C.c_void_p]

@@ -1,6 +1,6 @@
 // extern "C" entry points of libfruitnerf_b200.so: argument validation, conversion of the plain-C
 // structs of include/fruitnerf_b200.h into kernel arguments, dispatch between the tensor-core
-// (wgmma) and the fp32 simt instantiations of the kernels (fnr_tc.cu).  No host synchronisation, no allocation.
+// (wgmma) and the fp32 simt instantiations of the field kernels.  No host synchronisation, no allocation.
 #include <atomic>
 #include <cstdarg>
 #include <cstdio>
@@ -77,6 +77,11 @@ int validate_desc(const fnr_field_desc* d) {
   }
   if (d->num_images < 1) {
     set_error("num_images must be >= 1");
+    return FNR_ERR_INVALID_ARGUMENT;
+  }
+  // AUTO runs the tensor-core kernels like TCGEN05 (tc = impl != SIMT): every shape that passes validation is a shipped family
+  if (d->impl != FNR_IMPL_AUTO && d->impl != FNR_IMPL_SIMT && d->impl != FNR_IMPL_TCGEN05) {
+    set_error("invalid impl %d", d->impl);
     return FNR_ERR_INVALID_ARGUMENT;
   }
   if (classify(d) == kFamilyNone) {
@@ -194,29 +199,19 @@ int fnr_render_forward(const fnr_field_desc* desc, const fnr_field_params* param
     set_error("stash_encoding must be 32-byte aligned (written with 256-bit stores)");
     return FNR_ERR_INVALID_ARGUMENT;
   }
-  const Family fam = classify(desc);
-  const KField F = make_field(desc);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const bool composite = out->rgb || out->accumulation || out->depth || out->depth_index || out->semantics || out->weights;
-
+  if (composite && !(out->sample_density && out->sample_rgb && out->sample_semantics)) {
+    set_error("render: sample_density/sample_rgb/sample_semantics buffers are required when ray outputs are requested");
+    return FNR_ERR_INVALID_ARGUMENT;
+  }
+  const bool tc = desc->impl != FNR_IMPL_SIMT;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   KFieldOut O{out->sample_density, out->sample_rgb, out->sample_semantics, out->stash_encoding};
+  if ((rc = launch_field_forward(classify(desc), tc, make_field(desc), P, Rr, O, st))) return rc;
+  if (!composite) return FNR_OK;
   KComposite Cm{out->sample_density, out->sample_rgb, out->sample_semantics, out->rgb, out->accumulation, out->depth,
                 out->depth_index, out->semantics, out->weights, out->clamp_rgb};
-
-  int impl = desc->impl;
-  if (impl == FNR_IMPL_AUTO) impl = tc_supported(fam, F, Rr) ? FNR_IMPL_TCGEN05 : FNR_IMPL_SIMT;
-  if (impl == FNR_IMPL_TCGEN05) return launch_tc_render_forward(fam, F, P, Rr, O, Cm, st);
-  if (impl != FNR_IMPL_SIMT) {
-    set_error("invalid impl %d", impl);
-    return FNR_ERR_INVALID_ARGUMENT;
-  }
-  if (composite && !(out->sample_density && out->sample_rgb && out->sample_semantics)) {
-    set_error("simt render: sample_density/sample_rgb/sample_semantics buffers are required when ray outputs are requested");
-    return FNR_ERR_INVALID_ARGUMENT;
-  }
-  if ((rc = launch_simt_field_forward(fam, F, P, Rr, O, st))) return rc;
-  if (composite) return launch_simt_composite(Rr, Cm, st);
-  return FNR_OK;
+  return launch_simt_composite(Rr, Cm, st);
 }
 
 int fnr_render_backward_scratch_bytes(const fnr_field_desc* desc, int32_t num_rays, int32_t num_samples, size_t* bytes) {
@@ -275,15 +270,9 @@ int fnr_render_backward(const fnr_field_desc* desc, const fnr_field_params* para
                   point_grads,
                   desc->pass_semantic_gradients};
   if ((rc = launch_simt_composite_backward(Rr, B, st))) return rc;
-  const size_t pg_bytes = ((size_t)Rr.R * Rr.S * 5 * sizeof(float) + 255) & ~(size_t)255;
-  uint8_t* extra = reinterpret_cast<uint8_t*>(point_grads) + pg_bytes;
-  const size_t used = (size_t)(extra - reinterpret_cast<uint8_t*>(scratch));
-  KFieldBwd FB{point_grads, saved->stash_encoding, saved->sample_rgb, scratch_bytes > used ? extra : nullptr,
-               scratch_bytes > used ? scratch_bytes - used : 0};
-  int impl = desc->impl;
-  if (impl == FNR_IMPL_AUTO) impl = tc_backward_supported(fam, F, Rr, FB) ? FNR_IMPL_TCGEN05 : FNR_IMPL_SIMT;
-  if (impl == FNR_IMPL_TCGEN05) return launch_tc_field_backward(fam, F, P, G, Rr, FB, st);
-  return launch_simt_field_backward(fam, F, P, G, Rr, FB, st);
+  const bool tc = desc->impl != FNR_IMPL_SIMT;
+  const KFieldBwd FB{point_grads, saved->stash_encoding};
+  return launch_field_backward(fam, tc, F, P, G, Rr, FB, st);
 }
 
 int fnr_export_forward(const fnr_field_desc* desc, const fnr_field_params* params, const float* origins,
@@ -337,15 +326,8 @@ int fnr_export_forward(const fnr_field_desc* desc, const fnr_field_params* param
   E.sample_semantics = out->sample_semantics;
   E.sample_density = out->sample_density;
   E.semantics_colormap = out->semantics_colormap;
-  const Family fam = classify(desc);
-  int impl = desc->impl;
-  if (impl == FNR_IMPL_AUTO) impl = tc_export_supported(fam, E) ? FNR_IMPL_TCGEN05 : FNR_IMPL_SIMT;
-  if (impl == FNR_IMPL_TCGEN05) return launch_tc_export(fam, F, P, E, reinterpret_cast<cudaStream_t>(stream));
-  if (impl != FNR_IMPL_SIMT) {
-    set_error("invalid impl %d", impl);
-    return FNR_ERR_INVALID_ARGUMENT;
-  }
-  return launch_simt_export(fam, F, P, E, reinterpret_cast<cudaStream_t>(stream));
+  const bool tc = desc->impl != FNR_IMPL_SIMT;
+  return launch_export(classify(desc), tc, F, P, E, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int fnr_hash_indices(const fnr_field_desc* desc, const fnr_ray_batch* rays, int32_t* rows, float* positions, void* stream) {

@@ -75,9 +75,6 @@ struct KCompositeBwd {
 struct KFieldBwd {
   const float* point_grads;     // [N,5]
   const float* stash_encoding;  // [N,32] or NULL (recompute)
-  const float* sample_rgb;      // [N,3] forward rgb (tcgen05 backward: sigmoid' without re-running colour2)
-  void* extra;                  // big-family tensor-core backward: scratch for the per-point X / dY matrices
-  size_t extra_bytes;
 };
 
 struct KExport {
@@ -215,28 +212,14 @@ int proposal_limits(int* max_levels, int* hidden, int* max_bins);
 
 int sm_count();
 
-int launch_simt_field_forward(Family fam, const KField& F, const KParams& P, const KRays& Rr, const KFieldOut& O, cudaStream_t st);
+// Field kernels of fnr_simt.cu for a shipped family: tc selects the tensor-core (wgmma, sm_90a) instantiation, otherwise
+// the exact-fp32 simt one.
+int launch_field_forward(Family fam, bool tc, const KField& F, const KParams& P, const KRays& Rr, const KFieldOut& O, cudaStream_t st);
+int launch_field_backward(Family fam, bool tc, const KField& F, const KParams& P, const KParams& G, const KRays& Rr, const KFieldBwd& B,
+                          cudaStream_t st);
+int launch_export(Family fam, bool tc, const KField& F, const KParams& P, const KExport& E, cudaStream_t st);
 int launch_simt_composite(const KRays& Rr, const KComposite& Cm, cudaStream_t st);
 int launch_simt_composite_backward(const KRays& Rr, const KCompositeBwd& B, cudaStream_t st);
-int launch_simt_field_backward(Family fam, const KField& F, const KParams& P, const KParams& G, const KRays& Rr,
-                               const KFieldBwd& B, cudaStream_t st);
-int launch_simt_export(Family fam, const KField& F, const KParams& P, const KExport& E, cudaStream_t st);
 int launch_hash_indices(const KField& F, const KRays& Rr, int32_t* rows, float* positions, cudaStream_t st);
-
-// tensor-core (wgmma, sm_90a) instantiations of the field forward / export kernels (fnr_simt.cu, fnr_wgmma.cuh)
-int launch_wgmma_field_forward(Family fam, const KField& F, const KParams& P, const KRays& Rr, const KFieldOut& O, cudaStream_t st);
-int launch_wgmma_export(Family fam, const KField& F, const KParams& P, const KExport& E, cudaStream_t st);
-int launch_wgmma_field_backward(Family fam, const KField& F, const KParams& P, const KParams& G, const KRays& Rr, const KFieldBwd& B,
-                                cudaStream_t st);
-
-// impl = tcgen05 / auto dispatch (fnr_tc.cu): the wgmma kernels above for the shipped families.
-bool tc_supported(Family fam, const KField& F, const KRays& Rr);
-bool tc_export_supported(Family fam, const KExport& E);
-bool tc_backward_supported(Family fam, const KField& F, const KRays& Rr, const KFieldBwd& B);
-int launch_tc_render_forward(Family fam, const KField& F, const KParams& P, const KRays& Rr, const KFieldOut& O,
-                             const KComposite& Cm, cudaStream_t st);
-int launch_tc_export(Family fam, const KField& F, const KParams& P, const KExport& E, cudaStream_t st);
-int launch_tc_field_backward(Family fam, const KField& F, const KParams& P, const KParams& G, const KRays& Rr, const KFieldBwd& B,
-                             cudaStream_t st);
 
 }  // namespace fnr

@@ -1,12 +1,13 @@
-// fp32 CUDA-core kernels of the FruitNeRF hot path ("simt" implementation).
+// Kernels of the FruitNeRF hot path: one thread per sample point, per-ray compositing by one warp per ray.
 //
-// These are the exact-fp32 device path: one thread per sample point, MLP weights read straight
-// from the torch parameter tensors through the read-only path (warp-uniform addresses, float4
-// where the row alignment allows), per-ray compositing by one warp per ray.  They serve (a) every
-// shape / mode the fused tcgen05 kernel does not cover, (b) the backward pass, (c) the on-device
-// fp32 reference the tcgen05 kernel is checked against at full size.
+// The field kernels (forward, export, backward) are instantiated twice through Layers<C, TC>.  TC = false is the "simt"
+// implementation, the exact-fp32 device path: MLP weights read straight from the torch parameter tensors through the
+// read-only path (warp-uniform addresses, float4 where the row alignment allows); it is the on-device fp32 reference
+// the tensor-core path is checked against at full size.  TC = true runs the MLP layers block-wide on the Hopper tensor
+// cores (fnr_wgmma.cuh).
 //
 // Reference semantics: fruit_nerf/fruit_field.py:168-301, fruit_nerf/fruit_nerf.py:251-269,316-357.
+#include <type_traits>
 #include "fnr_common.cuh"
 #include "fnr_kernels.h"
 #include "fnr_wgmma.cuh"
@@ -140,27 +141,53 @@ __device__ __forceinline__ void hash_encode(const float2* __restrict__ table, co
 }
 
 // ------------------------------------------------------------------------------------------
-// Field evaluation of one point.  Keeps the activations the backward needs when KEEP.
+// Field evaluation of one point.
 // ------------------------------------------------------------------------------------------
-// How field_mlps evaluates a Linear layer: per thread in fp32 on the CUDA cores (the exact device reference), or
-// block-wide on the tensor cores (fnr_wgmma.cuh; every thread of the 128-thread CTA must take part).
-struct SimtLinear {
-  template <int K, int N, bool RELU>
-  static __device__ __forceinline__ void fwd(const float* __restrict__ W, const float* __restrict__ b, const float (&x)[K], float (&y)[N]) {
-    linear_fwd<K, N, RELU>(W, b, x, y);
+// fp32 weight gradient of one layer over the CTA's 128-point tile (K4 below)
+template <int K, int N>
+__device__ __forceinline__ void tile_weight_grad(float* __restrict__ sX, float* __restrict__ sY, const float (&x)[K],
+                                                 const float (&dy)[N], float* __restrict__ gW, float* __restrict__ gb);
+
+constexpr int cmax(int a, int b) { return a > b ? a : b; }
+
+// How the field kernels evaluate a Linear layer W [N][K]: forward y = act(W x + b), input gradient dx = W^T dy and
+// weight gradient dW = dY^T X over the CTA's tile.  TC = false: per thread in fp32 on the CUDA cores (the exact device
+// reference).  TC = true: block-wide on the tensor cores (fnr_wgmma.cuh; every thread of the 128-thread CTA must take part).
+template <class C, bool TC>
+struct Layers {
+  // the 1- and 3-wide output heads (64 MACs per point) stay in exact fp32 on the CUDA cores on both paths
+  static constexpr bool tensor(int n) { return TC && n >= 8; }
+  // dynamic shared memory: the sX / sY tiles of tile_weight_grad, and the wgmma operand plans (the backward's heads
+  // still use tile_weight_grad, so its tensor-core plan holds that tile too)
+  static constexpr int kTileBytes = 2 * kThreads * (((C::MAXW + 3) & ~3) + 4) * 4;
+  static constexpr int kFwdSmemBytes = TC ? wg::Smem<C::MAXW, C::MAXW>::kBytes : 0;
+  static constexpr int kBwdSmemBytes =
+      TC ? cmax(cmax(wg::Smem<C::MAXW, C::MAXW>::kBytes, wg::DwSmem<C::MAXW, C::MAXW>::kBytes), kTileBytes) : kTileBytes;
+
+  static __device__ __forceinline__ uint8_t* dyn_smem() {
+    extern __shared__ __align__(128) uint8_t wg_smem[];
+    return wg_smem;
   }
-};
-template <class C>
-struct WgmmaLinear {
-  static constexpr int kSmemBytes = wg::Smem<C::MAXW, C::MAXW>::kBytes;
   template <int K, int N, bool RELU>
   static __device__ __forceinline__ void fwd(const float* __restrict__ W, const float* __restrict__ b, const float (&x)[K], float (&y)[N]) {
-    if constexpr (N < 8) {  // the 1- and 3-wide output heads: 64 MACs per point, exact fp32 on the CUDA cores
+    if constexpr (tensor(N))
+      wg::linear<C::MAXW, C::MAXW, K, N, RELU>(dyn_smem(), W, b, x, y);
+    else
       linear_fwd<K, N, RELU>(W, b, x, y);
-    } else {
-      extern __shared__ __align__(128) uint8_t wg_smem[];
-      wg::linear<C::MAXW, C::MAXW, K, N, RELU>(wg_smem, W, b, x, y);
-    }
+  }
+  template <int K, int N>
+  static __device__ __forceinline__ void dx(const float* __restrict__ W, const float (&dy)[N], float (&dxv)[K]) {
+    if constexpr (tensor(N))
+      wg::linear_dx<C::MAXW, C::MAXW, K, N>(dyn_smem(), W, dy, dxv);
+    else
+      linear_bwd_input<K, N>(W, dy, dxv);
+  }
+  template <int K, int N>
+  static __device__ __forceinline__ void dw(float* sX, float* sY, const float (&x)[K], const float (&dy)[N], float* gW, float* gb) {
+    if constexpr (tensor(N))
+      wg::weight_grad<K, N>(dyn_smem(), x, dy, gW, gb);
+    else
+      tile_weight_grad<K, N>(sX, sY, x, dy, gW, gb);
   }
 };
 
@@ -177,9 +204,10 @@ struct Acts {
   float logit;
 };
 
-template <class C, class Lin = SimtLinear>
+template <class C, bool TC>
 __device__ __forceinline__ void field_mlps(const KParams& P, const float (&enc)[C::ENC], const float* __restrict__ dir,
                                            const float* __restrict__ app, Acts<C>& a) {
+  using Lin = Layers<C, TC>;
   Lin::template fwd<C::ENC, C::BASE_H, true>(P.base_w[0], P.base_b[0], enc, a.h1);
   Lin::template fwd<C::BASE_H, C::BASE_OUT, false>(P.base_w[1], P.base_b[1], a.h1, a.out);
   // semantic branch: mlp_semantics(detach(geo)) -> Linear head (fruit_field.py:263-268)
@@ -228,8 +256,8 @@ __device__ __forceinline__ void block_mean_embedding(const KParams& P, int num_i
 // K1: per-point field forward.
 // ------------------------------------------------------------------------------------------
 // The loop runs whole 128-point tiles per CTA (threads past N compute a clamped point and store nothing), so that the
-// block-wide tensor-core layers of WgmmaLinear see every thread.
-template <class C, class Lin = SimtLinear>
+// block-wide tensor-core layers see every thread.
+template <class C, bool TC>
 __global__ void __launch_bounds__(kThreads) simt_field_forward_kernel(KField F, KParams P, KRays Rr, KFieldOut O) {
   __shared__ float s_app[C::APP];
   block_mean_embedding(P, F.num_images, C::APP, F.appearance_mode, s_app);
@@ -256,7 +284,7 @@ __global__ void __launch_bounds__(kThreads) simt_field_forward_kernel(KField F, 
 #pragma unroll
     for (int i = 0; i < C::APP; ++i) appv[i] = (F.appearance_mode == FNR_APP_PER_CAMERA) ? __ldg(app + i) : app[i];
     Acts<C> a;
-    field_mlps<C, Lin>(P, enc, d, appv, a);
+    field_mlps<C, TC>(P, enc, d, appv, a);
     if (!valid) continue;
     const float density = sel ? expf(a.out[0]) : 0.f;
     if (O.sample_density) O.sample_density[p] = density;
@@ -537,51 +565,10 @@ __device__ __forceinline__ void tile_weight_grad(float* __restrict__ sX, float* 
   }
 }
 
-// How the backward evaluates a layer: recompute, input gradient dx = W^T dy and weight gradient dW = dY^T X per tile, either
-// in fp32 on the CUDA cores (the exact device reference) or block-wide on the tensor cores (fnr_wgmma.cuh).  The 1- and
-// 3-wide output heads stay in fp32 on both.
-struct SimtBackward {
-  using Lin = SimtLinear;
-  static constexpr int kSmemBytes(int maxw) { return 2 * kThreads * (((maxw + 3) & ~3) + 4) * 4; }
-  template <int K, int N>
-  static __device__ __forceinline__ void dx(const float* __restrict__ W, const float (&dy)[N], float (&dxv)[K]) {
-    linear_bwd_input<K, N>(W, dy, dxv);
-  }
-  template <int K, int N>
-  static __device__ __forceinline__ void dw(float* sX, float* sY, const float (&x)[K], const float (&dy)[N], float* gW, float* gb) {
-    tile_weight_grad<K, N>(sX, sY, x, dy, gW, gb);
-  }
-};
-template <class C>
-struct WgmmaBackward {
-  using Lin = WgmmaLinear<C>;
-  static constexpr int cmax(int a, int b) { return a > b ? a : b; }
-  static constexpr int kSmemBytes(int maxw) {
-    return cmax(cmax(WgmmaLinear<C>::kSmemBytes, wg::DwSmem<C::MAXW, C::MAXW>::kBytes), SimtBackward::kSmemBytes(maxw));
-  }
-  template <int K, int N>
-  static __device__ __forceinline__ void dx(const float* __restrict__ W, const float (&dy)[N], float (&dxv)[K]) {
-    if constexpr (N < 8) {
-      linear_bwd_input<K, N>(W, dy, dxv);
-    } else {
-      extern __shared__ __align__(128) uint8_t wg_smem[];
-      wg::linear_dx<C::MAXW, C::MAXW, K, N>(wg_smem, W, dy, dxv);
-    }
-  }
-  template <int K, int N>
-  static __device__ __forceinline__ void dw(float* sX, float* sY, const float (&x)[K], const float (&dy)[N], float* gW, float* gb) {
-    if constexpr (N < 8) {
-      tile_weight_grad<K, N>(sX, sY, x, dy, gW, gb);
-    } else {
-      extern __shared__ __align__(128) uint8_t wg_smem[];
-      wg::weight_grad<K, N>(wg_smem, x, dy, gW, gb);
-    }
-  }
-};
-
-template <class C, class Bw = SimtBackward>
+template <class C, bool TC>
 __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F, KParams P, KParams G, KRays Rr,
                                                                       KFieldBwd B) {
+  using Lin = Layers<C, TC>;
   extern __shared__ __align__(16) float smem[];
   constexpr int TP = ((C::MAXW + 3) & ~3) + 4;
   float* sX = smem;
@@ -620,7 +607,7 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
     for (int i = 0; i < C::APP; ++i)
       appv[i] = (F.appearance_mode == FNR_APP_PER_CAMERA) ? __ldg(P.app_embedding + (size_t)cam * C::APP + i) : s_app[i];
     Acts<C> a;
-    field_mlps<C, typename Bw::Lin>(P, enc, d, appv, a);
+    field_mlps<C, TC>(P, enc, d, appv, a);
 
     // upstream per-point grads (zero for padding threads)
     const float* pg = B.point_grads + 5 * (size_t)pc;
@@ -637,30 +624,30 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
     {
       float dlg[1] = {d_logit};
       float dzo[C::SEM_OUT];
-      Bw::template dx<C::SEM_OUT, 1>(P.head_w, dlg, dzo);
-      Bw::template dw<C::SEM_OUT, 1>(sX, sY, a.zo, dlg, G.head_w, G.head_b);
+      Lin::template dx<C::SEM_OUT, 1>(P.head_w, dlg, dzo);
+      Lin::template dw<C::SEM_OUT, 1>(sX, sY, a.zo, dlg, G.head_w, G.head_b);
       float geo[C::GEO];
 #pragma unroll
       for (int i = 0; i < C::GEO; ++i) geo[i] = a.out[1 + i];
       float dz1[C::SEM_H];
       if constexpr (C::SEM_LAYERS == 3) {
         float dz2[C::SEM_H];
-        Bw::template dx<C::SEM_H, C::SEM_OUT>(P.sem_w[2], dzo, dz2);
-        Bw::template dw<C::SEM_H, C::SEM_OUT>(sX, sY, a.z2, dzo, G.sem_w[2], G.sem_b[2]);
+        Lin::template dx<C::SEM_H, C::SEM_OUT>(P.sem_w[2], dzo, dz2);
+        Lin::template dw<C::SEM_H, C::SEM_OUT>(sX, sY, a.z2, dzo, G.sem_w[2], G.sem_b[2]);
 #pragma unroll
         for (int i = 0; i < C::SEM_H; ++i) dz2[i] = a.z2[i] > 0.f ? dz2[i] : 0.f;
-        Bw::template dx<C::SEM_H, C::SEM_H>(P.sem_w[1], dz2, dz1);
-        Bw::template dw<C::SEM_H, C::SEM_H>(sX, sY, a.z1, dz2, G.sem_w[1], G.sem_b[1]);
+        Lin::template dx<C::SEM_H, C::SEM_H>(P.sem_w[1], dz2, dz1);
+        Lin::template dw<C::SEM_H, C::SEM_H>(sX, sY, a.z1, dz2, G.sem_w[1], G.sem_b[1]);
       } else {
-        Bw::template dx<C::SEM_H, C::SEM_OUT>(P.sem_w[1], dzo, dz1);
-        Bw::template dw<C::SEM_H, C::SEM_OUT>(sX, sY, a.z1, dzo, G.sem_w[1], G.sem_b[1]);
+        Lin::template dx<C::SEM_H, C::SEM_OUT>(P.sem_w[1], dzo, dz1);
+        Lin::template dw<C::SEM_H, C::SEM_OUT>(sX, sY, a.z1, dzo, G.sem_w[1], G.sem_b[1]);
       }
 #pragma unroll
       for (int i = 0; i < C::SEM_H; ++i) dz1[i] = a.z1[i] > 0.f ? dz1[i] : 0.f;
-      Bw::template dw<C::GEO, C::SEM_H>(sX, sY, geo, dz1, G.sem_w[0], G.sem_b[0]);
+      Lin::template dw<C::GEO, C::SEM_H>(sX, sY, geo, dz1, G.sem_w[0], G.sem_b[0]);
       if (F.pass_semantic_gradients) {
         float dg[C::GEO];
-        Bw::template dx<C::GEO, C::SEM_H>(P.sem_w[0], dz1, dg);
+        Lin::template dx<C::GEO, C::SEM_H>(P.sem_w[0], dz1, dg);
 #pragma unroll
         for (int i = 0; i < C::GEO; ++i) d_geo[i] += dg[i];
       }
@@ -671,16 +658,16 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
 #pragma unroll
       for (int i = 0; i < 3; ++i) do3[i] = d_rgb[i] * a.rgb[i] * (1.0f - a.rgb[i]);
       float dc2[C::COL_H], dc1[C::COL_H], dcin[C::COL_IN];
-      Bw::template dx<C::COL_H, 3>(P.col_w[2], do3, dc2);
-      Bw::template dw<C::COL_H, 3>(sX, sY, a.c2, do3, G.col_w[2], G.col_b[2]);
+      Lin::template dx<C::COL_H, 3>(P.col_w[2], do3, dc2);
+      Lin::template dw<C::COL_H, 3>(sX, sY, a.c2, do3, G.col_w[2], G.col_b[2]);
 #pragma unroll
       for (int i = 0; i < C::COL_H; ++i) dc2[i] = a.c2[i] > 0.f ? dc2[i] : 0.f;
-      Bw::template dx<C::COL_H, C::COL_H>(P.col_w[1], dc2, dc1);
-      Bw::template dw<C::COL_H, C::COL_H>(sX, sY, a.c1, dc2, G.col_w[1], G.col_b[1]);
+      Lin::template dx<C::COL_H, C::COL_H>(P.col_w[1], dc2, dc1);
+      Lin::template dw<C::COL_H, C::COL_H>(sX, sY, a.c1, dc2, G.col_w[1], G.col_b[1]);
 #pragma unroll
       for (int i = 0; i < C::COL_H; ++i) dc1[i] = a.c1[i] > 0.f ? dc1[i] : 0.f;
-      Bw::template dx<C::COL_IN, C::COL_H>(P.col_w[0], dc1, dcin);
-      Bw::template dw<C::COL_IN, C::COL_H>(sX, sY, a.cin, dc1, G.col_w[0], G.col_b[0]);
+      Lin::template dx<C::COL_IN, C::COL_H>(P.col_w[0], dc1, dcin);
+      Lin::template dw<C::COL_IN, C::COL_H>(sX, sY, a.cin, dc1, G.col_w[0], G.col_b[0]);
 #pragma unroll
       for (int i = 0; i < C::GEO; ++i) d_geo[i] += dcin[C::SH + i];
       // appearance-embedding gradient (only the per-camera rows are parameters of the graph;
@@ -716,12 +703,12 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
 #pragma unroll
       for (int i = 0; i < C::GEO; ++i) dout[1 + i] = d_geo[i];
       float dh1[C::BASE_H];
-      Bw::template dx<C::BASE_H, C::BASE_OUT>(P.base_w[1], dout, dh1);
-      Bw::template dw<C::BASE_H, C::BASE_OUT>(sX, sY, a.h1, dout, G.base_w[1], G.base_b[1]);
+      Lin::template dx<C::BASE_H, C::BASE_OUT>(P.base_w[1], dout, dh1);
+      Lin::template dw<C::BASE_H, C::BASE_OUT>(sX, sY, a.h1, dout, G.base_w[1], G.base_b[1]);
 #pragma unroll
       for (int i = 0; i < C::BASE_H; ++i) dh1[i] = a.h1[i] > 0.f ? dh1[i] : 0.f;
-      Bw::template dx<C::ENC, C::BASE_H>(P.base_w[0], dh1, denc);
-      Bw::template dw<C::ENC, C::BASE_H>(sX, sY, enc, dh1, G.base_w[0], G.base_b[0]);
+      Lin::template dx<C::ENC, C::BASE_H>(P.base_w[0], dh1, denc);
+      Lin::template dw<C::ENC, C::BASE_H>(sX, sY, enc, dh1, G.base_w[0], G.base_b[0]);
     }
     // ---- hash-table scatter -----------------------------------------------------------------
     if (valid) {
@@ -759,7 +746,7 @@ __device__ __forceinline__ int warp_claim(int* counter, bool pred, int lane, int
   return basev;
 }
 
-template <class C, class Lin = SimtLinear>
+template <class C, bool TC>
 __global__ void __launch_bounds__(kThreads) simt_export_kernel(KField F, KParams P, KExport E) {
   __shared__ float s_app[C::APP];
   block_mean_embedding(P, F.num_images, C::APP, FNR_APP_MEAN, s_app);
@@ -787,7 +774,7 @@ __global__ void __launch_bounds__(kThreads) simt_export_kernel(KField F, KParams
 #pragma unroll
     for (int i = 0; i < C::APP; ++i) appv[i] = s_app[i];
     Acts<C> a;
-    field_mlps<C, Lin>(P, enc, E.normal, appv, a);
+    field_mlps<C, TC>(P, enc, E.normal, appv, a);
     const float density = sel ? expf(a.out[0]) : 0.f;
     const float sg = sigmoidf_(a.logit);
     // heaviside(sigmoid(logit) - thr, 0): 1 iff sigmoid - thr > 0
@@ -879,18 +866,6 @@ int sm_count() {
   return n;
 }
 
-int launch_simt_field_forward(Family fam, const KField& F, const KParams& P, const KRays& Rr, const KFieldOut& O,
-                              cudaStream_t st) {
-  const long long N = (long long)Rr.R * Rr.S;
-  if (N == 0) return FNR_OK;
-  const int grid = grid_for(N, kThreads, sm_count() * 16);
-  if (fam == kFamilySmall)
-    simt_field_forward_kernel<CfgSmall><<<grid, kThreads, 0, st>>>(F, P, Rr, O);
-  else
-    simt_field_forward_kernel<CfgBig><<<grid, kThreads, 0, st>>>(F, P, Rr, O);
-  return check_launch("simt_field_forward_kernel");
-}
-
 int launch_simt_composite(const KRays& Rr, const KComposite& Cm, cudaStream_t st) {
   if (Rr.R == 0) return FNR_OK;
   const int grid = grid_for(Rr.R, kThreads / 32, sm_count() * 16);
@@ -905,86 +880,57 @@ int launch_simt_composite_backward(const KRays& Rr, const KCompositeBwd& B, cuda
   return check_launch("simt_composite_backward_kernel");
 }
 
-template <class C, class Bw>
-static int launch_bwd(const KField& F, const KParams& P, const KParams& G, const KRays& Rr, const KFieldBwd& B, cudaStream_t st) {
-  constexpr int smem = Bw::kSmemBytes(C::MAXW);
-  auto kernel = simt_field_backward_kernel<C, Bw>;
-  // per device: set on every call (cheap), so that a process driving several GPUs opts in on each of them
-  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute(simt_field_backward_kernel)");
-  int per_sm = 0;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, smem);
-  if (e != cudaSuccess) return check_cuda(e, "cudaOccupancyMaxActiveBlocksPerMultiprocessor");
-  const long long N = (long long)Rr.R * Rr.S;
-  const int grid = grid_for(N, kThreads, sm_count() * (per_sm > 0 ? per_sm : 1));
-  kernel<<<grid, kThreads, smem, st>>>(F, P, G, Rr, B);
-  return check_launch("simt_field_backward_kernel");
-}
-
-int launch_simt_field_backward(Family fam, const KField& F, const KParams& P, const KParams& G, const KRays& Rr,
-                               const KFieldBwd& B, cudaStream_t st) {
-  if ((long long)Rr.R * Rr.S == 0) return FNR_OK;
-  return fam == kFamilySmall ? launch_bwd<CfgSmall, SimtBackward>(F, P, G, Rr, B, st) : launch_bwd<CfgBig, SimtBackward>(F, P, G, Rr, B, st);
-}
-
-int launch_wgmma_field_backward(Family fam, const KField& F, const KParams& P, const KParams& G, const KRays& Rr, const KFieldBwd& B,
-                                cudaStream_t st) {
-  if ((long long)Rr.R * Rr.S == 0) return FNR_OK;
-  return fam == kFamilySmall ? launch_bwd<CfgSmall, WgmmaBackward<CfgSmall>>(F, P, G, Rr, B, st)
-                             : launch_bwd<CfgBig, WgmmaBackward<CfgBig>>(F, P, G, Rr, B, st);
-}
-
-int launch_simt_export(Family fam, const KField& F, const KParams& P, const KExport& E, cudaStream_t st) {
-  const long long N = (long long)E.B * E.S;
+// One launch of a field kernel over N points.  Kernels with dynamic shared memory (the backward and every tensor-core
+// instantiation) opt in to it and run as many CTAs as fit on the SMs; the simt forward and export run 16 CTAs per SM.
+template <class Kernel, class... Args>
+static int launch_field_kernel(Kernel kernel, int smem, long long N, const char* name, cudaStream_t st, const Args&... args) {
   if (N == 0) return FNR_OK;
-  const int grid = grid_for(N, kThreads, sm_count() * 16);
-  if (fam == kFamilySmall)
-    simt_export_kernel<CfgSmall><<<grid, kThreads, 0, st>>>(F, P, E);
-  else
-    simt_export_kernel<CfgBig><<<grid, kThreads, 0, st>>>(F, P, E);
-  return check_launch("simt_export_kernel");
+  int per_sm = 16;
+  if (smem > 0) {
+    // per device: set on every call (cheap), so that a process driving several GPUs opts in on each of them
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute");
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, smem);
+    if (e != cudaSuccess) return check_cuda(e, "cudaOccupancyMaxActiveBlocksPerMultiprocessor");
+    if (per_sm < 1) per_sm = 1;
+  }
+  kernel<<<grid_for(N, kThreads, sm_count() * per_sm), kThreads, smem, st>>>(args...);
+  return check_launch(name);
 }
 
-// Tensor-core (wgmma) instantiations of the forward and export kernels: one 128-thread CTA (one warpgroup) per SM slot
-// the shared-memory plan of WgmmaLinear allows.
-template <class K, class C>
-static int wgmma_grid(K kernel, long long N, int& grid) {
-  // per device: set on every call (cheap), so that a process driving several GPUs opts in on each of them
-  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WgmmaLinear<C>::kSmemBytes);
-  if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute(wgmma field kernel)");
-  int per_sm = 0;
-  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, WgmmaLinear<C>::kSmemBytes);
-  if (e != cudaSuccess) return check_cuda(e, "cudaOccupancyMaxActiveBlocksPerMultiprocessor");
-  grid = grid_for(N, kThreads, sm_count() * (per_sm > 0 ? per_sm : 1));
-  return FNR_OK;
+// Calls launch(C{}, std::bool_constant<TC>{}) with the family's config C and the implementation TC as types.
+template <class Launch>
+static int with_layers(Family fam, bool tc, Launch launch) {
+  if (fam == kFamilySmall) return tc ? launch(CfgSmall{}, std::true_type{}) : launch(CfgSmall{}, std::false_type{});
+  return tc ? launch(CfgBig{}, std::true_type{}) : launch(CfgBig{}, std::false_type{});
 }
 
-template <class C>
-static int launch_wgmma_forward_c(const KField& F, const KParams& P, const KRays& Rr, const KFieldOut& O, cudaStream_t st) {
-  auto kernel = simt_field_forward_kernel<C, WgmmaLinear<C>>;
-  int grid = 0, rc = wgmma_grid<decltype(kernel), C>(kernel, (long long)Rr.R * Rr.S, grid);
-  if (rc) return rc;
-  kernel<<<grid, kThreads, WgmmaLinear<C>::kSmemBytes, st>>>(F, P, Rr, O);
-  return check_launch("simt_field_forward_kernel<wgmma>");
+int launch_field_forward(Family fam, bool tc, const KField& F, const KParams& P, const KRays& Rr, const KFieldOut& O, cudaStream_t st) {
+  return with_layers(fam, tc, [&](auto c, auto t) {
+    using C = decltype(c);
+    constexpr bool TC = decltype(t)::value;
+    return launch_field_kernel(simt_field_forward_kernel<C, TC>, Layers<C, TC>::kFwdSmemBytes, (long long)Rr.R * Rr.S,
+                               TC ? "simt_field_forward_kernel<wgmma>" : "simt_field_forward_kernel", st, F, P, Rr, O);
+  });
 }
 
-int launch_wgmma_field_forward(Family fam, const KField& F, const KParams& P, const KRays& Rr, const KFieldOut& O, cudaStream_t st) {
-  if ((long long)Rr.R * Rr.S == 0) return FNR_OK;
-  return fam == kFamilySmall ? launch_wgmma_forward_c<CfgSmall>(F, P, Rr, O, st) : launch_wgmma_forward_c<CfgBig>(F, P, Rr, O, st);
+int launch_field_backward(Family fam, bool tc, const KField& F, const KParams& P, const KParams& G, const KRays& Rr, const KFieldBwd& B,
+                          cudaStream_t st) {
+  return with_layers(fam, tc, [&](auto c, auto t) {
+    using C = decltype(c);
+    constexpr bool TC = decltype(t)::value;
+    return launch_field_kernel(simt_field_backward_kernel<C, TC>, Layers<C, TC>::kBwdSmemBytes, (long long)Rr.R * Rr.S,
+                               TC ? "simt_field_backward_kernel<wgmma>" : "simt_field_backward_kernel", st, F, P, G, Rr, B);
+  });
 }
 
-template <class C>
-static int launch_wgmma_export_c(const KField& F, const KParams& P, const KExport& E, cudaStream_t st) {
-  auto kernel = simt_export_kernel<C, WgmmaLinear<C>>;
-  int grid = 0, rc = wgmma_grid<decltype(kernel), C>(kernel, (long long)E.B * E.S, grid);
-  if (rc) return rc;
-  kernel<<<grid, kThreads, WgmmaLinear<C>::kSmemBytes, st>>>(F, P, E);
-  return check_launch("simt_export_kernel<wgmma>");
-}
-
-int launch_wgmma_export(Family fam, const KField& F, const KParams& P, const KExport& E, cudaStream_t st) {
-  if ((long long)E.B * E.S == 0) return FNR_OK;
-  return fam == kFamilySmall ? launch_wgmma_export_c<CfgSmall>(F, P, E, st) : launch_wgmma_export_c<CfgBig>(F, P, E, st);
+int launch_export(Family fam, bool tc, const KField& F, const KParams& P, const KExport& E, cudaStream_t st) {
+  return with_layers(fam, tc, [&](auto c, auto t) {
+    using C = decltype(c);
+    constexpr bool TC = decltype(t)::value;
+    return launch_field_kernel(simt_export_kernel<C, TC>, Layers<C, TC>::kFwdSmemBytes, (long long)E.B * E.S,
+                               TC ? "simt_export_kernel<wgmma>" : "simt_export_kernel", st, F, P, E);
+  });
 }
 
 int launch_hash_indices(const KField& F, const KRays& Rr, int32_t* rows, float* positions, cudaStream_t st) {

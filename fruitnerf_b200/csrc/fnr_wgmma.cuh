@@ -1,5 +1,5 @@
 // Hopper (sm_90a) warpgroup MMA layer: the MLP layers of the tensor-core field forward and backward (fnr_simt.cu,
-// WgmmaLinear / WgmmaBackward): y = W x + b, dx = W^T dy and dW = dY^T X of a 128-point tile.
+// Layers<C, true>): y = W x + b, dx = W^T dy and dW = dY^T X of a 128-point tile.
 //
 // One CTA of 128 threads = one warpgroup = one tile of 128 sample points, thread t owning point t.  A layer
 // y = W x + b is one block-wide step: every thread writes its row x[K] into shared memory as a bf16 hi/lo split

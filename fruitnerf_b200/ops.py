@@ -159,7 +159,7 @@ class _Render(torch.autograd.Function):
         params = [p.detach() for p in params]
         need_grad = any(ctx.needs_input_grad[7:])
         composite = mode["composite"]
-        desc = shape.desc(mode["position_mode"], mode["appearance_mode"], mode.get("impl", L.FNR_IMPL_AUTO))
+        desc = shape.desc(mode["position_mode"], mode["appearance_mode"], mode["impl"])
         pstruct = _params_struct(shape, params)
         rays = L.RayBatch(R, S, _ptr(origins), _ptr(directions), _ptr(starts), _ptr(ends), _ptr(cam))
 
@@ -202,7 +202,7 @@ class _Render(torch.autograd.Function):
             g_sd, g_srgb, g_ssem = g
             g_rgb = g_acc = g_sem = g_w = None
         gs = [None if t is None else _f32c(t) for t in (g_rgb, g_acc, g_sem, g_w, g_sd, g_srgb, g_ssem)]
-        desc = shape.desc(mode["position_mode"], mode["appearance_mode"], mode.get("bwd_impl", mode.get("impl", L.FNR_IMPL_AUTO)))
+        desc = shape.desc(mode["position_mode"], mode["appearance_mode"], mode["impl"])
         pstruct = _params_struct(shape, params)
         flat, views = flat_zero_grads(params, out=mode.get("flat_grad"))
         gstruct = _params_struct(shape, views)

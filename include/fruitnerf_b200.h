@@ -68,9 +68,9 @@ extern "C" {
 #define FNR_APP_ZEROS 2      /* zeros                    (eval without average embedding) */
 
 /* implementation selector for the forward, export and backward kernels */
-#define FNR_IMPL_AUTO 0    /* tensor-core kernels for the shipped network shapes, else simt */
+#define FNR_IMPL_AUTO 0    /* tensor-core kernels (every shape that passes validation has them) */
 #define FNR_IMPL_SIMT 1    /* fp32 CUDA-core kernels (exact-fp32 device reference) */
-#define FNR_IMPL_TCGEN05 2 /* tensor-core kernels (wgmma on sm_90a; historical name); FNR_ERR_UNSUPPORTED if shape unsupported */
+#define FNR_IMPL_TCGEN05 2 /* tensor-core kernels, as AUTO (wgmma on sm_90a; historical name) */
 
 /* One nn.Linear stack: n_layers Linear layers, ReLU between them (nerfstudio MLP torch path);
  * dims[0] = input width, dims[n_layers] = output width. */

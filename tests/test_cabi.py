@@ -60,6 +60,28 @@ def test_invalid_arguments_return_error_codes(native_lib):
     assert native_lib.fnr_render_backward_scratch_bytes(C.byref(d), 8, 8, C.byref(n)) == -2
 
 
+def test_invalid_impl_is_rejected_by_every_field_entry_point(native_lib):
+    from fruitnerf_b200 import _lib as L
+
+    d = L.FieldDesc()  # fruit_nerf (small family) shape
+    d.num_levels, d.features_per_level, d.log2_hashmap_size, d.num_images, d.appearance_dim = 16, 2, 19, 3, 32
+    d.geo_feat_dim = 15
+    for m, dims in ((d.base, (32, 64, 16)), (d.semantic, (15, 64, 64)), (d.color, (63, 64, 64, 3))):
+        m.n_layers = len(dims) - 1
+        for i, v in enumerate(dims):
+            m.dims[i] = v
+    d.impl = 7
+    calls = {
+        "fnr_render_forward": lambda: native_lib.fnr_render_forward(C.byref(d), None, None, None, None),
+        "fnr_render_backward": lambda: native_lib.fnr_render_backward(C.byref(d), None, None, None, None, None, None, 0, None),
+        "fnr_export_forward": lambda: native_lib.fnr_export_forward(C.byref(d), None, None, None, None, 0.0, 1.0, 0, 1, 0, None,
+                                                                    None, None),
+    }
+    for name, call in calls.items():
+        assert call() == -1, name
+        assert b"invalid impl" in native_lib.fnr_last_error(), name
+
+
 def test_ops_refuse_cpu_tensors(native_lib):
     import torch
 

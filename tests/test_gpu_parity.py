@@ -76,12 +76,7 @@ def test_field_forward_matches_oracle(native_lib, cuda_device, name, mode, impl)
             camera_indices=cam[:, None, None].expand(R, S, 1).cuda(),
         )
         with torch.no_grad():
-            try:
-                out = field(rs)
-            except L.FruitNerfNativeError as ex:
-                if impl == L.FNR_IMPL_TCGEN05 and "does not support" in str(ex):
-                    pytest.skip(str(ex))
-                raise
+            out = field(rs)
         ref = _oracle_field(sd, spec, o, d, s, e, cam, True, mode)
         assert_rel(out[FieldHeadNames.DENSITY], ref["density"], what="density")
         assert_rel(out[FieldHeadNames.RGB], ref["rgb"], what="rgb")
@@ -143,13 +138,8 @@ def test_render_forward_matches_oracle(native_lib, cuda_device, name, S, impl):
     sd, spec = make_state(name)
     field = make_field(name, sd, spec, cuda_device).train()
     o, d, s, e, cam = _rays(96, S, salt=3, far=3.0)
-    try:
-        with torch.no_grad():
-            out = _render_gpu(field, o, d, s, e, cam, impl)
-    except L.FruitNerfNativeError as ex:
-        if impl == L.FNR_IMPL_TCGEN05 and "does not support" in str(ex):
-            pytest.skip(str(ex))
-        raise
+    with torch.no_grad():
+        out = _render_gpu(field, o, d, s, e, cam, impl)
     f = _oracle_field(sd, spec, o, d, s, e, cam, True, "train")
     ref = fr.render(f, s[..., None], e[..., None], training=True)
     assert_rel(out["rgb"], ref["rgb"], what="rgb")
@@ -215,8 +205,8 @@ def _safe_ray_weights(f, R):
 @pytest.mark.parametrize("impl", [L.FNR_IMPL_SIMT, L.FNR_IMPL_TCGEN05, L.FNR_IMPL_AUTO], ids=["simt", "tcgen05", "auto"])
 @pytest.mark.parametrize("name,R,S", [("small", 128, 48), ("big", 128, 48), ("small", 111, 50), ("big", 77, 37)])
 def test_backward_matches_oracle_autograd(native_lib, cuda_device, name, R, S, impl):
-    """auto = fused tcgen05 forward + tensor-core backward where the shape is covered (small family),
-    simt kernels otherwise; 111 x 50 = 5550 points exercises a ragged last tile and warps that span rays."""
+    """tcgen05 and auto both run the wgmma forward and backward kernels, simt the fp32 ones; 111 x 50 = 5550 points
+    exercises a ragged last tile and warps that span rays."""
     sd, spec = make_state(name, log2T=15)  # small table keeps the oracle's dense grad comparison cheap
     field = make_field(name, sd, spec, cuda_device).train()
     o, d, s, e, cam = _rays(R, S, salt=5, far=3.0)
@@ -364,14 +354,9 @@ def test_full_size_properties(native_lib, cuda_device, impl):
     sd, spec = make_state("small", table_scale=0.5)
     field = make_field("small", sd, spec, cuda_device).train()
     o, d, s, e, cam = _rays(4096, 192, salt=1, num_images=7)
-    try:
-        with torch.no_grad():
-            a = _render_gpu(field, o, d, s, e, cam, impl)
-            b = _render_gpu(field, o, d, s, e, cam, impl)
-    except L.FruitNerfNativeError as ex:
-        if impl == L.FNR_IMPL_TCGEN05 and "does not support" in str(ex):
-            pytest.skip(str(ex))
-        raise
+    with torch.no_grad():
+        a = _render_gpu(field, o, d, s, e, cam, impl)
+        b = _render_gpu(field, o, d, s, e, cam, impl)
     for k in ("rgb", "accumulation", "semantics", "weights", "depth"):
         assert torch.equal(a[k], b[k]), f"{k} not deterministic"
     w = a["weights"]
