@@ -195,6 +195,11 @@ EXPORTED_SYMBOLS = (
     "fnr_spaced_bins",
     "fnr_render_losses",
     "fnr_ray_metrics",
+    "fnr_cluster_scratch_bytes",
+    "fnr_radius_count",
+    "fnr_voxel_down_sample",
+    "fnr_dbscan",
+    "fnr_cluster_sums",
 )
 
 _lib = None
@@ -259,6 +264,17 @@ def load() -> C.CDLL:
     lib.fnr_render_losses.argtypes = [vp, vp, vp, vp, i32, f32, vp, vp, vp, vp]
     lib.fnr_ray_metrics.restype = C.c_int
     lib.fnr_ray_metrics.argtypes = [vp, vp, vp, vp, i32, i32, vp, vp, vp]
+    i64, f64, f64p, sz = C.c_int64, C.c_double, C.POINTER(C.c_double), C.c_size_t
+    lib.fnr_cluster_scratch_bytes.restype = C.c_int
+    lib.fnr_cluster_scratch_bytes.argtypes = [i64, C.POINTER(C.c_size_t)]
+    lib.fnr_radius_count.restype = C.c_int
+    lib.fnr_radius_count.argtypes = [vp, i64, f64p, f64p, f64, i32, vp, vp, sz, vp]
+    lib.fnr_voxel_down_sample.restype = C.c_int
+    lib.fnr_voxel_down_sample.argtypes = [vp, i64, f64p, f64p, f64, vp, vp, vp, sz, vp]
+    lib.fnr_dbscan.restype = C.c_int
+    lib.fnr_dbscan.argtypes = [vp, i64, f64p, f64p, f64, i32, vp, vp, vp, sz, vp]
+    lib.fnr_cluster_sums.restype = C.c_int
+    lib.fnr_cluster_sums.argtypes = [vp, vp, i64, i32, vp, vp, vp, sz, vp]
     if lib.fnr_version() != ABI_VERSION:
         raise FruitNerfNativeError(f"ABI version mismatch: library reports {lib.fnr_version()}")
     _lib = lib

@@ -124,3 +124,57 @@ def write_ply(path, points: np.ndarray, colors: np.ndarray) -> None:
     with open(path, "wb") as f:
         f.write(header.encode("ascii"))
         f.write(rec.tobytes())
+
+
+_PLY_TYPES = {
+    "char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "<i2", "int16": "<i2", "ushort": "<u2", "uint16": "<u2",
+    "int": "<i4", "int32": "<i4", "uint": "<u4", "uint32": "<u4", "float": "<f4", "float32": "<f4", "double": "<f8", "float64": "<f8",
+}
+
+
+def read_ply(path):
+    """Binary little-endian PLY point cloud -> (points [N,3] float64, colors [N,3] float64 in [0,1] or None).
+
+    Reads what ``write_ply`` and open3d's write_point_cloud produce: float or double x/y/z, optional uchar
+    red/green/blue; any other vertex property is skipped by its declared type.  Elements other than ``vertex`` must have
+    no rows (a point cloud has no faces)."""
+    with open(path, "rb") as f:
+        if f.readline().strip() != b"ply":
+            raise ValueError(f"{path}: not a PLY file")
+        fmt, elements = None, []
+        while True:
+            line = f.readline()
+            if not line:
+                raise ValueError(f"{path}: PLY header has no end_header")
+            tok = line.decode("ascii", "replace").split()
+            if not tok or tok[0] in ("comment", "obj_info"):
+                continue
+            if tok[0] == "end_header":
+                break
+            if tok[0] == "format":
+                fmt = tok[1]
+            elif tok[0] == "element":
+                elements.append((tok[1], int(tok[2]), []))
+            elif tok[0] == "property":
+                if not elements:
+                    raise ValueError(f"{path}: property before any element")
+                if tok[1] == "list":
+                    raise ValueError(f"{path}: list property '{tok[-1]}' is not supported in a point cloud")
+                if tok[1] not in _PLY_TYPES:
+                    raise ValueError(f"{path}: unknown PLY type '{tok[1]}'")
+                elements[-1][2].append((tok[2], _PLY_TYPES[tok[1]]))
+        if fmt != "binary_little_endian":
+            raise ValueError(f"{path}: only binary_little_endian PLY is supported, got {fmt}")
+        vertex = None
+        for name, count, props in elements:
+            if name == "vertex":
+                vertex = np.frombuffer(f.read(count * np.dtype(props).itemsize), dtype=np.dtype(props), count=count)
+            elif count:
+                raise ValueError(f"{path}: element '{name}' with {count} rows is not a point cloud")
+    if vertex is None or not {"x", "y", "z"} <= set(vertex.dtype.names):
+        raise ValueError(f"{path}: no vertex x/y/z")
+    points = np.stack([vertex["x"], vertex["y"], vertex["z"]], axis=1).astype(np.float64)
+    colors = None
+    if {"red", "green", "blue"} <= set(vertex.dtype.names):
+        colors = np.stack([vertex["red"], vertex["green"], vertex["blue"]], axis=1).astype(np.float64) / 255.0
+    return points, colors

@@ -554,3 +554,92 @@ def median_depth(weights: Tensor, starts: Tensor, ends: Tensor) -> Tensor:
     L.check(L.load().fnr_ray_metrics(_f32c(weights.detach()).data_ptr(), None, _f32c(starts.detach()).data_ptr(), _f32c(ends.detach()).data_ptr(), R, S,
                                      None, depth.data_ptr(), _stream(dev)))
     return depth
+
+
+# ======================================================================================================
+# Fruit counting on the exported cloud (fnr_cluster.cu; clustering/clustering_base.py:138-143, 183-259)
+# ======================================================================================================
+def cluster_points(points: Tensor) -> Tensor:
+    """[n,3] fp64 contiguous copy/view of a CUDA point tensor (float32 is upcast).  Non-finite coordinates raise ValueError."""
+    _require_cuda(points)
+    pts = points.detach().reshape(-1, 3)
+    if pts.dtype != torch.float64:
+        pts = pts.double()
+    pts = pts.contiguous()
+    if pts.shape[0] and not bool(torch.isfinite(pts).all()):
+        raise ValueError("point cloud has non-finite coordinates")
+    return pts
+
+
+def _bounds(pts: Tensor):
+    """Per-axis minimum and maximum as host double[3] arrays: the grid origin and extent of fnr_cluster.cu."""
+    if pts.shape[0] == 0:
+        return None, None
+    lo, hi = torch.aminmax(pts, dim=0)
+    b = torch.stack([lo, hi]).cpu().tolist()
+    return (C.c_double * 3)(*b[0]), (C.c_double * 3)(*b[1])
+
+
+def _cluster_scratch(n: int, dev) -> Tensor:
+    nbytes = C.c_size_t(0)
+    L.check(L.load().fnr_cluster_scratch_bytes(n, C.byref(nbytes)))
+    return torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+
+
+def radius_count(points: Tensor, radius: float, cap: int) -> Tensor:
+    """int32 [n]: min(cap, number of points within ``radius`` of each point, itself included) -- the
+    NearestNeighbors(radius).radius_neighbors list lengths, saturated."""
+    pts = cluster_points(points)
+    n, dev = pts.shape[0], pts.device
+    counts = torch.empty(n, dtype=torch.int32, device=dev)
+    lo, hi = _bounds(pts)
+    scratch = _cluster_scratch(n, dev)
+    L.check(L.load().fnr_radius_count(_ptr(pts), n, lo, hi, float(radius), int(cap), _ptr(counts), _ptr(scratch), scratch.numel(),
+                                      _stream(dev)))
+    return counts
+
+
+def voxel_down_sample(points: Tensor, voxel: float) -> Tensor:
+    """[m,3] fp64: clustering.voxel_down_sample bit for bit (one mean per occupied voxel, lexicographic voxel order)."""
+    pts = cluster_points(points)
+    n, dev = pts.shape[0], pts.device
+    if n == 0 or voxel <= 0:
+        return pts
+    out = torch.empty((n, 3), dtype=torch.float64, device=dev)
+    num = torch.zeros(1, dtype=torch.int32, device=dev)
+    lo, hi = _bounds(pts)
+    scratch = _cluster_scratch(n, dev)
+    L.check(L.load().fnr_voxel_down_sample(_ptr(pts), n, lo, hi, float(voxel), _ptr(out), _ptr(num), _ptr(scratch), scratch.numel(),
+                                           _stream(dev)))
+    return out[: int(num.item())]
+
+
+def dbscan(points: Tensor, eps: float, min_samples: int) -> Tuple[Tensor, int]:
+    """(labels int32 [n], number of clusters): sklearn.cluster.DBSCAN(eps, min_samples).labels_, noise = -1."""
+    pts = cluster_points(points)
+    n, dev = pts.shape[0], pts.device
+    labels = torch.empty(n, dtype=torch.int32, device=dev)
+    num = torch.zeros(1, dtype=torch.int32, device=dev)
+    lo, hi = _bounds(pts)
+    scratch = _cluster_scratch(n, dev)
+    L.check(L.load().fnr_dbscan(_ptr(pts), n, lo, hi, float(eps), int(min_samples), _ptr(labels), _ptr(num), _ptr(scratch),
+                                scratch.numel(), _stream(dev)))
+    return labels, int(num.item())
+
+
+def cluster_sums(points: Tensor, labels: Tensor, num_clusters: int) -> Tuple[Tensor, Tensor]:
+    """(fp64 coordinate sums [K,3], int32 point counts [K]) of the labels 0..K-1 (deterministic)."""
+    pts = cluster_points(points)
+    _require_cuda(labels)
+    n, dev = pts.shape[0], pts.device
+    labels = labels.reshape(-1).to(torch.int32).contiguous()
+    if labels.shape[0] != n:
+        raise ValueError(f"{labels.shape[0]} labels for {n} points")
+    sums = torch.zeros((num_clusters, 3), dtype=torch.float64, device=dev)
+    counts = torch.zeros(num_clusters, dtype=torch.int32, device=dev)
+    if num_clusters == 0:
+        return sums, counts
+    scratch = _cluster_scratch(n, dev)
+    L.check(L.load().fnr_cluster_sums(_ptr(pts), _ptr(labels), n, int(num_clusters), _ptr(sums), _ptr(counts), _ptr(scratch),
+                                      scratch.numel(), _stream(dev)))
+    return sums, counts

@@ -62,7 +62,8 @@ def export_and_count(trainer: Trainer, points_per_side: int = 256, half_extent: 
     pts = clouds["semantic_colormap"]["points"]
     h = 2.0 * (2 * half_extent) / (points_per_side - 1)  # grid spacing after the exporter's scale(2)
     geom = dm.train_dataset.geometry
-    res = count_fruits(pts, eps=2.5 * h, min_samples=8, cluster_merge_distance=geom.fruit_radius if geom is not None else 0.04)
+    res = count_fruits(torch.from_numpy(pts).to(trainer.device), eps=2.5 * h, min_samples=8,
+                       cluster_merge_distance=geom.fruit_radius if geom is not None else 0.04)
     out = {"export_seconds": export_s, "export_points": int(num_rays * points_per_side),
            "cloud_sizes": {k: int(v["points"].shape[0]) for k, v in clouds.items()}, "fruit_count": res["count"],
            "fruit_count_before_merge": res["count_before_merge"]}

@@ -115,3 +115,28 @@ def density_state(num_levels: int = 5, log2_hashmap_size: int = 17, hidden: int 
     sd["mlp_base.1.layers.1.bias"] = hash_uniform(1, salt + 5, device) * k1
     sd["aabb"] = torch.tensor(aabb, dtype=torch.float32, device=device)
     return sd
+
+
+def fruit_shell_cloud(n: int, seed: int = 0, points_per_fruit: int = 4000, fruit_radius: float = 0.035, spacing: float = 0.15,
+                      noise_fraction: float = 0.02):
+    """[n,3] float64 numpy cloud that looks like an exported semantic cloud of a tree: n // points_per_fruit fruit shells
+    (radius ``fruit_radius`` with 3 % radial jitter) on a jittered lattice of pitch ``spacing``, plus a fraction of
+    uniform noise over the same box, in shuffled order.  With the defaults its density suits the reference's real-tree
+    counting parameters (clustering/config_real.py).  Unlike the hashed inputs above it comes from numpy's seeded
+    generator: clustering tests compare the CPU and GPU paths on the same machine."""
+    import numpy as np
+
+    rng = np.random.default_rng(seed)
+    k = max(1, n // points_per_fruit)
+    side = math.ceil(k ** (1.0 / 3.0) - 1e-9)
+    cell = np.stack(np.unravel_index(np.arange(k), (side, side, side)), axis=1).astype(np.float64)
+    centers = cell * spacing + rng.uniform(-0.15 * spacing, 0.15 * spacing, (k, 3))
+    n_noise = int(n * noise_fraction)
+    fruit = rng.integers(0, k, n - n_noise)
+    dirs = rng.standard_normal((n - n_noise, 3))
+    dirs /= np.linalg.norm(dirs, axis=1, keepdims=True)
+    radii = fruit_radius * (1.0 + 0.03 * rng.standard_normal((n - n_noise, 1)))
+    shells = centers[fruit] + dirs * radii
+    lo, hi = centers.min(axis=0) - 2 * fruit_radius, centers.max(axis=0) + 2 * fruit_radius
+    noise = rng.uniform(lo, hi, (n_noise, 3))
+    return np.concatenate([shells, noise])[rng.permutation(n)]

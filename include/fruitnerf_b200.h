@@ -35,6 +35,9 @@
  *                        proposal-level median depths (fruit_nerf.py:339-340)
  *   fnr_adam_step        torch.optim.Adam / RAdam over a param group (nerfstudio Optimizers; optimiser
  *                        settings fruit_nerf/fruit_nerf_config.py:47-56, 90-103, 140-153)
+ *   fnr_radius_count, fnr_voxel_down_sample, fnr_dbscan, fnr_cluster_sums
+ *                        stages 1-2 of the fruit counting (clustering/clustering_base.py:138-143, 183-259):
+ *                        radius-outlier removal, voxel down-sampling, DBSCAN, the sums of the centre merge
  */
 #ifndef FRUITNERF_B200_H
 #define FRUITNERF_B200_H
@@ -338,6 +341,43 @@ typedef struct fnr_nvls_desc {
  * the same numel; the kernels of all ranks meet on the signal pads, so all ranks must launch it (like a collective).
  * wire_bf16 != 0: operands cross the links as bf16 (fp32 accumulation in the switch), result rounded to bf16. */
 int fnr_nvls_allreduce_mean(const fnr_nvls_desc* d, size_t numel, int32_t wire_bf16, void* stream);
+
+/* ---- fruit counting on the exported cloud: stages 1-2 of the reference clustering
+ * (clustering/clustering_base.py:138-143 radius-outlier removal + voxel down-sampling, :183-207 DBSCAN, :209-259 the
+ * cluster sums the centre merge runs on).  points: DEVICE [n,3] fp64, 0 <= n <= 2^31 - 1.  lo / hi: HOST arrays of 3
+ * doubles, the per-axis minimum and maximum of the points (the grid origin and extent).  They must enclose every point:
+ * with bounds that do not, points are clamped into the edge cells and counts, voxels and labels are undefined (no
+ * out-of-bounds access; the calls do not detect it).  voxel_down_sample additionally needs lo to be the exact minimum,
+ * as its keys are floor((p - lo) / voxel).  Every call needs the
+ * caller-owned device scratch of fnr_cluster_scratch_bytes(n).  Distances are fp64, d2 = (dx*dx + dy*dy) + dz*dz with
+ * no FMA, compared with <= r*r: scikit-learn's KD-tree radius_neighbors predicate.  Grid cells are keyed with 21 bits
+ * per axis; a radius (eps, voxel size) that needs more cells on an axis returns FNR_ERR_UNSUPPORTED. ---- */
+
+/* Bytes of device scratch any fruit-counting call on n points needs. */
+int fnr_cluster_scratch_bytes(int64_t num_points, size_t* bytes);
+
+/* counts[i] = min(cap, #{j : |p_i - p_j| <= radius}), the point itself included (cap >= 1): the neighbour counts of
+ * radius-outlier removal (keep count - 1 >= nb_points, clustering_base.py:138-143) and of the DBSCAN core test. */
+int fnr_radius_count(const double* points, int64_t num_points, const double* lo, const double* hi, double radius, int32_t cap,
+                     int32_t* counts, void* scratch, size_t scratch_bytes, void* stream);
+
+/* open3d voxel_down_sample as clustering.voxel_down_sample (clustering_base.py:141-143), bit for bit: voxel key
+ * floor((p - lo) / voxel), one row per occupied voxel in lexicographic key order, the mean of its points summed in input
+ * order.  out: DEVICE [n,3] (rows beyond *num_out untouched); *num_out: DEVICE int32. */
+int fnr_voxel_down_sample(const double* points, int64_t num_points, const double* lo, const double* hi, double voxel, double* out,
+                          int32_t* num_out, void* scratch, size_t scratch_bytes, void* stream);
+
+/* sklearn.cluster.DBSCAN(eps, min_samples).labels_ (clustering_base.py:183-207): clusters are the connected components of
+ * the core points (>= min_samples points within eps, itself included), numbered in increasing order of their smallest
+ * core index; a non-core point within eps of a core takes the smallest such cluster label, any other point -1.
+ * labels: DEVICE [n] int32; *num_clusters: DEVICE int32. */
+int fnr_dbscan(const double* points, int64_t num_points, const double* lo, const double* hi, double eps, int32_t min_samples,
+               int32_t* labels, int32_t* num_clusters, void* scratch, size_t scratch_bytes, void* stream);
+
+/* Per-cluster fp64 coordinate sums [num_clusters,3] and point counts [num_clusters] of labels in [0, num_clusters) -- the
+ * inputs of the centre merge (clustering_base.py:209-259).  Deterministic: the same input gives the same bits. */
+int fnr_cluster_sums(const double* points, const int32_t* labels, int64_t num_points, int32_t num_clusters, double* sums,
+                     int32_t* counts, void* scratch, size_t scratch_bytes, void* stream);
 
 /* Hash-grid row indices (exact-integer parity hook): rows[N,L,8] in nerfstudio corner order for
  * the masked [0,1]^3 positions of the given samples; also writes positions[N,3] if non-NULL. */
