@@ -200,6 +200,9 @@ EXPORTED_SYMBOLS = (
     "fnr_voxel_down_sample",
     "fnr_dbscan",
     "fnr_cluster_sums",
+    "fnr_knn_mean_distance",
+    "fnr_estimate_normals",
+    "fnr_backproject_select",
 )
 
 _lib = None
@@ -275,6 +278,12 @@ def load() -> C.CDLL:
     lib.fnr_dbscan.argtypes = [vp, i64, f64p, f64p, f64, i32, vp, vp, vp, sz, vp]
     lib.fnr_cluster_sums.restype = C.c_int
     lib.fnr_cluster_sums.argtypes = [vp, vp, i64, i32, vp, vp, vp, sz, vp]
+    lib.fnr_knn_mean_distance.restype = C.c_int
+    lib.fnr_knn_mean_distance.argtypes = [vp, i64, f64p, f64p, i32, vp, vp, sz, vp]
+    lib.fnr_estimate_normals.restype = C.c_int
+    lib.fnr_estimate_normals.argtypes = [vp, i64, f64p, f64p, i32, vp, vp, vp, sz, vp]
+    lib.fnr_backproject_select.restype = C.c_int
+    lib.fnr_backproject_select.argtypes = [vp, vp, vp, vp, vp, i32, i32, _f32p, _f32p, i32, vp, vp, vp, vp, vp]
     if lib.fnr_version() != ABI_VERSION:
         raise FruitNerfNativeError(f"ABI version mismatch: library reports {lib.fnr_version()}")
     _lib = lib

@@ -13,6 +13,8 @@
 // scikit-learn's KD-tree radius predicate bit for bit.  No host synchronisation; data-dependent sizes (cells, voxels,
 // clusters) stay in device memory.
 #include <cub/cub.cuh>
+#include <math_constants.h>
+#include <algorithm>
 #include <cmath>
 #include "fnr_common.cuh"
 #include "fnr_kernels.h"
@@ -352,6 +354,362 @@ __global__ void __launch_bounds__(kThreads) cluster_sums_kernel(const double* __
   }
 }
 
+// ---- k nearest neighbours -------------------------------------------------------------------------------------------
+// The point-cloud export's statistical outlier removal (k = 20) and normal estimation (k = 30): open3d's KD-tree kNN,
+// exact.  A query walks Chebyshev rings of cells outward and keeps its k best (distance^2, input index) pairs, ordered
+// by that pair, so ties go to the smaller index and every run gives the same list.
+constexpr int kMaxK = 32;
+constexpr int kKnnThreads = 128;
+constexpr int kRingCap = 4;           // rings walked before a query moves to the exhaustive pass
+constexpr double kRingMargin = 0.25;  // cells; key rounding moves a point by less than 2^-11 of a cell (check_extent)
+
+// Calls f(cell) for every occupied cell at Chebyshev distance exactly `ring` from `key`: the side columns of the ring
+// whole (one z range), the inner columns at their two z caps only (two one-cell ranges).  f has one call site, so the
+// per-point work it inlines exists once.
+template <class F>
+__device__ __forceinline__ void for_each_cell_in_ring(const Grid& g, int nc, uint64_t key, int ring, F&& f) {
+  const long long cx = (long long)(key >> (2 * kAxisBits)), cy = (long long)((key >> kAxisBits) & kAxisMask),
+                  cz = (long long)(key & kAxisMask);
+#pragma unroll 1
+  for (int dx = -ring; dx <= ring; ++dx) {
+    const long long x = cx + dx;
+    if (x < 0 || x >= kAxisCells) continue;
+#pragma unroll 1
+    for (int dy = -ring; dy <= ring; ++dy) {
+      const long long y = cy + dy;
+      if (y < 0 || y >= kAxisCells) continue;
+      const bool side = max(abs(dx), abs(dy)) == ring;
+#pragma unroll 1
+      for (int part = 0; part < (side ? 1 : 2); ++part) {
+        long long zlo = part == 0 ? cz - ring : cz + ring;
+        long long zhi = side ? cz + ring : zlo;
+        if (zhi < 0 || zlo >= kAxisCells) continue;
+        zlo = zlo < 0 ? 0 : zlo;
+        zhi = zhi >= kAxisCells ? kAxisCells - 1 : zhi;
+        const uint64_t hi = pack_key(x, y, zhi);
+#pragma unroll 1
+        for (int c = lower_bound(g.ukeys, nc, pack_key(x, y, zlo)); c < nc && g.ukeys[c] <= hi; ++c) f(c);
+      }
+    }
+  }
+}
+
+__device__ __forceinline__ bool knn_less(double a, int ai, double b, int bi) { return a < b || (a == b && ai < bi); }
+
+// The k best pairs in ascending order; entries k.. stay (+inf, kNone).  All indexing is static after unrolling, so the
+// list lives in registers.
+struct KnnList {
+  double d[kMaxK];
+  int i[kMaxK];
+  double wd;  // the k-th entry, (+inf, kNone) until k pairs are in
+  int wi;
+
+  __device__ __forceinline__ void init() {
+#pragma unroll
+    for (int t = 0; t < kMaxK; ++t) {
+      d[t] = CUDART_INF;
+      i[t] = kNone;
+    }
+    wd = CUDART_INF;
+    wi = kNone;
+  }
+
+  __device__ __forceinline__ void insert(int k, double nd, int ni) {
+    if (!knn_less(nd, ni, wd, wi)) return;
+#pragma unroll
+    for (int t = kMaxK - 1; t > 0; --t) {  // descending: slot t reads the untouched slot t - 1
+      if (t < k) {
+        if (knn_less(nd, ni, d[t - 1], i[t - 1])) {
+          d[t] = d[t - 1];
+          i[t] = i[t - 1];
+        } else if (knn_less(nd, ni, d[t], i[t])) {
+          d[t] = nd;
+          i[t] = ni;
+        }
+      }
+    }
+    if (knn_less(nd, ni, d[0], i[0])) {
+      d[0] = nd;
+      i[0] = ni;
+    }
+#pragma unroll
+    for (int t = 0; t < kMaxK; ++t)
+      if (t == k - 1) {
+        wd = d[t];
+        wi = i[t];
+      }
+  }
+};
+
+// Per-query result writers.  `i` is the input index of the query, L its k nearest neighbours (self included).
+struct MeanDistanceOut {
+  double* mean;
+  __device__ __forceinline__ void finish(int i, const KnnList& L, int k) const {
+    double s = 0.0;  // ascending, sequential: np.cumsum(d, axis=1)[:, -1]
+#pragma unroll
+    for (int t = 0; t < kMaxK; ++t)
+      if (t < k) s = __dadd_rn(s, __dsqrt_rn(L.d[t]));
+    mean[i] = __ddiv_rn(s, (double)k);
+  }
+};
+
+__device__ __forceinline__ void cross3(const double* a, const double* b, double* c) {
+  c[0] = a[1] * b[2] - a[2] * b[1];
+  c[1] = a[2] * b[0] - a[0] * b[2];
+  c[2] = a[0] * b[1] - a[1] * b[0];
+}
+
+// Direction of the null space of B - l*I for a symmetric 3x3 B (b = {b00, b01, b02, b11, b12, b22}): the largest cross
+// product of two of its rows.  Returns that product's squared length (~0 when l is a double eigenvalue).
+__device__ __forceinline__ double null_direction(const double* b, double l, double* v) {
+  const double r[3][3] = {{b[0] - l, b[1], b[2]}, {b[1], b[3] - l, b[4]}, {b[2], b[4], b[5] - l}};
+  double best = -1.0;
+  for (int a = 0; a < 3; ++a) {
+    double c[3];
+    cross3(r[a], r[(a + 1) % 3], c);
+    const double m = c[0] * c[0] + c[1] * c[1] + c[2] * c[2];
+    if (m > best) {
+      best = m;
+      v[0] = c[0];
+      v[1] = c[1];
+      v[2] = c[2];
+    }
+  }
+  return best;
+}
+
+// Unit eigenvector of the smallest eigenvalue of a symmetric 3x3 matrix (closed-form eigenvalues, then a null vector by
+// cross products).  When the smallest eigenvalue is (numerically) double, every unit vector orthogonal to the largest
+// eigenvalue's eigenvector is an answer, and one of them is returned.  The zero matrix and a multiple of the identity
+// give (0, 0, 1).
+__device__ __forceinline__ void smallest_eigenvector(const double* a, double* n) {
+  n[0] = 0.0;
+  n[1] = 0.0;
+  n[2] = 1.0;
+  double s = 0.0;
+  for (int t = 0; t < 6; ++t) s = fmax(s, fabs(a[t]));
+  if (!(s > 0.0)) return;
+  double b[6];
+  for (int t = 0; t < 6; ++t) b[t] = a[t] / s;
+  const double q = (b[0] + b[3] + b[5]) / 3.0;
+  const double p1 = b[1] * b[1] + b[2] * b[2] + b[4] * b[4];
+  const double p2 = (b[0] - q) * (b[0] - q) + (b[3] - q) * (b[3] - q) + (b[5] - q) * (b[5] - q) + 2.0 * p1;
+  if (!(p2 > 0.0)) return;
+  const double p = sqrt(p2 / 6.0);
+  const double c0 = (b[0] - q) / p, c1 = b[1] / p, c2 = b[2] / p, c3 = (b[3] - q) / p, c4 = b[4] / p, c5 = (b[5] - q) / p;
+  const double det = c0 * (c3 * c5 - c4 * c4) - c1 * (c1 * c5 - c4 * c2) + c2 * (c1 * c4 - c3 * c2);
+  const double r = fmin(1.0, fmax(-1.0, det / 2.0));
+  const double phi = acos(r) / 3.0;
+  const double l1 = q + 2.0 * p * cos(phi);                          // largest
+  const double l3 = q + 2.0 * p * cos(phi + 2.0 * CUDART_PI / 3.0);  // smallest
+  double v[3];
+  if (!(null_direction(b, l3, v) > 1e-28)) {
+    double u[3];
+    if (!(null_direction(b, l1, u) > 1e-28)) return;
+    if (fabs(u[0]) > fabs(u[1])) {
+      v[0] = -u[2];
+      v[1] = 0.0;
+      v[2] = u[0];
+    } else {
+      v[0] = 0.0;
+      v[1] = u[2];
+      v[2] = -u[1];
+    }
+  }
+  const double len = sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+  if (!(len > 0.0)) return;
+  n[0] = v[0] / len;
+  n[1] = v[1] / len;
+  n[2] = v[2] / len;
+}
+
+// open3d EstimateNormals on the k nearest neighbours: fewer than 3 -> (0, 0, 1); else the smallest-eigenvalue
+// eigenvector of their covariance (two passes: the mean, then the centred products).  With view directions, a normal
+// whose fp32 dot product with its point's view direction is positive is flipped.
+struct NormalsOut {
+  const double* pts;  // input order
+  const float* view;  // [n,3] or NULL
+  double* normals;
+  __device__ __forceinline__ void finish(int i, const KnnList& L, int k) const {
+    double n[3] = {0.0, 0.0, 1.0};
+    if (k >= 3) {
+      double m[3] = {0.0, 0.0, 0.0};
+#pragma unroll
+      for (int t = 0; t < kMaxK; ++t)
+        if (t < k) {
+          const double* q = pts + 3 * (size_t)L.i[t];
+          m[0] += q[0];
+          m[1] += q[1];
+          m[2] += q[2];
+        }
+      for (int a = 0; a < 3; ++a) m[a] /= (double)k;
+      double c[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};  // c00 c01 c02 c11 c12 c22
+#pragma unroll
+      for (int t = 0; t < kMaxK; ++t)
+        if (t < k) {
+          const double* q = pts + 3 * (size_t)L.i[t];
+          const double x = q[0] - m[0], y = q[1] - m[1], z = q[2] - m[2];
+          c[0] += x * x;
+          c[1] += x * y;
+          c[2] += x * z;
+          c[3] += y * y;
+          c[4] += y * z;
+          c[5] += z * z;
+        }
+      for (int a = 0; a < 6; ++a) c[a] /= (double)k;
+      smallest_eigenvector(c, n);
+    }
+    if (view) {
+      const float* v = view + 3 * (size_t)i;
+      const float dot = __fadd_rn(__fadd_rn(__fmul_rn(v[0], __double2float_rn(n[0])), __fmul_rn(v[1], __double2float_rn(n[1]))),
+                                  __fmul_rn(v[2], __double2float_rn(n[2])));
+      if (dot > 0.0f) {
+        n[0] = -n[0];
+        n[1] = -n[1];
+        n[2] = -n[2];
+      }
+    }
+    double* o = normals + 3 * (size_t)i;
+    o[0] = n[0];
+    o[1] = n[1];
+    o[2] = n[2];
+  }
+};
+
+// One thread per query, in sorted order so a warp walks neighbouring cells.  After ring R every point not yet seen is
+// at least (R - kRingMargin) * h away; the walk stops once the k-th distance is below that (or every point was seen).
+// A query still open after kRingCap rings is queued for knn_exhaustive_kernel.
+template <class Out>
+__global__ void __launch_bounds__(kKnnThreads) knn_kernel(Grid g, int k, double h, Out out, int* __restrict__ open,
+                                                          int* __restrict__ num_open) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= g.n) return;
+  const int nc = *g.ncells;
+  const double px = g.x[j], py = g.y[j], pz = g.z[j];
+  const uint64_t key = g.keys[j];
+  KnnList L;
+  L.init();
+  int seen = 0;
+#pragma unroll 1
+  for (int ring = 0; ring <= kRingCap; ++ring) {
+    for_each_cell_in_ring(g, nc, key, ring, [&](int c) {
+      const int b = g.cstart[c], e = g.cstart[c + 1];
+      seen += e - b;
+#pragma unroll 1
+      for (int m = b; m < e; ++m) L.insert(k, dist2(px, py, pz, g.x[m], g.y[m], g.z[m]), g.perm[m]);
+    });
+    const double bound = (ring - kRingMargin) * h;
+    if (seen == g.n || (ring > 0 && L.wd < bound * bound * (1.0 - 1e-9))) {
+      out.finish(g.perm[j], L, k);
+      return;
+    }
+  }
+  open[atomicAdd(num_open, 1)] = j;
+}
+
+// Exact pass for the queued queries, one block each: every thread keeps the best k of a strided share of all points,
+// then k rounds of a block-wide minimum over the list heads merge them.
+template <class Out>
+__global__ void __launch_bounds__(kKnnThreads) knn_exhaustive_kernel(Grid g, int k, Out out, const int* __restrict__ open,
+                                                                     const int* __restrict__ num_open) {
+  __shared__ double sd[kKnnThreads];
+  __shared__ int si[kKnnThreads], st[kKnnThreads];
+  __shared__ double rd[kMaxK];
+  __shared__ int ri[kMaxK];
+  const int t = threadIdx.x;
+  const int total = *num_open;
+  for (int q = blockIdx.x; q < total; q += gridDim.x) {
+    const int j = open[q];
+    const double px = g.x[j], py = g.y[j], pz = g.z[j];
+    KnnList L;
+    L.init();
+#pragma unroll 1
+    for (int m = t; m < g.n; m += kKnnThreads) L.insert(k, dist2(px, py, pz, g.x[m], g.y[m], g.z[m]), g.perm[m]);
+    int head = 0;
+    for (int r = 0; r < k; ++r) {
+      double hd = CUDART_INF;
+      int hi = kNone;
+#pragma unroll
+      for (int u = 0; u < kMaxK; ++u)
+        if (u == head) {
+          hd = L.d[u];
+          hi = L.i[u];
+        }
+      sd[t] = hd;
+      si[t] = hi;
+      st[t] = t;
+      __syncthreads();
+      for (int w = kKnnThreads / 2; w > 0; w >>= 1) {
+        if (t < w && knn_less(sd[t + w], si[t + w], sd[t], si[t])) {
+          sd[t] = sd[t + w];
+          si[t] = si[t + w];
+          st[t] = st[t + w];
+        }
+        __syncthreads();
+      }
+      if (t == st[0]) ++head;
+      if (t == 0) {
+        rd[r] = sd[0];
+        ri[r] = si[0];
+      }
+      __syncthreads();
+    }
+    if (t == 0) {
+#pragma unroll
+      for (int u = 0; u < kMaxK; ++u)
+        if (u < k) {
+          L.d[u] = rd[u];
+          L.i[u] = ri[u];
+        }
+      out.finish(g.perm[j], L, k);
+    }
+    __syncthreads();
+  }
+}
+
+// ---- back-projection of rendered rays ---------------------------------------------------------------------------------
+constexpr int kSelectThreads = 1024;
+
+// point = origin + direction * depth (fp32, multiply then add, no FMA); keep accumulation > 0.5 and, with the box, every
+// coordinate strictly inside it.  One block walks the batch in ray order and appends the kept rays at *count, so the
+// rows come out in ray order; rows at or beyond `capacity` are counted but not written.
+__global__ void __launch_bounds__(kSelectThreads) backproject_select_kernel(
+    const float* __restrict__ origins, const float* __restrict__ directions, const float* __restrict__ depth,
+    const float* __restrict__ rgb, const float* __restrict__ accumulation, int R, int use_box, float3 bmin, float3 bmax,
+    int capacity, float* __restrict__ points, float* __restrict__ colors, float* __restrict__ view_dirs, int* __restrict__ count) {
+  using Scan = cub::BlockScan<int, kSelectThreads>;
+  __shared__ typename Scan::TempStorage tmp;
+  __shared__ int base;
+  if (threadIdx.x == 0) base = *count;
+  __syncthreads();
+  for (int r0 = 0; r0 < R; r0 += kSelectThreads) {
+    const int r = r0 + threadIdx.x;
+    float p[3];
+    int keep = 0;
+    if (r < R) {
+      const float t = depth[r];
+      for (int a = 0; a < 3; ++a) p[a] = __fadd_rn(origins[3 * (size_t)r + a], __fmul_rn(directions[3 * (size_t)r + a], t));
+      keep = accumulation[r] > 0.5f;
+      if (use_box)
+        keep = keep && p[0] > bmin.x && p[1] > bmin.y && p[2] > bmin.z && p[0] < bmax.x && p[1] < bmax.y && p[2] < bmax.z;
+    }
+    int pos, kept;
+    Scan(tmp).ExclusiveSum(keep, pos, kept);
+    if (keep && base + pos < capacity) {
+      const size_t row = 3 * (size_t)(base + pos);
+      for (int a = 0; a < 3; ++a) {
+        points[row + a] = p[a];
+        colors[row + a] = rgb[3 * (size_t)r + a];
+        view_dirs[row + a] = directions[3 * (size_t)r + a];
+      }
+    }
+    __syncthreads();  // every thread has read `base` and `tmp`
+    if (threadIdx.x == 0) base += kept;
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *count = base;
+}
+
 // ---- host side ------------------------------------------------------------------------------------------------------
 int blocks_for(long long n) { return (int)((n + kThreads - 1) / kThreads); }
 
@@ -492,6 +850,56 @@ int build_grid(const double* pts, int n, const double* lo, double h, const Scrat
 
 double cell_side(double r) { return kCellShrink * r / std::sqrt(3.0); }
 
+// Cell side of the kNN grid, from n, k and the bounds alone (no device read-back): the side at which k points would
+// share a cell if the n points filled the bounding box evenly, taken over the box itself and over its largest face and
+// longest edge (the largest of the three, so flat and thin clouds get cells sized for their own dimension).  It is then
+// raised to the smallest side the keys allow: at most 2^21 - 1 cells per axis and 2^39 cells from the origin.  The
+// rule sets the cost of a query, never its result.
+double knn_cell_side(int n, int k, const double* lo, const double* hi) {
+  double e[3] = {hi[0] - lo[0], hi[1] - lo[1], hi[2] - lo[2]};
+  std::sort(e, e + 3, [](double a, double b) { return a > b; });
+  double h = 0.0, prod = 1.0;
+  for (int d = 1; d <= 3; ++d) {
+    prod *= e[d - 1];
+    if (prod > 0.0) h = std::fmax(h, std::pow(prod * k / n, 1.0 / d));
+  }
+  for (int a = 0; a < 3; ++a) {
+    h = std::fmax(h, (hi[a] - lo[a]) / (double)(kAxisCells - 2));
+    h = std::fmax(h, std::fmax(std::fabs(lo[a]), std::fabs(hi[a])) / (kMaxCoordOverCell / 2.0));
+  }
+  return h > 0.0 && std::isfinite(h) ? h : 1.0;  // all points identical: one cell
+}
+
+template <class Out>
+int run_knn(const char* what, const double* points, int64_t num_points, const double* lo, const double* hi, int32_t k, bool out_ok,
+            const Out& out, void* scratch, size_t scratch_bytes, void* stream) {
+  if (int rc = check_points(what, points, num_points, lo, hi)) return rc;
+  if (k < 1 || (num_points > 0 && !out_ok)) {
+    set_error("%s: k must be >= 1 and the output non-NULL (k %d)", what, k);
+    return FNR_ERR_INVALID_ARGUMENT;
+  }
+  if (k > kMaxK) {
+    set_error("%s: k = %d neighbours; at most %d are supported", what, k, kMaxK);
+    return FNR_ERR_UNSUPPORTED;
+  }
+  const int n = (int)num_points;
+  if (n == 0) return FNR_OK;
+  const int kk = std::min(k, n);
+  const double h = knn_cell_side(n, kk, lo, hi);
+  if (int rc = check_extent(what, "kNN cell side", h, h, lo, hi)) return rc;
+  Scratch s;
+  if (int rc = bind_scratch(what, n, scratch, scratch_bytes, &s)) return rc;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  Grid g;
+  if (int rc = build_grid(points, n, lo, h, s, st, &g)) return rc;
+  // the DBSCAN regions are free here: `core` holds the queue of open queries, `cmin[0]` its length
+  if (int rc = check_cuda(cudaMemsetAsync(s.cmin, 0, sizeof(int), st), "kNN queue reset")) return rc;
+  knn_kernel<Out><<<(n + kKnnThreads - 1) / kKnnThreads, kKnnThreads, 0, st>>>(g, kk, h, out, s.core, s.cmin);
+  if (int rc = check_launch("knn_kernel")) return rc;
+  knn_exhaustive_kernel<Out><<<std::min(n, 4 * sm_count()), kKnnThreads, 0, st>>>(g, kk, out, s.core, s.cmin);
+  return check_launch("knn_exhaustive_kernel");
+}
+
 }  // namespace
 
 }  // namespace fnr
@@ -629,6 +1037,36 @@ int fnr_cluster_sums(const double* points, const int32_t* labels, int64_t num_po
   if (int rc = check_launch("segment_bounds_kernel")) return rc;
   cluster_sums_kernel<<<std::min(K, 8 * sm_count()), kThreads, 0, st>>>(points, s.perm, s.cstart, s.cell_of, K, sums, counts);
   return check_launch("cluster_sums_kernel");
+}
+
+int fnr_knn_mean_distance(const double* points, int64_t num_points, const double* lo, const double* hi, int32_t k, double* mean_dist,
+                          void* scratch, size_t scratch_bytes, void* stream) {
+  return run_knn("fnr_knn_mean_distance", points, num_points, lo, hi, k, mean_dist != nullptr, MeanDistanceOut{mean_dist}, scratch,
+                 scratch_bytes, stream);
+}
+
+int fnr_estimate_normals(const double* points, int64_t num_points, const double* lo, const double* hi, int32_t k, const float* view_dirs,
+                         double* normals, void* scratch, size_t scratch_bytes, void* stream) {
+  return run_knn("fnr_estimate_normals", points, num_points, lo, hi, k, normals != nullptr, NormalsOut{points, view_dirs, normals},
+                 scratch, scratch_bytes, stream);
+}
+
+int fnr_backproject_select(const float* origins, const float* directions, const float* depth, const float* rgb, const float* accumulation,
+                           int32_t num_rays, int32_t use_bounding_box, const float* box_min, const float* box_max, int32_t capacity,
+                           float* points, float* colors, float* view_dirs, int32_t* count, void* stream) {
+  const char* what = "fnr_backproject_select";
+  if (num_rays < 0 || capacity < 0 || !count || (use_bounding_box && (!box_min || !box_max)) ||
+      (num_rays > 0 && (!origins || !directions || !depth || !rgb || !accumulation)) ||
+      (capacity > 0 && (!points || !colors || !view_dirs))) {
+    set_error("%s: invalid arguments (rays %d, capacity %d)", what, num_rays, capacity);
+    return FNR_ERR_INVALID_ARGUMENT;
+  }
+  if (num_rays == 0) return FNR_OK;
+  const float3 bmin = use_bounding_box ? make_float3(box_min[0], box_min[1], box_min[2]) : make_float3(0.f, 0.f, 0.f);
+  const float3 bmax = use_bounding_box ? make_float3(box_max[0], box_max[1], box_max[2]) : make_float3(0.f, 0.f, 0.f);
+  backproject_select_kernel<<<1, kSelectThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      origins, directions, depth, rgb, accumulation, num_rays, use_bounding_box ? 1 : 0, bmin, bmax, capacity, points, colors, view_dirs, count);
+  return check_launch("backproject_select_kernel");
 }
 
 }  // extern "C"

@@ -106,19 +106,82 @@ def sample_volume(pipeline, num_points: int, output_dir: Optional[pathlib.Path] 
     return out
 
 
-def write_ply(path, points: np.ndarray, colors: np.ndarray) -> None:
-    """Binary little-endian PLY with double xyz and uchar rgb -- what open3d's write_point_cloud
-    produces for a coloured cloud (fruit_nerf/scripts/exporter.py:116-119)."""
+MAX_EMPTY_BATCHES = 100  # consecutive batches without a kept ray after which generate_point_cloud gives up
+
+
+def generate_point_cloud(pipeline, num_points: int = 1000000, remove_outliers: bool = True, reorient_normals: bool = True,
+                         estimate_normals: bool = False, rgb_output_name: str = "rgb", depth_output_name: str = "depth",
+                         normal_output_name: Optional[str] = None, use_bounding_box: bool = True,
+                         bounding_box_min=(-1.0, -1.0, -1.0), bounding_box_max=(1.0, 1.0, 1.0), std_ratio: float = 10.0) -> Dict:
+    """nerfstudio exporter_utils.generate_point_cloud (0.3.2) on the GPU.  Renders training-ray batches until at least
+    ``num_points`` rays are kept (the last batch whole), back-projects each ray's median depth, keeps rays with
+    accumulation > 0.5 (and, with the box, points strictly inside it), then optionally removes statistical outliers
+    (20 neighbours, ``std_ratio``), estimates normals (30 neighbours) and flips them against the view direction.
+    Returns {'points' [N,3], 'colors' [N,3], 'normals' [N,3] or None}, float64 numpy, in the dataparser frame.
+
+    Unlike the reference, which loops forever when no ray survives, this raises RuntimeError after
+    ``MAX_EMPTY_BATCHES`` consecutive batches that keep nothing."""
+    from .. import pointcloud
+
+    if normal_output_name is not None:
+        raise ValueError(f"normal output '{normal_output_name}': FruitModel renders no normals; estimate them from the cloud")
+    if use_bounding_box and not all(lo < hi for lo, hi in zip(bounding_box_min, bounding_box_max)):
+        raise ValueError("Bounding box min must be smaller than max")
+    model, dm = pipeline.model, pipeline.datamanager
+    dev = next(model.parameters()).device
+    buffers = ops.PointBuffers(max(0, num_points) + dm.config.train_num_rays_per_batch, dev)
+    box = (bounding_box_min, bounding_box_max) if use_bounding_box else None
+    count = empty = 0
+    with torch.no_grad():
+        while count < num_points:
+            ray_bundle, _ = dm.next_train(0)
+            outputs = model(ray_bundle)
+            rgba = model.get_rgba_image(outputs, rgb_output_name)
+            ops.backproject_select(ray_bundle.origins, ray_bundle.directions, outputs[depth_output_name], rgba[..., :3], rgba[..., 3],
+                                   buffers, box)
+            kept = int(buffers.count.item())  # the one host read per batch
+            if kept > buffers.capacity:
+                raise RuntimeError(f"point buffer of {buffers.capacity} rows overflowed ({kept}): the ray batch size changed")
+            empty = empty + 1 if kept == count else 0
+            if empty >= MAX_EMPTY_BATCHES:
+                raise RuntimeError(f"no ray was kept in {MAX_EMPTY_BATCHES} consecutive batches ({count} points so far): "
+                                   "check the bounding box and the trained model")
+            count = kept
+        points = buffers.points[:count].double()
+        colors = buffers.colors[:count]
+        view_dirs = buffers.view_dirs[:count]
+        if remove_outliers:
+            points, ind = pointcloud.remove_statistical_outliers(points, 20, std_ratio, return_index=True)
+            colors, view_dirs = colors[ind], view_dirs[ind]
+        normals = None
+        if estimate_normals:
+            normals = pointcloud.estimate_normals(points, 30, view_dirs if reorient_normals else None)
+            if reorient_normals:
+                normals = normals.float().double()  # the reference reorients fp32 normals and stores them back
+    return {"points": points.cpu().numpy(), "colors": colors.double().cpu().numpy(),
+            "normals": None if normals is None else normals.cpu().numpy()}
+
+
+def write_ply(path,points: np.ndarray, colors: np.ndarray, normals: Optional[np.ndarray] = None) -> None:
+    """Binary little-endian PLY with double xyz, double nx/ny/nz when ``normals`` is given, and uchar rgb -- what
+    open3d's write_point_cloud produces for a coloured cloud (fruit_nerf/scripts/exporter.py:116-119)."""
     pts = np.asarray(points, dtype="<f8")
     col = np.clip(np.asarray(colors, dtype=np.float64) * 255.0, 0, 255).astype(np.uint8)
     n = pts.shape[0]
+    normal_props = "property double nx\nproperty double ny\nproperty double nz\n" if normals is not None else ""
     header = (
         "ply\nformat binary_little_endian 1.0\ncomment fruitnerf_b200 export\n"
-        f"element vertex {n}\nproperty double x\nproperty double y\nproperty double z\n"
+        f"element vertex {n}\nproperty double x\nproperty double y\nproperty double z\n{normal_props}"
         "property uchar red\nproperty uchar green\nproperty uchar blue\nend_header\n"
     )
-    rec = np.empty(n, dtype=[("x", "<f8"), ("y", "<f8"), ("z", "<f8"), ("r", "u1"), ("g", "u1"), ("b", "u1")])
+    fields = [("x", "<f8"), ("y", "<f8"), ("z", "<f8")]
+    if normals is not None:
+        fields += [("nx", "<f8"), ("ny", "<f8"), ("nz", "<f8")]
+    rec = np.empty(n, dtype=fields + [("r", "u1"), ("g", "u1"), ("b", "u1")])
     rec["x"], rec["y"], rec["z"] = pts[:, 0], pts[:, 1], pts[:, 2]
+    if normals is not None:
+        nrm = np.asarray(normals, dtype="<f8")
+        rec["nx"], rec["ny"], rec["nz"] = nrm[:, 0], nrm[:, 1], nrm[:, 2]
     rec["r"], rec["g"], rec["b"] = col[:, 0], col[:, 1], col[:, 2]
     pathlib.Path(path).parent.mkdir(parents=True, exist_ok=True)
     with open(path, "wb") as f:

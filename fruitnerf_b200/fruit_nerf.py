@@ -245,6 +245,17 @@ class FruitModel(nn.Module):
 
     get_inference_outputs = get_outputs
 
+    def get_rgba_image(self, outputs: Dict[str, Tensor], output_name: str = "rgb") -> Tensor:
+        """nerfstudio Model.get_rgba_image for the "last_sample" background FruitModel renders with: the colour and the
+        accumulation of each ray side by side, [..., 4]."""
+        accumulation_name = output_name.replace("rgb", "accumulation")
+        if output_name not in outputs or accumulation_name not in outputs:
+            raise NotImplementedError(f"get_rgba_image needs '{output_name}' and '{accumulation_name}' among the outputs")
+        rgb, acc = outputs[output_name], outputs[accumulation_name]
+        if acc.dim() < rgb.dim():
+            acc = acc.unsqueeze(-1)
+        return torch.cat((rgb, acc), dim=-1)
+
     def get_export_outputs(self, ray_bundle: RayBundle, buffers: Optional[ops.ExportBuffers] = None, point_base: int = 0,
                            dense: bool = True):
         """fruit_nerf.py:251-269: uniform bins -> field (aabb-normalised, mean appearance) ->

@@ -643,3 +643,68 @@ def cluster_sums(points: Tensor, labels: Tensor, num_clusters: int) -> Tuple[Ten
     L.check(L.load().fnr_cluster_sums(_ptr(pts), _ptr(labels), n, int(num_clusters), _ptr(sums), _ptr(counts), _ptr(scratch),
                                       scratch.numel(), _stream(dev)))
     return sums, counts
+
+
+# ======================================================================================================
+# The `pointcloud` export (fnr_cluster.cu; nerfstudio ExportPointCloud / generate_point_cloud)
+# ======================================================================================================
+def knn_mean_distance(points: Tensor, k: int) -> Tensor:
+    """fp64 [n]: mean Euclidean distance to the min(k, n) nearest neighbours, the point itself included, summed in
+    ascending order (open3d remove_statistical_outlier's per-point statistic)."""
+    pts = cluster_points(points)
+    n, dev = pts.shape[0], pts.device
+    out = torch.empty(n, dtype=torch.float64, device=dev)
+    lo, hi = _bounds(pts)
+    scratch = _cluster_scratch(n, dev)
+    L.check(L.load().fnr_knn_mean_distance(_ptr(pts), n, lo, hi, int(k), _ptr(out), _ptr(scratch), scratch.numel(), _stream(dev)))
+    return out
+
+
+def estimate_normals(points: Tensor, k: int, view_dirs: Optional[Tensor] = None) -> Tensor:
+    """fp64 [n,3] unit normals from the min(k, n) nearest neighbours (open3d estimate_normals with KNN(k)); with
+    ``view_dirs`` [n,3], normals facing along their view direction (fp32 dot product > 0) are flipped."""
+    pts = cluster_points(points)
+    n, dev = pts.shape[0], pts.device
+    if view_dirs is not None:
+        _require_cuda(view_dirs)
+        view_dirs = _f32c(view_dirs.detach().reshape(-1, 3))
+        if view_dirs.shape[0] != n:
+            raise ValueError(f"{view_dirs.shape[0]} view directions for {n} points")
+    out = torch.empty((n, 3), dtype=torch.float64, device=dev)
+    lo, hi = _bounds(pts)
+    scratch = _cluster_scratch(n, dev)
+    L.check(L.load().fnr_estimate_normals(_ptr(pts), n, lo, hi, int(k), _ptr(view_dirs), _ptr(out), _ptr(scratch), scratch.numel(),
+                                          _stream(dev)))
+    return out
+
+
+class PointBuffers:
+    """Device rows a point-cloud export appends to: xyz, rgb and view direction ([capacity,3] fp32 each) and the
+    running row count (a device int32)."""
+
+    def __init__(self, capacity: int, device):
+        f32 = dict(dtype=torch.float32, device=device)
+        self.capacity = capacity
+        self.points = torch.empty((capacity, 3), **f32)
+        self.colors = torch.empty((capacity, 3), **f32)
+        self.view_dirs = torch.empty((capacity, 3), **f32)
+        self.count = torch.zeros(1, dtype=torch.int32, device=device)
+
+
+def backproject_select(origins: Tensor, directions: Tensor, depth: Tensor, rgb: Tensor, accumulation: Tensor, buffers: PointBuffers,
+                       bounding_box=None) -> None:
+    """Appends the rays of one rendered batch with accumulation > 0.5 (and, with ``bounding_box`` = (min xyz, max xyz),
+    their point strictly inside it) to ``buffers`` in ray order: point = origin + direction * depth in fp32."""
+    dev = _require_cuda(origins, directions, depth, rgb, accumulation)
+    R = origins.reshape(-1, 3).shape[0]
+    o, d, c = (_f32c(t.detach().reshape(-1, 3)) for t in (origins, directions, rgb))
+    t, a = (_f32c(x.detach().reshape(-1)) for x in (depth, accumulation))
+    if not (d.shape[0] == c.shape[0] == t.shape[0] == a.shape[0] == R):
+        raise ValueError("origins, directions, depth, rgb and accumulation must describe the same rays")
+    bmin = bmax = None
+    if bounding_box is not None:
+        bmin = (C.c_float * 3)(*[float(v) for v in bounding_box[0]])
+        bmax = (C.c_float * 3)(*[float(v) for v in bounding_box[1]])
+    L.check(L.load().fnr_backproject_select(_ptr(o), _ptr(d), _ptr(t), _ptr(c), _ptr(a), R, int(bounding_box is not None), bmin, bmax,
+                                            buffers.capacity, _ptr(buffers.points), _ptr(buffers.colors), _ptr(buffers.view_dirs),
+                                            _ptr(buffers.count), _stream(dev)))

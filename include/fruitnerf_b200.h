@@ -38,6 +38,9 @@
  *   fnr_radius_count, fnr_voxel_down_sample, fnr_dbscan, fnr_cluster_sums
  *                        stages 1-2 of the fruit counting (clustering/clustering_base.py:138-143, 183-259):
  *                        radius-outlier removal, voxel down-sampling, DBSCAN, the sums of the centre merge
+ *   fnr_backproject_select, fnr_knn_mean_distance, fnr_estimate_normals
+ *                        the `pointcloud` export (fruit_nerf/scripts/exporter.py:124-129, nerfstudio ExportPointCloud):
+ *                        back-projection and selection of rendered rays, statistical outlier removal, normal estimation
  */
 #ifndef FRUITNERF_B200_H
 #define FRUITNERF_B200_H
@@ -378,6 +381,33 @@ int fnr_dbscan(const double* points, int64_t num_points, const double* lo, const
  * inputs of the centre merge (clustering_base.py:209-259).  Deterministic: the same input gives the same bits. */
 int fnr_cluster_sums(const double* points, const int32_t* labels, int64_t num_points, int32_t num_clusters, double* sums,
                      int32_t* counts, void* scratch, size_t scratch_bytes, void* stream);
+
+/* ---- the RGB surface cloud export (nerfstudio ExportPointCloud / generate_point_cloud as the reference CLI's
+ * `pointcloud` subcommand runs it, fruit_nerf/scripts/exporter.py:124-129).  The k-nearest-neighbour calls take points,
+ * bounds and scratch as the fruit-counting calls above (fnr_cluster_scratch_bytes(n)).  Neighbours are exact: the
+ * min(k, n) points with the smallest fp64 distance, self included, ordered by (distance, input index).
+ * 1 <= k <= 32; a larger k returns FNR_ERR_UNSUPPORTED. ---- */
+
+/* mean_dist[i] = (sum of the Euclidean distances to the min(k, n) nearest neighbours of point i, added in ascending
+ * order) / min(k, n): the per-point statistic of open3d remove_statistical_outlier.  mean_dist: DEVICE [n] fp64. */
+int fnr_knn_mean_distance(const double* points, int64_t num_points, const double* lo, const double* hi, int32_t k, double* mean_dist,
+                          void* scratch, size_t scratch_bytes, void* stream);
+
+/* open3d estimate_normals with KNN(k): the unit eigenvector of the smallest eigenvalue of the (two-pass, fp64) covariance of
+ * the min(k, n) nearest neighbours; (0, 0, 1) with fewer than 3 neighbours or a zero covariance.  The sign is the solver's.
+ * view_dirs: DEVICE [n,3] fp32 or NULL; when given, a normal whose fp32 dot product with view_dirs[i] is > 0 is flipped.
+ * normals: DEVICE [n,3] fp64. */
+int fnr_estimate_normals(const double* points, int64_t num_points, const double* lo, const double* hi, int32_t k, const float* view_dirs,
+                         double* normals, void* scratch, size_t scratch_bytes, void* stream);
+
+/* One rendered batch of generate_point_cloud: point = origin + direction * depth in fp32 (multiply, then add), kept when
+ * accumulation > 0.5 and, with use_bounding_box, box_min < point < box_max on every axis (box_min / box_max: HOST float[3]).
+ * Kept rays are appended in ray order at row *count of points / colors (rgb) / view_dirs (direction), all DEVICE [capacity,3]
+ * fp32; *count (DEVICE int32) is advanced by the number kept.  Rows at or beyond capacity are counted but not written.
+ * origins, directions, rgb: DEVICE [R,3]; depth, accumulation: DEVICE [R]; all fp32. */
+int fnr_backproject_select(const float* origins, const float* directions, const float* depth, const float* rgb, const float* accumulation,
+                           int32_t num_rays, int32_t use_bounding_box, const float* box_min, const float* box_max, int32_t capacity,
+                           float* points, float* colors, float* view_dirs, int32_t* count, void* stream);
 
 /* Hash-grid row indices (exact-integer parity hook): rows[N,L,8] in nerfstudio corner order for
  * the masked [0,1]^3 positions of the given samples; also writes positions[N,3] if non-NULL. */
