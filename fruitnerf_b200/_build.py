@@ -34,35 +34,41 @@ def _stale(target: Path, deps) -> bool:
     return any(Path(d).stat().st_mtime > t for d in deps)
 
 
-def build(force: bool = False, verbose: bool = False) -> Path:
+def build(force: bool = False, verbose: bool = False, defines=(), out_dir=None) -> Path:
+    """Build the library; ``defines`` (e.g. ``["FNR_BWD_PHASE_TIMERS"]``) are passed as -D flags, and a diagnostic build
+    with them should name its own ``out_dir`` for the objects and the library so that it never replaces the normal one."""
+    flags = [*NVCC_FLAGS, *(f"-D{d}" for d in defines)]
+    dest = Path(out_dir) if out_dir is not None else CSRC
+    dest.mkdir(parents=True, exist_ok=True)
+    lib, stamp = dest / LIB.name, dest / STAMP.name
     # objects built with other flags or sources (an older architecture, say) are stale whatever their mtimes
-    recipe = " ".join([*NVCC_FLAGS, *SOURCES])
-    if not STAMP.exists() or STAMP.read_text() != recipe:
+    recipe = " ".join([*flags, *SOURCES])
+    if not stamp.exists() or stamp.read_text() != recipe:
         force = True
     headers = list(CSRC.glob("*.cuh")) + list(CSRC.glob("*.h")) + [CSRC.parent.parent / "include" / "fruitnerf_b200.h"]
     objs = []
     procs = []
     for src in SOURCES:
-        obj = CSRC / (src[:-3] + ".o")
+        obj = dest / (src[:-3] + ".o")
         objs.append(obj)
         if force or _stale(obj, [CSRC / src, *headers]):
-            cmd = [_nvcc(), *NVCC_FLAGS, "-c", str(CSRC / src), "-o", str(obj)]
+            cmd = [_nvcc(), *flags, "-c", str(CSRC / src), "-o", str(obj)]
             if verbose:
                 cmd.insert(1, "-Xptxas=-v")
             procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
     for src, p in procs:
-        out, _ = p.communicate()
-        if verbose and out:
-            print(out)
+        log, _ = p.communicate()
+        if verbose and log:
+            print(log)
         if p.returncode != 0:
-            raise RuntimeError(f"nvcc failed on {src}:\n{out}")
-    if force or procs or _stale(LIB, objs):
-        cmd = [_nvcc(), "-shared", "-o", str(LIB), *map(str, objs), "-lcudart"]
+            raise RuntimeError(f"nvcc failed on {src}:\n{log}")
+    if force or procs or _stale(lib, objs):
+        cmd = [_nvcc(), "-shared", "-o", str(lib), *map(str, objs), "-lcudart"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}{r.stderr}")
-        STAMP.write_text(recipe)
-    return LIB
+        stamp.write_text(recipe)
+    return lib
 
 
 if __name__ == "__main__":

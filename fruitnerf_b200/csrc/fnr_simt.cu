@@ -181,6 +181,7 @@ struct Layers {
       wg::linear_dx<C::MAXW, C::MAXW, K, N>(dyn_smem(), W, dy, dxv);
     else
       linear_bwd_input<K, N>(W, dy, dxv);
+    FNR_PHASE(kPhDx);
   }
   template <int K, int N>
   static __device__ __forceinline__ void dw(float* sX, float* sY, const float (&x)[K], const float (&dy)[N], float* gW, float* gb) {
@@ -188,6 +189,7 @@ struct Layers {
       wg::weight_grad<K, N>(dyn_smem(), x, dy, gW, gb);
     else
       tile_weight_grad<K, N>(sX, sY, x, dy, gW, gb);
+    FNR_PHASE(kPhDw);
   }
 };
 
@@ -565,6 +567,10 @@ __device__ __forceinline__ void tile_weight_grad(float* __restrict__ sX, float* 
   }
 }
 
+#ifdef FNR_BWD_PHASE_TIMERS
+__device__ unsigned long long g_bwd_phase_cycles[kBwdPhases];
+#endif
+
 template <class C, bool TC>
 __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F, KParams P, KParams G, KRays Rr,
                                                                       KFieldBwd B) {
@@ -575,6 +581,10 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
   float* sY = smem + kThreads * TP;
   __shared__ float s_app[C::APP];
   block_mean_embedding(P, F.num_images, C::APP, F.appearance_mode, s_app);
+#ifdef FNR_BWD_PHASE_TIMERS
+  if (threadIdx.x < kBwdPhases) phase::cycles[threadIdx.x] = 0;
+  if (threadIdx.x == 0) phase::last = clock64();
+#endif
   const long long N = (long long)Rr.R * Rr.S;
   const long long tiles = (N + kThreads - 1) / kThreads;
   const int lane = threadIdx.x & 31;
@@ -606,44 +616,59 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
 #pragma unroll
     for (int i = 0; i < C::APP; ++i)
       appv[i] = (F.appearance_mode == FNR_APP_PER_CAMERA) ? __ldg(P.app_embedding + (size_t)cam * C::APP + i) : s_app[i];
-    Acts<C> a;
-    field_mlps<C, TC>(P, enc, d, appv, a);
-
     // upstream per-point grads (zero for padding threads)
     const float* pg = B.point_grads + 5 * (size_t)pc;
     const float vm = valid ? 1.f : 0.f;
     const float d_sigma = pg[0] * vm;
     const float d_rgb[3] = {pg[1] * vm, pg[2] * vm, pg[3] * vm};
     const float d_logit = pg[4] * vm;
+    FNR_PHASE(kPhLoad);
+
+    // The forward is recomputed branch by branch (the same layer calls as field_mlps, so the same values), and each
+    // branch is back-propagated right after its forward: only the base MLP's activations live across the whole tile.
+    float h1[C::BASE_H], out[C::BASE_OUT];
+    Lin::template fwd<C::ENC, C::BASE_H, true>(P.base_w[0], P.base_b[0], enc, h1);
+    Lin::template fwd<C::BASE_H, C::BASE_OUT, false>(P.base_w[1], P.base_b[1], h1, out);
+    float geo[C::GEO];
+#pragma unroll
+    for (int i = 0; i < C::GEO; ++i) geo[i] = out[1 + i];
+    FNR_PHASE(kPhRecompute);
 
     float d_geo[C::GEO];
 #pragma unroll
     for (int i = 0; i < C::GEO; ++i) d_geo[i] = 0.f;
 
-    // ---- semantic branch -------------------------------------------------------------------
+    // ---- semantic branch (its logit head is not needed: d_logit is the upstream gradient) ------------------------
     {
+      float z1[C::SEM_H], zo[C::SEM_OUT];
+      float z2[C::SEM_LAYERS == 3 ? C::SEM_H : 1];
+      Lin::template fwd<C::GEO, C::SEM_H, true>(P.sem_w[0], P.sem_b[0], geo, z1);
+      if constexpr (C::SEM_LAYERS == 3) {
+        Lin::template fwd<C::SEM_H, C::SEM_H, true>(P.sem_w[1], P.sem_b[1], z1, z2);
+        Lin::template fwd<C::SEM_H, C::SEM_OUT, false>(P.sem_w[2], P.sem_b[2], z2, zo);
+      } else {
+        Lin::template fwd<C::SEM_H, C::SEM_OUT, false>(P.sem_w[1], P.sem_b[1], z1, zo);
+      }
+      FNR_PHASE(kPhRecompute);
       float dlg[1] = {d_logit};
       float dzo[C::SEM_OUT];
       Lin::template dx<C::SEM_OUT, 1>(P.head_w, dlg, dzo);
-      Lin::template dw<C::SEM_OUT, 1>(sX, sY, a.zo, dlg, G.head_w, G.head_b);
-      float geo[C::GEO];
-#pragma unroll
-      for (int i = 0; i < C::GEO; ++i) geo[i] = a.out[1 + i];
+      Lin::template dw<C::SEM_OUT, 1>(sX, sY, zo, dlg, G.head_w, G.head_b);
       float dz1[C::SEM_H];
       if constexpr (C::SEM_LAYERS == 3) {
         float dz2[C::SEM_H];
         Lin::template dx<C::SEM_H, C::SEM_OUT>(P.sem_w[2], dzo, dz2);
-        Lin::template dw<C::SEM_H, C::SEM_OUT>(sX, sY, a.z2, dzo, G.sem_w[2], G.sem_b[2]);
+        Lin::template dw<C::SEM_H, C::SEM_OUT>(sX, sY, z2, dzo, G.sem_w[2], G.sem_b[2]);
 #pragma unroll
-        for (int i = 0; i < C::SEM_H; ++i) dz2[i] = a.z2[i] > 0.f ? dz2[i] : 0.f;
+        for (int i = 0; i < C::SEM_H; ++i) dz2[i] = z2[i] > 0.f ? dz2[i] : 0.f;
         Lin::template dx<C::SEM_H, C::SEM_H>(P.sem_w[1], dz2, dz1);
-        Lin::template dw<C::SEM_H, C::SEM_H>(sX, sY, a.z1, dz2, G.sem_w[1], G.sem_b[1]);
+        Lin::template dw<C::SEM_H, C::SEM_H>(sX, sY, z1, dz2, G.sem_w[1], G.sem_b[1]);
       } else {
         Lin::template dx<C::SEM_H, C::SEM_OUT>(P.sem_w[1], dzo, dz1);
-        Lin::template dw<C::SEM_H, C::SEM_OUT>(sX, sY, a.z1, dzo, G.sem_w[1], G.sem_b[1]);
+        Lin::template dw<C::SEM_H, C::SEM_OUT>(sX, sY, z1, dzo, G.sem_w[1], G.sem_b[1]);
       }
 #pragma unroll
-      for (int i = 0; i < C::SEM_H; ++i) dz1[i] = a.z1[i] > 0.f ? dz1[i] : 0.f;
+      for (int i = 0; i < C::SEM_H; ++i) dz1[i] = z1[i] > 0.f ? dz1[i] : 0.f;
       Lin::template dw<C::GEO, C::SEM_H>(sX, sY, geo, dz1, G.sem_w[0], G.sem_b[0]);
       if (F.pass_semantic_gradients) {
         float dg[C::GEO];
@@ -654,20 +679,35 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
     }
     // ---- colour branch ---------------------------------------------------------------------
     {
+      // cat[SH(dir), geo, appearance] -> MLP -> sigmoid (fruit_field.py:270-278)
+      float cin[C::COL_IN], c1[C::COL_H], c2[C::COL_H];
+      sh_degree4(d[0], d[1], d[2], cin);
+#pragma unroll
+      for (int i = 0; i < C::GEO; ++i) cin[C::SH + i] = geo[i];
+#pragma unroll
+      for (int i = 0; i < C::APP; ++i) cin[C::SH + C::GEO + i] = appv[i];
+      Lin::template fwd<C::COL_IN, C::COL_H, true>(P.col_w[0], P.col_b[0], cin, c1);
+      Lin::template fwd<C::COL_H, C::COL_H, true>(P.col_w[1], P.col_b[1], c1, c2);
+      float o3[3];
+      Lin::template fwd<C::COL_H, 3, false>(P.col_w[2], P.col_b[2], c2, o3);
+      FNR_PHASE(kPhRecompute);
       float do3[3];
 #pragma unroll
-      for (int i = 0; i < 3; ++i) do3[i] = d_rgb[i] * a.rgb[i] * (1.0f - a.rgb[i]);
+      for (int i = 0; i < 3; ++i) {
+        const float rgb = sigmoidf_(o3[i]);
+        do3[i] = d_rgb[i] * rgb * (1.0f - rgb);
+      }
       float dc2[C::COL_H], dc1[C::COL_H], dcin[C::COL_IN];
       Lin::template dx<C::COL_H, 3>(P.col_w[2], do3, dc2);
-      Lin::template dw<C::COL_H, 3>(sX, sY, a.c2, do3, G.col_w[2], G.col_b[2]);
+      Lin::template dw<C::COL_H, 3>(sX, sY, c2, do3, G.col_w[2], G.col_b[2]);
 #pragma unroll
-      for (int i = 0; i < C::COL_H; ++i) dc2[i] = a.c2[i] > 0.f ? dc2[i] : 0.f;
+      for (int i = 0; i < C::COL_H; ++i) dc2[i] = c2[i] > 0.f ? dc2[i] : 0.f;
       Lin::template dx<C::COL_H, C::COL_H>(P.col_w[1], dc2, dc1);
-      Lin::template dw<C::COL_H, C::COL_H>(sX, sY, a.c1, dc2, G.col_w[1], G.col_b[1]);
+      Lin::template dw<C::COL_H, C::COL_H>(sX, sY, c1, dc2, G.col_w[1], G.col_b[1]);
 #pragma unroll
-      for (int i = 0; i < C::COL_H; ++i) dc1[i] = a.c1[i] > 0.f ? dc1[i] : 0.f;
+      for (int i = 0; i < C::COL_H; ++i) dc1[i] = c1[i] > 0.f ? dc1[i] : 0.f;
       Lin::template dx<C::COL_IN, C::COL_H>(P.col_w[0], dc1, dcin);
-      Lin::template dw<C::COL_IN, C::COL_H>(sX, sY, a.cin, dc1, G.col_w[0], G.col_b[0]);
+      Lin::template dw<C::COL_IN, C::COL_H>(sX, sY, cin, dc1, G.col_w[0], G.col_b[0]);
 #pragma unroll
       for (int i = 0; i < C::GEO; ++i) d_geo[i] += dcin[C::SH + i];
       // appearance-embedding gradient (only the per-camera rows are parameters of the graph;
@@ -699,14 +739,14 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
     {
       float dout[C::BASE_OUT];
       // trunc_exp backward: g * exp(clamp(x, -15, 15)); density = exp(h0) * selector
-      dout[0] = sel ? d_sigma * expf(fminf(fmaxf(a.out[0], -15.f), 15.f)) : 0.f;
+      dout[0] = sel ? d_sigma * expf(fminf(fmaxf(out[0], -15.f), 15.f)) : 0.f;
 #pragma unroll
       for (int i = 0; i < C::GEO; ++i) dout[1 + i] = d_geo[i];
       float dh1[C::BASE_H];
       Lin::template dx<C::BASE_H, C::BASE_OUT>(P.base_w[1], dout, dh1);
-      Lin::template dw<C::BASE_H, C::BASE_OUT>(sX, sY, a.h1, dout, G.base_w[1], G.base_b[1]);
+      Lin::template dw<C::BASE_H, C::BASE_OUT>(sX, sY, h1, dout, G.base_w[1], G.base_b[1]);
 #pragma unroll
-      for (int i = 0; i < C::BASE_H; ++i) dh1[i] = a.h1[i] > 0.f ? dh1[i] : 0.f;
+      for (int i = 0; i < C::BASE_H; ++i) dh1[i] = h1[i] > 0.f ? dh1[i] : 0.f;
       Lin::template dx<C::ENC, C::BASE_H>(P.base_w[0], dh1, denc);
       Lin::template dw<C::ENC, C::BASE_H>(sX, sY, enc, dh1, G.base_w[0], G.base_b[0]);
     }
@@ -727,8 +767,23 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
         }
       }
     }
+    FNR_PHASE(kPhScatter);
   }
+#ifdef FNR_BWD_PHASE_TIMERS
+  __syncthreads();  // thread 0's update of the last phase is visible to the threads that flush the counters
+  if (threadIdx.x < kBwdPhases) atomicAdd(g_bwd_phase_cycles + threadIdx.x, phase::cycles[threadIdx.x]);
+#endif
 }
+
+#ifdef FNR_BWD_PHASE_TIMERS
+// Cycles per backward phase summed over all CTAs since the last call (tools/bench_backward.py --phases); resets them.
+extern "C" int fnr_bwd_phase_cycles(unsigned long long* out) {
+  static const unsigned long long zero[kBwdPhases] = {};
+  cudaError_t e = cudaMemcpyFromSymbol(out, g_bwd_phase_cycles, sizeof(g_bwd_phase_cycles));
+  if (e == cudaSuccess) e = cudaMemcpyToSymbol(g_bwd_phase_cycles, zero, sizeof(zero));
+  return e == cudaSuccess ? 0 : (int)e;
+}
+#endif
 
 // ------------------------------------------------------------------------------------------
 // Export kernel: uniform bins, field in AABB / mean-appearance mode, thresholds + compaction

@@ -16,6 +16,30 @@
 #include <cuda_bf16.h>
 #include <stdint.h>
 
+// Diagnostic build of the backward (-DFNR_BWD_PHASE_TIMERS, tools/bench_backward.py --phases; never set by the normal
+// build): FNR_PHASE(i) closes phase i of the current tile.  Every thread of the CTA calls it; after a barrier, thread 0
+// adds the clock64() cycles since the previous mark to the CTA's counter of phase i.
+namespace fnr {
+enum BwdPhase { kPhLoad, kPhRecompute, kPhDx, kPhDw, kPhDwFlush, kPhScatter, kBwdPhases };
+#ifdef FNR_BWD_PHASE_TIMERS
+namespace phase {
+__shared__ unsigned long long cycles[kBwdPhases];
+__shared__ long long last;
+__device__ __forceinline__ void mark(int i) {
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const long long now = clock64();
+    cycles[i] += (unsigned long long)(now - last);
+    last = now;
+  }
+}
+}  // namespace phase
+#define FNR_PHASE(i) ::fnr::phase::mark(i)
+#else
+#define FNR_PHASE(i) ((void)0)
+#endif
+}  // namespace fnr
+
 namespace fnr {
 namespace wg {
 
@@ -74,6 +98,21 @@ __device__ __forceinline__ void split_store(uint8_t* hi, uint8_t* lo, int off, f
   *reinterpret_cast<__nv_bfloat16*>(lo + off) = __float2bfloat16_rn(x - __bfloat162float(h));
 }
 
+// hi / lo split of 8 consecutive k of one row: one core-matrix row, one 16-byte store into each half.
+__device__ __forceinline__ void split_store8(uint8_t* hi, uint8_t* lo, int off, const float (&x)[8]) {
+  uint32_t h[4], l[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const __nv_bfloat162 hv = __floats2bfloat162_rn(x[2 * i], x[2 * i + 1]);
+    const float2 hf = __bfloat1622float2(hv);
+    const __nv_bfloat162 lv = __floats2bfloat162_rn(x[2 * i] - hf.x, x[2 * i + 1] - hf.y);
+    h[i] = *reinterpret_cast<const uint32_t*>(&hv);
+    l[i] = *reinterpret_cast<const uint32_t*>(&lv);
+  }
+  *reinterpret_cast<uint4*>(hi + off) = make_uint4(h[0], h[1], h[2], h[3]);
+  *reinterpret_cast<uint4*>(lo + off) = make_uint4(l[0], l[1], l[2], l[3]);
+}
+
 constexpr int pad16(int k) { return (k + 15) / 16 * 16; }
 constexpr int padn(int n) { return n <= 16 ? 16 : n <= 32 ? 32 : n <= 64 ? 64 : 128; }
 
@@ -101,10 +140,23 @@ __device__ __forceinline__ void rowgemm(uint8_t* smem, const float (&x)[R], floa
   const int t = threadIdx.x;
   __syncthreads();  // the previous step's readers are done with every buffer
 #pragma unroll
-  for (int k = 0; k < KP; ++k) split_store(xhi, xlo, (k >> 3) * (128 * 16) + t * 16 + (k & 7) * 2, k < R ? x[k < R ? k : 0] : 0.f);
-  for (int i = t; i < NP * KP; i += 128) {
-    const int n = i / KP, k = i % KP;
-    split_store(whi, wlo, (k >> 3) * (NP * 16) + n * 16 + (k & 7) * 2, (n < NO && k < R) ? getw(n, k) : 0.f);
+  for (int kc = 0; kc < KP / 8; ++kc) {
+    float v[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) v[j] = 8 * kc + j < R ? x[8 * kc + j < R ? 8 * kc + j : 0] : 0.f;
+    split_store8(xhi, xlo, kc * (128 * 16) + t * 16, v);
+  }
+  // weight tile in (row, 8-k chunk) units, consecutive threads on consecutive rows of one chunk column
+  constexpr int kChunks = NP * KP / 8;
+#pragma unroll 1
+  for (int it = 0; it < (kChunks + 127) / 128; ++it) {
+    const int i = t + 128 * it;
+    if (kChunks % 128 != 0 && i >= kChunks) break;
+    const int n = i % NP, kc = i / NP;
+    float v[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) v[j] = (n < NO && 8 * kc + j < R) ? getw(n, 8 * kc + j) : 0.f;
+    split_store8(whi, wlo, kc * (NP * 16) + n * 16, v);
   }
   fence_proxy_async();
   __syncthreads();
@@ -133,15 +185,22 @@ __device__ __forceinline__ void rowgemm(uint8_t* smem, const float (&x)[R], floa
     const int r0 = h * 64 + 16 * warp + (lane >> 2), c0 = 2 * (lane & 3);
 #pragma unroll
     for (int i = 0; i < NP / 8; ++i) {
-      ys[r0 * S::kYStride + 8 * i + c0] = d[4 * i];
-      ys[r0 * S::kYStride + 8 * i + c0 + 1] = d[4 * i + 1];
-      ys[(r0 + 8) * S::kYStride + 8 * i + c0] = d[4 * i + 2];
-      ys[(r0 + 8) * S::kYStride + 8 * i + c0 + 1] = d[4 * i + 3];
+      *reinterpret_cast<float2*>(ys + r0 * S::kYStride + 8 * i + c0) = make_float2(d[4 * i], d[4 * i + 1]);
+      *reinterpret_cast<float2*>(ys + (r0 + 8) * S::kYStride + 8 * i + c0) = make_float2(d[4 * i + 2], d[4 * i + 3]);
     }
   }
   __syncthreads();
+  // row t, 16-byte aligned (kYStride is a multiple of 4)
 #pragma unroll
-  for (int n = 0; n < NO; ++n) y[n] = ys[t * S::kYStride + n];
+  for (int n = 0; n < NO / 4 * 4; n += 4) {
+    const float4 v = *reinterpret_cast<const float4*>(ys + t * S::kYStride + n);
+    y[n] = v.x;
+    y[n + 1] = v.y;
+    y[n + 2] = v.z;
+    y[n + 3] = v.w;
+  }
+#pragma unroll
+  for (int n = NO / 4 * 4; n < NO; ++n) y[n] = ys[t * S::kYStride + n];
 }
 
 // y[N] = W x + b (optionally ReLU), W in torch layout [N][K].
@@ -218,6 +277,7 @@ __device__ __forceinline__ void weight_grad(uint8_t* smem, const float (&x)[K], 
     }
     commit();
     wait_all();
+    FNR_PHASE(kPhDw);
     const int n0 = h * 64 + 16 * warp + (lane >> 2), c0 = 2 * (lane & 3);
 #pragma unroll
     for (int i = 0; i < KP / 8; ++i) {
@@ -234,6 +294,7 @@ __device__ __forceinline__ void weight_grad(uint8_t* smem, const float (&x)[K], 
     for (int p = 0; p < 128; ++p) sum += ys[p * S::YS + n];
     if (sum != 0.f) atomicAdd(gb + n, sum);
   }
+  FNR_PHASE(kPhDwFlush);
 }
 
 }  // namespace wg
