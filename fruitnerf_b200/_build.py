@@ -12,7 +12,8 @@ from pathlib import Path
 CSRC = Path(__file__).resolve().parent / "csrc"
 LIB = CSRC / "libfruitnerf_b200.so"
 STAMP = CSRC / "libfruitnerf_b200.recipe"  # flags and sources LIB was built from
-SOURCES = ["fnr_api.cu", "fnr_simt.cu", "fnr_proposal.cu", "fnr_optim.cu", "fnr_glue.cu", "fnr_nvls.cu", "fnr_cluster.cu"]
+SOURCES = ["fnr_api.cu", "fnr_simt.cu", "fnr_proposal.cu", "fnr_optim.cu", "fnr_glue.cu", "fnr_nvls.cu", "fnr_cluster.cu",
+           "fnr_fruit_split.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr",

@@ -203,6 +203,9 @@ EXPORTED_SYMBOLS = (
     "fnr_knn_mean_distance",
     "fnr_estimate_normals",
     "fnr_backproject_select",
+    "fnr_icp_scaled",
+    "fnr_ward_cut",
+    "fnr_hausdorff",
 )
 
 _lib = None
@@ -284,6 +287,12 @@ def load() -> C.CDLL:
     lib.fnr_estimate_normals.argtypes = [vp, i64, f64p, f64p, i32, vp, vp, vp, sz, vp]
     lib.fnr_backproject_select.restype = C.c_int
     lib.fnr_backproject_select.argtypes = [vp, vp, vp, vp, vp, i32, i32, _f32p, _f32p, i32, vp, vp, vp, vp, vp]
+    lib.fnr_icp_scaled.restype = C.c_int
+    lib.fnr_icp_scaled.argtypes = [vp, i32, vp, vp, i32, i32, vp, f64, i32, f64, f64, vp, vp, vp, vp, vp]
+    lib.fnr_ward_cut.restype = C.c_int
+    lib.fnr_ward_cut.argtypes = [vp, vp, i32, i32, vp, vp]
+    lib.fnr_hausdorff.restype = C.c_int
+    lib.fnr_hausdorff.argtypes = [vp, vp, vp, vp, i32, vp, vp]
     if lib.fnr_version() != ABI_VERSION:
         raise FruitNerfNativeError(f"ABI version mismatch: library reports {lib.fnr_version()}")
     _lib = lib

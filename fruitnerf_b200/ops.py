@@ -9,6 +9,7 @@ import ctypes as C
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 from torch import Tensor
 
@@ -708,3 +709,70 @@ def backproject_select(origins: Tensor, directions: Tensor, depth: Tensor, rgb: 
     L.check(L.load().fnr_backproject_select(_ptr(o), _ptr(d), _ptr(t), _ptr(c), _ptr(a), R, int(bounding_box is not None), bmin, bmax,
                                             buffers.capacity, _ptr(buffers.points), _ptr(buffers.colors), _ptr(buffers.view_dirs),
                                             _ptr(buffers.count), _stream(dev)))
+
+
+# ======================================================================================================
+# Stage 3 of the fruit count (fnr_fruit_split.cu; clustering/clustering_base.py:261-429)
+# ======================================================================================================
+def _segments(bounds, num: int, what: str) -> Tuple[np.ndarray, int]:
+    """Host int64 segment bounds checked against ``num`` rows, and the largest segment."""
+    b = np.asarray(bounds.cpu() if isinstance(bounds, Tensor) else bounds, dtype=np.int64)
+    lo, hi = (b[:-1], b[1:]) if b.ndim == 1 else (b[:, 0], b[:, 1])
+    if b.ndim not in (1, 2) or (b.ndim == 2 and b.shape[1] != 2) or bool((lo < 0).any()) or bool((hi > num).any()) or bool((hi < lo).any()):
+        raise ValueError(f"{what}: segment bounds must be ascending offsets or (begin, end) rows within {num} rows")
+    return b, int((hi - lo).max(initial=0))
+
+
+def icp_scaled(source: Tensor, targets: Tensor, target_offsets, init_translation: Tensor, max_distance: float = 0.01,
+               max_iteration: int = 2000, relative_fitness: float = 1e-6, relative_rmse: float = 1e-6):
+    """Scaled point-to-point ICP of one ``source`` cloud [m,3] onto each target segment (rows target_offsets[b] ..
+    target_offsets[b+1] of ``targets``), starting from a translation ``init_translation`` [B,3]: clustering.icp_scaled
+    batched.  ``target_offsets``: host sequence of B+1 ascending ints.  Returns (transforms [B,4,4] fp64, fitness [B],
+    rmse [B], iterations [B] int32)."""
+    src, tgt, init = cluster_points(source), cluster_points(targets), cluster_points(init_translation)
+    dev = tgt.device
+    offs, max_n = _segments(target_offsets, tgt.shape[0], "icp_scaled")
+    B = offs.shape[0] - 1
+    if init.shape[0] != B:
+        raise ValueError(f"{init.shape[0]} initial translations for {B} problems")
+    if B and (offs[1:] == offs[:-1]).any():
+        raise ValueError("icp_scaled: every target segment needs at least one point")
+    T = torch.empty((B, 4, 4), dtype=torch.float64, device=dev)
+    fitness, rmse = torch.empty(B, dtype=torch.float64, device=dev), torch.empty(B, dtype=torch.float64, device=dev)
+    iters = torch.empty(B, dtype=torch.int32, device=dev)
+    offs_d = torch.from_numpy(offs).to(dev)
+    L.check(L.load().fnr_icp_scaled(_ptr(src), src.shape[0], _ptr(tgt), _ptr(offs_d), B, max(max_n, 1), _ptr(init), float(max_distance),
+                                    int(max_iteration), float(relative_fitness), float(relative_rmse), _ptr(T), _ptr(fitness), _ptr(rmse),
+                                    _ptr(iters), _stream(dev)))
+    return T, fitness, rmse, iters
+
+
+def ward_cut(points: Tensor, offsets) -> Tensor:
+    """clustering.ward_cut_centres for each segment (rows offsets[b] .. offsets[b+1] of ``points``; at most 4096 rows,
+    more raise the library's unsupported error): [B,20,3] fp64.  ``offsets``: host sequence of B+1 ascending ints."""
+    pts = cluster_points(points)
+    dev = pts.device
+    offs, max_n = _segments(offsets, pts.shape[0], "ward_cut")
+    B = offs.shape[0] - 1
+    out = torch.empty((B, 20, 3), dtype=torch.float64, device=dev)
+    offs_d = torch.from_numpy(offs).to(dev)
+    L.check(L.load().fnr_ward_cut(_ptr(pts), _ptr(offs_d), B, max(max_n, 1), _ptr(out), _stream(dev)))
+    return out
+
+
+def hausdorff(a: Tensor, a_ranges, b: Tensor, b_ranges) -> Tensor:
+    """Symmetric Hausdorff distances [P] fp64 of the pairs (rows a_ranges[p] of ``a``, rows b_ranges[p] of ``b``):
+    clustering.hausdorff batched, bit for bit.  Ranges: host [P,2] (begin, end) ints; empty sets raise ValueError."""
+    pa, pb = cluster_points(a), cluster_points(b)
+    dev = pa.device
+    ra, _ = _segments(a_ranges, pa.shape[0], "hausdorff")
+    rb, _ = _segments(b_ranges, pb.shape[0], "hausdorff")
+    if ra.ndim != 2 or rb.ndim != 2 or ra.shape[0] != rb.shape[0]:
+        raise ValueError("hausdorff: a_ranges and b_ranges must both be [P,2]")
+    if (ra[:, 1] == ra[:, 0]).any() or (rb[:, 1] == rb[:, 0]).any():
+        raise ValueError("hausdorff: every set needs at least one point")
+    P = ra.shape[0]
+    out = torch.empty(P, dtype=torch.float64, device=dev)
+    ra_d, rb_d = torch.from_numpy(np.ascontiguousarray(ra)).to(dev), torch.from_numpy(np.ascontiguousarray(rb)).to(dev)
+    L.check(L.load().fnr_hausdorff(_ptr(pa), _ptr(ra_d), _ptr(pb), _ptr(rb_d), P, _ptr(out), _stream(dev)))
+    return out

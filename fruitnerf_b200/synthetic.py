@@ -140,3 +140,52 @@ def fruit_shell_cloud(n: int, seed: int = 0, points_per_fruit: int = 4000, fruit
     lo, hi = centers.min(axis=0) - 2 * fruit_radius, centers.max(axis=0) + 2 * fruit_radius
     noise = rng.uniform(lo, hi, (n_noise, 3))
     return np.concatenate([shells, noise])[rng.permutation(n)]
+
+
+def sphere_template(radius: float = 0.035, n: int = 1000):
+    """[n,3] float64 fruit template: n points of a Fibonacci lattice on a sphere of ``radius`` about the origin (their
+    mean is the origin to rounding).  Stands in for the reference's scanned fruit templates in tests and benchmarks."""
+    import numpy as np
+
+    i = np.arange(n, dtype=np.float64) + 0.5
+    z = 1.0 - 2.0 * i / n
+    r = np.sqrt(np.maximum(0.0, 1.0 - z * z))
+    phi = i * (math.pi * (3.0 - math.sqrt(5.0)))
+    return radius * np.stack([r * np.cos(phi), r * np.sin(phi), z], axis=1)
+
+
+def touching_fruit_cloud(seed: int = 0, singles: int = 3, pairs: int = 3, triples: int = 2, fragments: int = 2, fruit_radius: float = 0.035,
+                         points_per_fruit: int = 4000, fragment_radius: float = 0.012, points_per_fragment: int = 800,
+                         overlap: float = 0.95, spacing: float = 0.3, jitter: float = 0.02):
+    """(points [n,3] float64, true fruit centres [K,3]) of a tree-like semantic cloud for the split stage of the count:
+    single fruit shells, touching pairs and triples (centres ``overlap`` * 2 * ``fruit_radius`` apart, in random
+    orientations) and fragments (shells of ``fragment_radius``, well under 0.3 of a fruit's volume, which are no fruit).
+    Shells have ``jitter`` relative radial noise; the groups sit on a lattice of pitch ``spacing`` with random offsets,
+    far enough apart that DBSCAN never joins two of them.  At the defaults the density suits the reference's real-tree
+    counting parameters (clustering/config_real.py).  numpy's seeded generator, points in shuffled order."""
+    import numpy as np
+
+    rng = np.random.default_rng(seed)
+    kinds = ["single"] * singles + ["pair"] * pairs + ["triple"] * triples + ["fragment"] * fragments
+    side = max(1, math.ceil(len(kinds) ** (1.0 / 3.0) - 1e-9))
+    shells, centres = [], []
+
+    def shell(c, radius, n):
+        d = rng.standard_normal((n, 3))
+        d /= np.linalg.norm(d, axis=1, keepdims=True)
+        return c + d * (radius * (1.0 + jitter * rng.standard_normal((n, 1))))
+
+    for g, kind in enumerate(rng.permutation(kinds)):
+        anchor = np.array(np.unravel_index(g, (side, side, side)), dtype=np.float64) * spacing + rng.uniform(-0.05, 0.05, 3) * spacing
+        if kind == "fragment":
+            shells.append(shell(anchor, fragment_radius, points_per_fragment))
+            continue
+        k = {"single": 1, "pair": 2, "triple": 3}[kind]
+        q, _ = np.linalg.qr(rng.standard_normal((3, 3)))  # random orientation of the group
+        step = overlap * 2.0 * fruit_radius
+        offsets = np.array([[0.0, 0.0, 0.0], [step, 0.0, 0.0], [step / 2.0, step * math.sqrt(3.0) / 2.0, 0.0]])[:k]
+        for c in (offsets - offsets.mean(axis=0)) @ q.T + anchor:
+            centres.append(c)
+            shells.append(shell(c, fruit_radius, points_per_fruit))
+    pts = np.concatenate(shells)
+    return pts[rng.permutation(pts.shape[0])], np.array(centres)

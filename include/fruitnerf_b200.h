@@ -41,6 +41,9 @@
  *   fnr_backproject_select, fnr_knn_mean_distance, fnr_estimate_normals
  *                        the `pointcloud` export (fruit_nerf/scripts/exporter.py:124-129, nerfstudio ExportPointCloud):
  *                        back-projection and selection of rendered rays, statistical outlier removal, normal estimation
+ *   fnr_icp_scaled, fnr_ward_cut, fnr_hausdorff
+ *                        stage 3 of the fruit counting (clustering/clustering_base.py:261-429): scaled ICP of the fruit
+ *                        template, Ward sub-centres for k = 2..6 and Hausdorff distances of each group to split
  */
 #ifndef FRUITNERF_B200_H
 #define FRUITNERF_B200_H
@@ -408,6 +411,38 @@ int fnr_estimate_normals(const double* points, int64_t num_points, const double*
 int fnr_backproject_select(const float* origins, const float* directions, const float* depth, const float* rgb, const float* accumulation,
                            int32_t num_rays, int32_t use_bounding_box, const float* box_min, const float* box_max, int32_t capacity,
                            float* points, float* colors, float* view_dirs, int32_t* count, void* stream);
+
+/* ---- stage 3 of the fruit counting: the split of merged groups larger than one fruit (clustering_base.py:261-429).
+ * Batched: one CTA per problem, fp64, distances (dx*dx + dy*dy) + dz*dz without FMA.  Segment bounds are DEVICE int64;
+ * every other array is DEVICE fp64 unless stated.  Deterministic: the same input gives the same bits. */
+
+/* open3d registration_icp(source, target_b, max_distance, translation(init_translation[b]),
+ * TransformationEstimationPointToPoint(with_scaling=True), ICPConvergenceCriteria(relative_fitness, relative_rmse,
+ * max_iteration)) for B targets that share one source: each iteration pairs every transformed source point with its
+ * nearest target (lowest index on ties) when the squared distance is < max_distance^2, solves Umeyama with scale on the
+ * pairs (identity with fewer than 3 pairs, zero spread or a cross-covariance of rank < 2) and left-multiplies it onto
+ * the transform, until |d fitness| < relative_fitness and |d rmse| < relative_rmse.  source: [num_source,3]
+ * (1..16384 points); target b: rows target_offsets[b] .. target_offsets[b+1] of targets, 1..max_targets <= 4096 rows
+ * (a segment outside that range gets a NaN transform and iteration count -1).  Outputs: transforms [B,4,4] row-major,
+ * fitness [B], rmse [B], iterations [B] int32 (updates applied). */
+int fnr_icp_scaled(const double* source, int32_t num_source, const double* targets, const int64_t* target_offsets, int32_t num_problems,
+                   int32_t max_targets, const double* init_translation, double max_distance, int32_t max_iteration,
+                   double relative_fitness, double relative_rmse, double* transforms, double* fitness, double* rmse, int32_t* iterations,
+                   void* stream);
+
+/* sklearn AgglomerativeClustering(n_clusters=k, linkage="ward") sub-centres for k = 2..6 from one Ward tree per segment
+ * (nearest-neighbour chain; ties go to the chain's predecessor, then to the lower cluster slot, a cluster's slot being
+ * its smallest point index).  Segment b: rows offsets[b] .. offsets[b+1] of points, 1..max_points <= 4096 rows.
+ * centres: [B,20,3]; rows 0-1 hold k = 2, 2-4 k = 3, 5-8 k = 4, 9-13 k = 5, 14-19 k = 6, each cut's sub-cluster means
+ * ordered by smallest point index.  Rows of a cut with more clusters than points, and every row of a segment outside
+ * 1..max_points, are NaN. */
+int fnr_ward_cut(const double* points, const int64_t* offsets, int32_t num_segments, int32_t max_points, double* centres, void* stream);
+
+/* Symmetric Hausdorff distance max(h(A_p, B_p), h(B_p, A_p)), exact, for num_pairs pairs: A_p is rows
+ * a_ranges[2p] .. a_ranges[2p+1] of a, B_p rows b_ranges[2p] .. b_ranges[2p+1] of b.  distances: [num_pairs]; NaN for a
+ * pair with an empty set. */
+int fnr_hausdorff(const double* a, const int64_t* a_ranges, const double* b, const int64_t* b_ranges, int32_t num_pairs, double* distances,
+                  void* stream);
 
 /* Hash-grid row indices (exact-integer parity hook): rows[N,L,8] in nerfstudio corner order for
  * the masked [0,1]^3 positions of the given samples; also writes positions[N,3] if non-NULL. */
