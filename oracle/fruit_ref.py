@@ -135,15 +135,16 @@ def field_forward(
     }
 
 
-def render(field_out: Dict[str, Tensor], starts: Tensor, ends: Tensor, training: bool = True) -> Dict[str, Tensor]:
+def render(field_out: Dict[str, Tensor], starts: Tensor, ends: Tensor, training: bool = True,
+           pass_semantic_gradients: bool = False) -> Dict[str, Tensor]:
     """FruitModel.get_outputs after the field call (fruit_nerf.py:325-355), without the proposal
-    entries.  ``semantics`` uses detached weights (pass_semantic_gradients=False, 343-345)."""
+    entries.  ``semantics`` uses detached weights unless ``pass_semantic_gradients`` (301-305, 343-345)."""
     deltas = ends - starts
     weights = ns.get_weights(deltas, field_out["density"])
     rgb = ns.render_rgb_last_sample(field_out["rgb"], weights, training)
     depth, depth_idx = ns.render_depth_median(weights, starts, ends)
     acc = ns.render_accumulation(weights)
-    sem = ns.render_semantics(field_out["semantics"], weights.detach())
+    sem = ns.render_semantics(field_out["semantics"], weights if pass_semantic_gradients else weights.detach())
     labels = torch.heaviside(torch.sigmoid(sem.detach()) - 0.9, torch.tensor(0.0, dtype=sem.dtype)).to(torch.long)
     return {
         "rgb": rgb,

@@ -438,3 +438,28 @@ def test_median_depth_is_the_first_sample_reaching_half_the_weight():
                 break
         assert int(idx[r]) == k
         assert float(depth[r]) == pytest.approx(float(starts[r, k] + starts[r, k + 1]) / 2, abs=1e-6)
+
+
+def test_render_pass_semantic_gradients_flag():
+    """fruit_nerf.py:301-305: the semantic renderer's weights are detached unless pass_semantic_gradients.  The flag changes
+    the gradients of the density path (base MLP, hash table) under a semantics loss, and no forward value."""
+    v = syn.SMALL
+    sd = syn.field_state(geo=v["geo"], sem_dims=v["sem_dims"], log2_hashmap_size=10, num_images=3, table_scale=0.5, weight_gain=1.5)
+    o, d, s, e, cam = syn.ray_batch(8, 12, salt=17, far=3.0, num_images=3)
+    _, mask = syn.targets(8, salt=18)
+    res = {}
+    for flag in (False, True):
+        spec = fr.FieldSpec(max_res=v["max_res"], log2_hashmap_size=10, geo_feat_dim=v["geo"])  # geo stays detached
+        st = {k: t.double().requires_grad_(k != "aabb") for k, t in sd.items()}
+        f = fr.field_forward(st, spec, o[:, None, :], d[:, None, :], s[..., None], e[..., None], cam, True, "train")
+        r = fr.render(f, s[..., None], e[..., None], training=True, pass_semantic_gradients=flag)
+        ns.semantic_bce(r["semantics"], mask.double()).backward()
+        res[flag] = (r, {k: t.grad for k, t in st.items() if k != "aabb"})
+    (r0, g0), (r1, g1) = res[False], res[True]
+    for k in ("rgb", "accumulation", "semantics", "weights", "depth"):
+        assert torch.equal(r0[k], r1[k]), k
+    for k in ("mlp_base_mlp.layers.0.weight", "mlp_base_mlp.layers.1.weight", "mlp_base_mlp.layers.1.bias", "mlp_base_grid.hash_table"):
+        assert g0[k] is None or float(g0[k].abs().max()) == 0.0, k  # the semantics loss cannot reach the density path
+        assert g1[k] is not None and float(g1[k].abs().max()) > 0.0, k
+    for k in ("mlp_semantics.layers.0.weight", "field_head_semantics.net.bias"):
+        assert torch.allclose(g0[k], g1[k], rtol=1e-12, atol=0.0), k  # the semantic branch itself sees the same weights
