@@ -15,6 +15,7 @@
 #include <cub/cub.cuh>
 #include <math_constants.h>
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include "fnr_common.cuh"
 #include "fnr_kernels.h"
@@ -33,11 +34,6 @@ constexpr double kMaxCoordOverCell = 1099511627776.0;  // 2^40: beyond it a key'
 
 __device__ __forceinline__ uint64_t pack_key(long long x, long long y, long long z) {
   return ((uint64_t)x << (2 * kAxisBits)) | ((uint64_t)y << kAxisBits) | (uint64_t)z;
-}
-
-__device__ __forceinline__ double dist2(double ax, double ay, double az, double bx, double by, double bz) {
-  const double dx = __dsub_rn(ax, bx), dy = __dsub_rn(ay, by), dz = __dsub_rn(az, bz);
-  return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
 }
 
 // floor((p - origin) / h), clamped into the key range: the per-axis voxel key of clustering.voxel_down_sample
@@ -711,8 +707,6 @@ __global__ void __launch_bounds__(kSelectThreads) backproject_select_kernel(
 }
 
 // ---- host side ------------------------------------------------------------------------------------------------------
-int blocks_for(long long n) { return (int)((n + kThreads - 1) / kThreads); }
-
 // Caller-owned device scratch, carved in a fixed order (base == nullptr: sizes only).
 struct Scratch {
   uint64_t* keys_in;
@@ -832,17 +826,17 @@ int check_extent(const char* what, const char* what_len, double len, double h, c
 
 // Sorted cell keys, sorted coordinates, cells and their first positions for cell side h and origin lo.
 int build_grid(const double* pts, int n, const double* lo, double h, const Scratch& s, cudaStream_t st, Grid* g) {
-  cell_key_kernel<<<blocks_for(n), kThreads, 0, st>>>(pts, n, lo[0], lo[1], lo[2], h, s.keys_in, s.idx_in);
+  cell_key_kernel<<<grid_for(n, kThreads, INT_MAX), kThreads, 0, st>>>(pts, n, lo[0], lo[1], lo[2], h, s.keys_in, s.idx_in);
   if (int rc = check_launch("cell_key_kernel")) return rc;
   size_t tb = s.cub_bytes;
   if (int rc = check_cuda(cub::DeviceRadixSort::SortPairs(s.cub, tb, s.keys_in, s.keys, s.idx_in, s.perm, n, 0, 3 * kAxisBits, st),
                           "cub SortPairs (cell keys)"))
     return rc;
-  gather_kernel<<<blocks_for(n), kThreads, 0, st>>>(pts, n, s.keys, s.perm, s.x, s.y, s.z, s.flag);
+  gather_kernel<<<grid_for(n, kThreads, INT_MAX), kThreads, 0, st>>>(pts, n, s.keys, s.perm, s.x, s.y, s.z, s.flag);
   if (int rc = check_launch("gather_kernel")) return rc;
   tb = s.cub_bytes;
   if (int rc = check_cuda(cub::DeviceScan::InclusiveSum(s.cub, tb, s.flag, s.cell_of, n, st), "cub InclusiveSum (cells)")) return rc;
-  cells_kernel<<<blocks_for(n), kThreads, 0, st>>>(n, s.keys, s.cell_of, s.ukeys, s.cstart, s.ncells);
+  cells_kernel<<<grid_for(n, kThreads, INT_MAX), kThreads, 0, st>>>(n, s.keys, s.cell_of, s.ukeys, s.cstart, s.ncells);
   if (int rc = check_launch("cells_kernel")) return rc;
   *g = Grid{n, s.keys, s.perm, s.x, s.y, s.z, s.cell_of, s.ukeys, s.cstart, s.ncells};
   return FNR_OK;
@@ -937,7 +931,7 @@ int fnr_radius_count(const double* points, int64_t num_points, const double* lo,
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   Grid g;
   if (int rc = build_grid(points, n, lo, h, s, st, &g)) return rc;
-  radius_count_kernel<<<blocks_for(n), kThreads, 0, st>>>(g, radius * radius, cap, counts, nullptr);
+  radius_count_kernel<<<grid_for(n, kThreads, INT_MAX), kThreads, 0, st>>>(g, radius * radius, cap, counts, nullptr);
   return check_launch("radius_count_kernel");
 }
 
@@ -957,7 +951,7 @@ int fnr_voxel_down_sample(const double* points, int64_t num_points, const double
   if (int rc = bind_scratch(what, n, scratch, scratch_bytes, &s)) return rc;
   Grid g;
   if (int rc = build_grid(points, n, lo, voxel, s, st, &g)) return rc;
-  voxel_mean_kernel<<<blocks_for(n), kThreads, 0, st>>>(g, out);
+  voxel_mean_kernel<<<grid_for(n, kThreads, INT_MAX), kThreads, 0, st>>>(g, out);
   if (int rc = check_launch("voxel_mean_kernel")) return rc;
   return check_cuda(cudaMemcpyAsync(num_out, s.ncells, sizeof(int32_t), cudaMemcpyDeviceToDevice, st), "fnr_voxel_down_sample (count)");
 }
@@ -980,7 +974,7 @@ int fnr_dbscan(const double* points, int64_t num_points, const double* lo, const
   Grid g;
   if (int rc = build_grid(points, n, lo, h, s, st, &g)) return rc;
   const double e2 = eps * eps;
-  const int nb = blocks_for(n);
+  const int nb = grid_for(n, kThreads, INT_MAX);
   radius_count_kernel<<<nb, kThreads, 0, st>>>(g, e2, min_samples, nullptr, s.core);
   if (int rc = check_launch("radius_count_kernel")) return rc;
   fill_kernel<<<nb, kThreads, 0, st>>>(s.cmin, n, kNone);
@@ -1021,7 +1015,7 @@ int fnr_cluster_sums(const double* points, const int32_t* labels, int64_t num_po
   // sort key = label + 1 (noise first), stable: every cluster's points stay in input order
   uint32_t* kin = reinterpret_cast<uint32_t*>(s.keys_in);
   uint32_t* kout = reinterpret_cast<uint32_t*>(s.keys);
-  const int nb = blocks_for(n);
+  const int nb = grid_for(n, kThreads, INT_MAX);
   label_key_kernel<<<nb, kThreads, 0, st>>>(labels, n, K, kin, s.idx_in);
   if (int rc = check_launch("label_key_kernel")) return rc;
   int bits = 1;
@@ -1030,7 +1024,7 @@ int fnr_cluster_sums(const double* points, const int32_t* labels, int64_t num_po
   if (int rc = check_cuda(cub::DeviceRadixSort::SortPairs(s.cub, tb, kin, kout, s.idx_in, s.perm, n, 0, bits, st), "cub SortPairs (labels)"))
     return rc;
   for (int* b : {s.cstart, s.cell_of}) {  // an id no point carries sums to zero
-    fill_kernel<<<blocks_for(K), kThreads, 0, st>>>(b, K, 0);
+    fill_kernel<<<grid_for(K, kThreads, INT_MAX), kThreads, 0, st>>>(b, K, 0);
     if (int rc = check_launch("fill_kernel")) return rc;
   }
   segment_bounds_kernel<<<nb, kThreads, 0, st>>>(n, kout, s.cstart, s.cell_of);

@@ -119,6 +119,29 @@ __device__ __forceinline__ float2 trilerp(const float2 (&f)[8], const LevelCell&
   return r;
 }
 
+// The two features of one hash-grid level at p: gather the cell's 8 corner rows (float2) and blend them.
+__device__ __forceinline__ float2 level_gather(const float2* __restrict__ table, const Vec3& p, float scale, int level,
+                                               uint32_t log2T) {
+  const LevelCell c = level_cell(p, scale);
+  const uint32_t mask = (1u << log2T) - 1u, base = (uint32_t)level << log2T;
+  float2 f[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) f[k] = __ldg(table + corner_row(c, k, mask, base));
+  return trilerp(f, c);
+}
+
+// Backward of level_gather: adds (g0, g1) times each corner's trilinear weight to the corner's gradient row.
+__device__ __forceinline__ void level_scatter(float2* __restrict__ table_grad, const Vec3& p, float scale, int level,
+                                              uint32_t log2T, float g0, float g1) {
+  const LevelCell c = level_cell(p, scale);
+  const uint32_t mask = (1u << log2T) - 1u, base = (uint32_t)level << log2T;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const float w = corner_weight(c, k);
+    if (w != 0.f) atomicAdd(table_grad + corner_row(c, k, mask, base), make_float2(w * g0, w * g1));
+  }
+}
+
 // [NS] components_from_spherical_harmonics(levels=4) on the shifted direction (d+1)/2.
 __device__ __forceinline__ void sh_degree4(float dx, float dy, float dz, float* __restrict__ c) {
   const float x = (dx + 1.0f) * 0.5f, y = (dy + 1.0f) * 0.5f, z = (dz + 1.0f) * 0.5f;
@@ -148,6 +171,103 @@ __device__ __forceinline__ float nan_to_num(float v) {
 }
 
 __device__ __forceinline__ float sigmoidf_(float v) { return 1.0f / (1.0f + expf(-v)); }
+
+// fp64 squared distance (dx*dx + dy*dy) + dz*dz with round-to-nearest intrinsics (no FMA): the numpy / scikit-learn order.
+__device__ __forceinline__ double dist2(double ax, double ay, double az, double bx, double by, double bz) {
+  const double dx = __dsub_rn(ax, bx), dy = __dsub_rn(ay, by), dz = __dsub_rn(az, bz);
+  return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
+}
+
+// ---- warp-per-ray primitives ----------------------------------------------------------------
+// A ray's samples are walked in chunks of 32, lane i holding sample c0 + i; `run` arguments carry a sum over the
+// earlier chunks.
+constexpr unsigned kFull = 0xffffffffu;
+
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
+  return v;
+}
+__device__ __forceinline__ float warp_incl_scan(float v, int lane) {  // sum over lanes <= lane
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const float t = __shfl_up_sync(kFull, v, o);
+    if (lane >= o) v += t;
+  }
+  return v;
+}
+__device__ __forceinline__ float warp_rev_incl_scan(float v, int lane) {  // sum over lanes >= lane
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const float t = __shfl_down_sync(kFull, v, o);
+    if (lane + o < 32) v += t;
+  }
+  return v;
+}
+
+// Inclusive cumsum of value(i) over i < n: out(i, value(0) + ... + value(i)), the sum formed chunk by chunk.
+template <class Value, class Out>
+__device__ __forceinline__ void warp_cumsum(int n, int lane, Value value, Out out) {
+  float run = 0.f;
+  for (int c0 = 0; c0 < n; c0 += 32) {
+    const int i = c0 + lane;
+    const float incl = warp_incl_scan(i < n ? value(i) : 0.f, lane);
+    if (i < n) out(i, run + incl);
+    run += __shfl_sync(kFull, incl, 31);
+  }
+}
+
+// RaySamples.get_weights on one chunk: w_i = nan_to_num((1 - e^{-x_i}) e^{-X_i}), x = delta * sigma, X_i = sum_{j<i} x_j
+// (0 for lanes past the ray's end, `in` false).  Adds the chunk's x to run_x.
+__device__ __forceinline__ float chunk_weight(float x, bool in, int lane, float& run_x) {
+  const float incl = warp_incl_scan(x, lane);
+  // exclusive prefix by shuffle, not `incl - x`: an infinite sigma*delta must give T = 1 in front of it (torch.cumsum semantics)
+  float excl = __shfl_up_sync(kFull, incl, 1);
+  if (lane == 0) excl = 0.f;
+  float w = 0.f;
+  if (in) {
+    const float alpha = 1.0f - expf(-x);
+    const float T = expf(-(run_x + excl));
+    w = nan_to_num(alpha * T);
+  }
+  run_x += __shfl_sync(kFull, incl, 31);
+  return w;
+}
+
+// Backward of get_weights, with G_i = dL/dw_i:  dL/dx_j = G_j T_{j+1} - sum_{i>j} G_i w_i.  The suffix sums are formed
+// from per-chunk totals and reverse scans, without the cancellation of "total - prefix" on long rays.
+//
+// sum of G_i w_i over the chunks after chunk ci, in lane ci (rays of at most 32 chunks); gw(i) = G_i w_i, i < S.
+template <class GW>
+__device__ __forceinline__ float later_chunks_sum(int S, int lane, GW gw) {
+  float chunk_tot = 0.f;
+  for (int c0 = 0, ci = 0; c0 < S; c0 += 32, ++ci) {
+    const int i = c0 + lane;
+    const float t = warp_sum(i < S ? gw(i) : 0.f);
+    if (lane == ci) chunk_tot = t;
+  }
+  return warp_rev_incl_scan(chunk_tot, lane) - chunk_tot;
+}
+// sum_{k>i} G_k w_k for lane i of chunk ci: the in-chunk reverse scan plus the later chunks (later_chunks_sum)
+__device__ __forceinline__ float chunk_suffix(float gw, float later_chunks, int ci, int lane) {
+  return (warp_rev_incl_scan(gw, lane) - gw) + __shfl_sync(kFull, later_chunks, ci & 31);
+}
+// dL/dsigma_i = delta_i dL/dx_i; xin = the chunk's inclusive scan of x, so T_{i+1} = e^{-(run_x + xin)}
+__device__ __forceinline__ float weights_dsigma(float delta, float G, float run_x, float xin, float suffix) {
+  const float Tnext = expf(-(run_x + xin));
+  return delta * (G * Tnext - suffix);
+}
+
+// DepthRenderer(method="median") on one chunk: searchsorted(cumsum(w), 0.5, side="left"), the first index whose
+// cumulative weight is >= 0.5.  Returns true and sets `median` if it lies in this chunk; the caller starts `median` at
+// S - 1, the clamp for rays whose weights never reach 0.5.  Adds the chunk's weight to run_w.
+__device__ __forceinline__ bool median_chunk(float w, bool in, int c0, int lane, float& run_w, int& median) {
+  const float wincl = warp_incl_scan(w, lane);
+  const unsigned m = __ballot_sync(kFull, in && run_w + wincl >= 0.5f);
+  run_w += __shfl_sync(kFull, wincl, 31);
+  if (m) median = c0 + __ffs(m) - 1;
+  return m != 0;
+}
 
 // host-side error plumbing -------------------------------------------------------------------
 void set_error(const char* fmt, ...);

@@ -24,11 +24,6 @@ constexpr int kMaxTop = 5;     // merges undone by the k = 6 cut
 constexpr int kCutRows = 20;   // 2 + 3 + 4 + 5 + 6 sub-centres
 constexpr int kTile = 1024;    // Hausdorff: points of the scanned set staged per tile (24 KB)
 
-__device__ __forceinline__ double dist2(double ax, double ay, double az, double bx, double by, double bz) {
-  const double dx = __dsub_rn(ax, bx), dy = __dsub_rn(ay, by), dz = __dsub_rn(az, bz);
-  return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
-}
-
 // row r of the 3x4 transform T applied to (x, y, z)
 __device__ __forceinline__ double affine_row(const double* T, int r, double x, double y, double z) {
   return __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T[4 * r], x), __dmul_rn(T[4 * r + 1], y)), __dmul_rn(T[4 * r + 2], z)), T[4 * r + 3]);

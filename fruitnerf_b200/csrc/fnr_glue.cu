@@ -16,13 +16,6 @@ namespace fnr {
 namespace {
 
 constexpr int kThreads = 256;
-constexpr unsigned kFull = 0xffffffffu;
-
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-  return v;
-}
 
 __global__ void __launch_bounds__(kThreads) pixel_batch_kernel(KPixelBatch A) {
   for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < A.R; r += gridDim.x * blockDim.x) {
@@ -156,25 +149,12 @@ __global__ void __launch_bounds__(kThreads) ray_metrics_kernel(KRayMetrics A) {
       __syncwarp();
     }
     if (A.depth) {
-      // searchsorted(cumsum(w), 0.5, side="left"): first index with cum >= 0.5, clamped to S - 1
       float run = 0.f;
       int idx = A.S - 1;
       bool found = false;
       for (int c0 = 0; c0 < A.S && !found; c0 += 32) {
         const int i = c0 + lane;
-        float v = i < A.S ? wr[i] : 0.f;
-        float incl = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-          const float tt = __shfl_up_sync(kFull, incl, o);
-          if (lane >= o) incl += tt;
-        }
-        const unsigned m = __ballot_sync(kFull, i < A.S && run + incl >= 0.5f);
-        if (m) {
-          idx = c0 + __ffs(m) - 1;
-          found = true;
-        }
-        run += __shfl_sync(kFull, incl, 31);
+        found = median_chunk(i < A.S ? wr[i] : 0.f, i < A.S, c0, lane, run, idx);
       }
       if (lane == 0) A.depth[r] = (A.starts[(size_t)r * A.S + idx] + A.ends[(size_t)r * A.S + idx]) / 2;
     }
@@ -193,9 +173,7 @@ int launch_pixel_batch(const KPixelBatch& A, cudaStream_t st) {
 int launch_spaced_bins(const KSpacedBins& A, cudaStream_t st) {
   const long long total = (long long)A.R * (A.S + 1);
   if (total == 0) return FNR_OK;
-  long long blocks = (total + kThreads - 1) / kThreads;
-  if (blocks > sm_count() * 8) blocks = sm_count() * 8;
-  spaced_bins_kernel<<<(int)blocks, kThreads, 0, st>>>(A);
+  spaced_bins_kernel<<<grid_for(total, kThreads, sm_count() * 8), kThreads, 0, st>>>(A);
   return check_launch("spaced_bins_kernel");
 }
 
@@ -208,9 +186,7 @@ int launch_ray_metrics(const KRayMetrics& A, cudaStream_t st) {
   if (A.R == 0) return FNR_OK;
   const int wpb = kThreads / 32;
   const size_t smem = (size_t)wpb * 2 * A.S * sizeof(float);
-  int blocks = (A.R + wpb - 1) / wpb;
-  if (blocks > sm_count() * 4) blocks = sm_count() * 4;
-  ray_metrics_kernel<<<blocks, kThreads, smem, st>>>(A);
+  ray_metrics_kernel<<<grid_for(A.R, wpb, sm_count() * 4), kThreads, smem, st>>>(A);
   return check_launch("ray_metrics_kernel");
 }
 

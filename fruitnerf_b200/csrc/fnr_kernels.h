@@ -212,6 +212,14 @@ int proposal_limits(int* max_levels, int* hidden, int* max_bins);
 
 int sm_count();
 
+// Blocks for `work` items at `per_block` items per block: at least 1, at most `max_blocks`.
+inline int grid_for(long long work, int per_block, int max_blocks) {
+  long long b = (work + per_block - 1) / per_block;
+  if (b < 1) b = 1;
+  if (b > max_blocks) b = max_blocks;
+  return (int)b;
+}
+
 // Field kernels of fnr_simt.cu for a shipped family: tc selects the tensor-core (wgmma, sm_90a) instantiation, otherwise
 // the exact-fp32 simt one.
 int launch_field_forward(Family fam, bool tc, const KField& F, const KParams& P, const KRays& Rr, const KFieldOut& O, cudaStream_t st);

@@ -71,14 +71,11 @@ int launch_adam(const KAdam& A, int radam, const float* hyper, cudaStream_t st) 
   long long total = 0;
   for (int t = 0; t < A.count; ++t) total += A.t[t].n;
   if (total == 0) return FNR_OK;
-  long long blocks = (total / 4 + kThreads - 1) / kThreads;
-  const long long cap = (long long)sm_count() * 8;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
+  const int blocks = grid_for(total / 4, kThreads, sm_count() * 8);
   if (radam)
-    adam_kernel<true><<<(int)blocks, kThreads, 0, st>>>(A, hyper);
+    adam_kernel<true><<<blocks, kThreads, 0, st>>>(A, hyper);
   else
-    adam_kernel<false><<<(int)blocks, kThreads, 0, st>>>(A, hyper);
+    adam_kernel<false><<<blocks, kThreads, 0, st>>>(A, hyper);
   return check_launch("adam_kernel");
 }
 

@@ -14,32 +14,9 @@ namespace fnr {
 
 namespace {
 
-constexpr unsigned kFull = 0xffffffffu;
 constexpr int kHidden = 16;
 constexpr int kMaxLevels = 8;
 constexpr int kWarpsPerBlock = 4;
-
-__device__ __forceinline__ float warp_incl_scan(float v, int lane) {
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const float t = __shfl_up_sync(kFull, v, o);
-    if (lane >= o) v += t;
-  }
-  return v;
-}
-__device__ __forceinline__ float warp_rev_incl_scan(float v, int lane) {  // sum over lanes >= lane
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const float t = __shfl_down_sync(kFull, v, o);
-    if (lane + o < 32) v += t;
-  }
-  return v;
-}
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-  return v;
-}
 
 struct PropNet {  // shared-memory copy of the tiny MLP
   float w0[kHidden][2 * kMaxLevels];
@@ -67,16 +44,10 @@ __device__ __forceinline__ Vec3 prop_position(const KDensity& D, const float* o,
 // encode + MLP.  enc / hid are kept for the backward.
 __device__ __forceinline__ float prop_mlp(const KDensity& D, const PropNet& n, const Vec3& p, float (&enc)[2 * kMaxLevels], float (&hid)[kHidden]) {
   const float2* table = reinterpret_cast<const float2*>(D.hash_table);
-  const uint32_t mask = (1u << D.log2T) - 1u;
 #pragma unroll
   for (int l = 0; l < kMaxLevels; ++l) {
     if (l < D.L) {
-      const LevelCell c = level_cell(p, D.scalings[l]);
-      const uint32_t base = (uint32_t)l << D.log2T;
-      float2 f[8];
-#pragma unroll
-      for (int k = 0; k < 8; ++k) f[k] = __ldg(table + corner_row(c, k, mask, base));
-      const float2 r = trilerp(f, c);
+      const float2 r = level_gather(table, p, D.scalings[l], l, D.log2T);
       enc[2 * l] = r.x;
       enc[2 * l + 1] = r.y;
     } else {
@@ -123,16 +94,8 @@ __global__ void __launch_bounds__(32 * kWarpsPerBlock) proposal_weights_forward_
         if (density) density[base + i] = sigma;
         x = (en - st) * sigma;
       }
-      const float incl = warp_incl_scan(x, lane);
-      // exclusive prefix by shuffle, not `incl - x`: an infinite sigma*delta must give T = 1 in front of it (torch.cumsum semantics)
-      float excl = __shfl_up_sync(kFull, incl, 1);
-      if (lane == 0) excl = 0.f;
-      if (in) {
-        const float alpha = 1.0f - expf(-x);
-        const float T = expf(-(run_x + excl));
-        weights[base + i] = nan_to_num(alpha * T);
-      }
-      run_x += __shfl_sync(kFull, incl, 31);
+      const float w = chunk_weight(x, in, lane, run_x);
+      if (in) weights[base + i] = w;
     }
   }
 }
@@ -155,22 +118,12 @@ __global__ void __launch_bounds__(32 * kWarpsPerBlock) proposal_weights_backward
   load_net(net, D);
   const int lane = threadIdx.x & 31;
   const int S = Rr.S;
-  const uint32_t mask = (1u << D.log2T) - 1u;
   float2* gtab = reinterpret_cast<float2*>(G.hash_table);
   for (int r = blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5); r < Rr.R; r += gridDim.x * kWarpsPerBlock) {
     const float* o = Rr.origins + 3 * (size_t)r;
     const float* d = Rr.directions + 3 * (size_t)r;
     const size_t base = (size_t)r * S;
-    // pass 1: per-chunk totals of G_i w_i (lane c keeps chunk c), then the sum over LATER chunks by a reverse
-    // scan: suffix sums are formed without the cancellation of "total - prefix" (long rays, far bins)
-    float chunk_tot = 0.f;
-    for (int c0 = 0, ci = 0; c0 < S; c0 += 32, ++ci) {
-      const int i = c0 + lane;
-      const float v = i < S ? d_weights[base + i] * weights[base + i] : 0.f;
-      const float t = warp_sum(v);
-      if (lane == ci) chunk_tot = t;
-    }
-    const float later_chunks = warp_rev_incl_scan(chunk_tot, lane) - chunk_tot;
+    const float later_chunks = later_chunks_sum(S, lane, [&](int i) { return d_weights[base + i] * weights[base + i]; });
     float run_x = 0.f;
     for (int c0 = 0, ci = 0; c0 < S; c0 += 32, ++ci) {
       const int i = c0 + lane;
@@ -185,8 +138,7 @@ __global__ void __launch_bounds__(32 * kWarpsPerBlock) proposal_weights_backward
         Gi = d_weights[base + i];
       }
       const float xin = warp_incl_scan(x, lane);
-      const float gw = Gi * w;
-      const float suffix = (warp_rev_incl_scan(gw, lane) - gw) + __shfl_sync(kFull, later_chunks, ci);  // sum_{k>i} G_k w_k
+      const float suffix = chunk_suffix(Gi * w, later_chunks, ci, lane);
       float dh = 0.f;
       float enc[2 * kMaxLevels], hid[kHidden];
       Vec3 p = {0.f, 0.f, 0.f};
@@ -196,8 +148,7 @@ __global__ void __launch_bounds__(32 * kWarpsPerBlock) proposal_weights_backward
 #pragma unroll
       for (int j = 0; j < kHidden; ++j) hid[j] = 0.f;
       if (in) {
-        const float Tnext = expf(-(run_x + xin));
-        const float dsig = delta * (Gi * Tnext - suffix);
+        const float dsig = weights_dsigma(delta, Gi, run_x, xin, suffix);
         p = prop_position(D, o, d, st, en, sel);
         const float h = prop_mlp(D, net, p, enc, hid);
         dh = sel ? dsig * expf(fminf(fmaxf(h, -15.f), 15.f)) : 0.f;  // trunc_exp backward
@@ -243,13 +194,7 @@ __global__ void __launch_bounds__(32 * kWarpsPerBlock) proposal_weights_backward
               g0 = fmaf(net.w0[j][2 * l], dhid[j], g0);
               g1 = fmaf(net.w0[j][2 * l + 1], dhid[j], g1);
             }
-            const LevelCell c = level_cell(p, D.scalings[l]);
-            const uint32_t lb = (uint32_t)l << D.log2T;
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-              const float w = corner_weight(c, k);
-              if (w != 0.f) atomicAdd(gtab + corner_row(c, k, mask, lb), make_float2(w * g0, w * g1));
-            }
+            level_scatter(gtab, p, D.scalings[l], l, D.log2T, g0, g1);
           }
         }
       }
@@ -294,20 +239,15 @@ __global__ void __launch_bounds__(32 * kWarpsPerBlock) pdf_sample_kernel(KPdf A)
     const float padding = fmaxf(A.eps - wsum, 0.f);
     wsum += padding;
     const float pad_each = padding / (float)S;
-    float run = 0.f;
     if (lane == 0) cdf[0] = 0.f;
-    for (int c0 = 0; c0 < S; c0 += 32) {
-      const int i = c0 + lane;
-      float pdf = 0.f;
-      if (i < S) {
-        float v = w[i];
-        if (anneal != 1.0f) v = powf(v, anneal);
-        pdf = (v + A.hist_padding + pad_each) / wsum;
-      }
-      const float incl = warp_incl_scan(pdf, lane);
-      if (i < S) cdf[i + 1] = fminf(1.0f, run + incl);
-      run += __shfl_sync(kFull, incl, 31);
-    }
+    warp_cumsum(
+        S, lane,
+        [=](int i) {
+          float v = w[i];
+          if (anneal != 1.0f) v = powf(v, anneal);
+          return (v + A.hist_padding + pad_each) / wsum;
+        },
+        [=](int i, float c) { cdf[i + 1] = fminf(1.0f, c); });
     __syncwarp();
     const float near_s = lindisp_fn(A.nears[r]), far_s = lindisp_fn(A.fars[r]);
     float* out_bins = A.new_bins + (size_t)r * NB;
@@ -354,15 +294,8 @@ __global__ void __launch_bounds__(32 * kWarpsPerBlock) interlevel_loss_kernel(KI
     const float* cp = A.cp + (size_t)r * (Sp + 1);
     const float* wp = A.wp + (size_t)r * Sp;
     // cy = [0, cumsum(wp)]
-    float run = 0.f;
     if (lane == 0) cy[0] = 0.f;
-    for (int c0 = 0; c0 < Sp; c0 += 32) {
-      const int i = c0 + lane;
-      const float v = i < Sp ? wp[i] : 0.f;
-      const float incl = warp_incl_scan(v, lane);
-      if (i < Sp) cy[i + 1] = run + incl;
-      run += __shfl_sync(kFull, incl, 31);
-    }
+    warp_cumsum(Sp, lane, [&](int i) { return wp[i]; }, [&](int i, float c) { cy[i + 1] = c; });
     for (int i = lane; i <= Sp; i += 32) dcy[i] = 0.f;
     __syncwarp();
     for (int i = lane; i < Sc; i += 32) {
@@ -400,15 +333,10 @@ __global__ void __launch_bounds__(32 * kWarpsPerBlock) interlevel_loss_kernel(KI
       float tot = 0.f;
       for (int i = lane; i <= Sp; i += 32) tot += dcy[i];
       tot = warp_sum(tot);
-      float runp = 0.f;  // prefix of dcy[0..]
-      for (int c0 = 0; c0 <= Sp; c0 += 32) {
-        const int i = c0 + lane;
-        const float v = i <= Sp ? dcy[i] : 0.f;
-        const float incl = warp_incl_scan(v, lane);
-        // suffix over m >= i+1  = tot - prefix(i)
-        if (i < Sp) dwp[i] = tot - (runp + incl);
-        runp += __shfl_sync(kFull, incl, 31);
-      }
+      // suffix over m >= i+1  = tot - prefix(i)
+      warp_cumsum(Sp + 1, lane, [&](int i) { return dcy[i]; }, [&](int i, float c) {
+        if (i < Sp) dwp[i] = tot - c;
+      });
     }
     __syncwarp();
   }
@@ -416,40 +344,32 @@ __global__ void __launch_bounds__(32 * kWarpsPerBlock) interlevel_loss_kernel(KI
   if (lane == 0 && loss_part != 0.f) atomicAdd(A.loss, loss_part * A.scale);
 }
 
-int grid_for_rays(int R) {
-  long long b = ((long long)R + kWarpsPerBlock - 1) / kWarpsPerBlock;
-  const long long cap = (long long)sm_count() * 16;
-  if (b > cap) b = cap;
-  if (b < 1) b = 1;
-  return (int)b;
-}
-
 }  // namespace
 
 int launch_proposal_weights_forward(const KDensity& D, const KRays& Rr, float* density, float* weights, cudaStream_t st) {
   if (Rr.R == 0) return FNR_OK;
-  proposal_weights_forward_kernel<<<grid_for_rays(Rr.R), 32 * kWarpsPerBlock, 0, st>>>(D, Rr, density, weights);
+  const int grid = grid_for(Rr.R, kWarpsPerBlock, sm_count() * 16);
+  proposal_weights_forward_kernel<<<grid, 32 * kWarpsPerBlock, 0, st>>>(D, Rr, density, weights);
   return check_launch("proposal_weights_forward_kernel");
 }
 
 int launch_proposal_weights_backward(const KDensity& D, const KDensity& G, const KRays& Rr, const float* density, const float* weights,
                                      const float* d_weights, cudaStream_t st) {
   if (Rr.R == 0) return FNR_OK;
-  int grid = grid_for_rays(Rr.R);
-  if (grid > sm_count() * 4) grid = sm_count() * 4;
+  const int grid = grid_for(Rr.R, kWarpsPerBlock, sm_count() * 4);
   proposal_weights_backward_kernel<<<grid, 32 * kWarpsPerBlock, 0, st>>>(D, G, Rr, density, weights, d_weights);
   return check_launch("proposal_weights_backward_kernel");
 }
 
 int launch_pdf_sample(const KPdf& A, cudaStream_t st) {
   if (A.R == 0) return FNR_OK;
-  pdf_sample_kernel<<<grid_for_rays(A.R), 32 * kWarpsPerBlock, 0, st>>>(A);
+  pdf_sample_kernel<<<grid_for(A.R, kWarpsPerBlock, sm_count() * 16), 32 * kWarpsPerBlock, 0, st>>>(A);
   return check_launch("pdf_sample_kernel");
 }
 
 int launch_interlevel_loss(const KInterlevel& A, cudaStream_t st) {
   if (A.R == 0) return FNR_OK;
-  interlevel_loss_kernel<<<grid_for_rays(A.R), 32 * kWarpsPerBlock, 0, st>>>(A);
+  interlevel_loss_kernel<<<grid_for(A.R, kWarpsPerBlock, sm_count() * 16), 32 * kWarpsPerBlock, 0, st>>>(A);
   return check_launch("interlevel_loss_kernel");
 }
 

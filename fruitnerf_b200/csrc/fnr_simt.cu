@@ -15,7 +15,6 @@
 namespace fnr {
 
 constexpr int kThreads = 128;
-constexpr unsigned kFull = 0xffffffffu;
 
 template <int GEO_, int SEM_LAYERS_, int SEM_H_>
 struct Cfg {
@@ -126,15 +125,9 @@ __device__ __forceinline__ void linear_bwd_input(const float* __restrict__ W, co
 template <int L>
 __device__ __forceinline__ void hash_encode(const float2* __restrict__ table, const float* __restrict__ scalings,
                                             uint32_t log2T, const Vec3& p, float (&enc)[2 * L]) {
-  const uint32_t mask = (1u << log2T) - 1u;
 #pragma unroll 2
   for (int l = 0; l < L; ++l) {
-    const LevelCell c = level_cell(p, scalings[l]);
-    const uint32_t base = (uint32_t)l << log2T;
-    float2 f[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) f[k] = __ldg(table + corner_row(c, k, mask, base));
-    const float2 r = trilerp(f, c);
+    const float2 r = level_gather(table, p, scalings[l], l, log2T);
     enc[2 * l] = r.x;
     enc[2 * l + 1] = r.y;
   }
@@ -206,38 +199,71 @@ struct Acts {
   float logit;
 };
 
+// The field's branch forwards.  field_mlps and the backward's recompute both run these, so the recompute gives the
+// forward's pre-activations bit for bit and its ReLU masks agree with the forward that ran.
+//
+// base MLP: enc -> [h0, geo...]; geo = out[1:]
+template <class C, bool TC>
+__device__ __forceinline__ void base_fwd(const KParams& P, const float (&enc)[C::ENC], float (&h1)[C::BASE_H],
+                                         float (&out)[C::BASE_OUT], float (&geo)[C::GEO]) {
+  using Lin = Layers<C, TC>;
+  Lin::template fwd<C::ENC, C::BASE_H, true>(P.base_w[0], P.base_b[0], enc, h1);
+  Lin::template fwd<C::BASE_H, C::BASE_OUT, false>(P.base_w[1], P.base_b[1], h1, out);
+#pragma unroll
+  for (int i = 0; i < C::GEO; ++i) geo[i] = out[1 + i];
+}
+
+// semantic branch up to the logit head: mlp_semantics(detach(geo)) (fruit_field.py:263-268)
+template <class C, bool TC>
+__device__ __forceinline__ void semantic_fwd(const KParams& P, const float (&geo)[C::GEO], float (&z1)[C::SEM_H],
+                                             float (&z2)[C::SEM_LAYERS == 3 ? C::SEM_H : 1], float (&zo)[C::SEM_OUT]) {
+  using Lin = Layers<C, TC>;
+  Lin::template fwd<C::GEO, C::SEM_H, true>(P.sem_w[0], P.sem_b[0], geo, z1);
+  if constexpr (C::SEM_LAYERS == 3) {
+    Lin::template fwd<C::SEM_H, C::SEM_H, true>(P.sem_w[1], P.sem_b[1], z1, z2);
+    Lin::template fwd<C::SEM_H, C::SEM_OUT, false>(P.sem_w[2], P.sem_b[2], z2, zo);
+  } else {
+    Lin::template fwd<C::SEM_H, C::SEM_OUT, false>(P.sem_w[1], P.sem_b[1], z1, zo);
+  }
+}
+
+// colour branch up to the sigmoid: cat[SH(dir), geo, appearance] -> MLP (fruit_field.py:270-278)
+template <class C, bool TC>
+__device__ __forceinline__ void colour_fwd(const KParams& P, const float* __restrict__ dir, const float (&geo)[C::GEO],
+                                           const float (&app)[C::APP], float (&cin)[C::COL_IN], float (&c1)[C::COL_H],
+                                           float (&c2)[C::COL_H], float (&o3)[3]) {
+  using Lin = Layers<C, TC>;
+  sh_degree4(dir[0], dir[1], dir[2], cin);
+#pragma unroll
+  for (int i = 0; i < C::GEO; ++i) cin[C::SH + i] = geo[i];
+#pragma unroll
+  for (int i = 0; i < C::APP; ++i) cin[C::SH + C::GEO + i] = app[i];
+  Lin::template fwd<C::COL_IN, C::COL_H, true>(P.col_w[0], P.col_b[0], cin, c1);
+  Lin::template fwd<C::COL_H, C::COL_H, true>(P.col_w[1], P.col_b[1], c1, c2);
+  Lin::template fwd<C::COL_H, 3, false>(P.col_w[2], P.col_b[2], c2, o3);
+}
+
 template <class C, bool TC>
 __device__ __forceinline__ void field_mlps(const KParams& P, const float (&enc)[C::ENC], const float* __restrict__ dir,
-                                           const float* __restrict__ app, Acts<C>& a) {
-  using Lin = Layers<C, TC>;
-  Lin::template fwd<C::ENC, C::BASE_H, true>(P.base_w[0], P.base_b[0], enc, a.h1);
-  Lin::template fwd<C::BASE_H, C::BASE_OUT, false>(P.base_w[1], P.base_b[1], a.h1, a.out);
-  // semantic branch: mlp_semantics(detach(geo)) -> Linear head (fruit_field.py:263-268)
+                                           const float (&app)[C::APP], Acts<C>& a) {
   float geo[C::GEO];
-#pragma unroll
-  for (int i = 0; i < C::GEO; ++i) geo[i] = a.out[1 + i];
-  Lin::template fwd<C::GEO, C::SEM_H, true>(P.sem_w[0], P.sem_b[0], geo, a.z1);
-  if constexpr (C::SEM_LAYERS == 3) {
-    Lin::template fwd<C::SEM_H, C::SEM_H, true>(P.sem_w[1], P.sem_b[1], a.z1, a.z2);
-    Lin::template fwd<C::SEM_H, C::SEM_OUT, false>(P.sem_w[2], P.sem_b[2], a.z2, a.zo);
-  } else {
-    Lin::template fwd<C::SEM_H, C::SEM_OUT, false>(P.sem_w[1], P.sem_b[1], a.z1, a.zo);
-  }
+  base_fwd<C, TC>(P, enc, a.h1, a.out, geo);
+  semantic_fwd<C, TC>(P, geo, a.z1, a.z2, a.zo);
   float lg[1];
-  Lin::template fwd<C::SEM_OUT, 1, false>(P.head_w, P.head_b, a.zo, lg);
+  Layers<C, TC>::template fwd<C::SEM_OUT, 1, false>(P.head_w, P.head_b, a.zo, lg);
   a.logit = lg[0];
-  // colour branch: cat[SH(dir), geo, appearance] -> MLP -> sigmoid (fruit_field.py:270-278)
-  sh_degree4(dir[0], dir[1], dir[2], a.cin);
-#pragma unroll
-  for (int i = 0; i < C::GEO; ++i) a.cin[C::SH + i] = geo[i];
-#pragma unroll
-  for (int i = 0; i < C::APP; ++i) a.cin[C::SH + C::GEO + i] = app[i];
-  Lin::template fwd<C::COL_IN, C::COL_H, true>(P.col_w[0], P.col_b[0], a.cin, a.c1);
-  Lin::template fwd<C::COL_H, C::COL_H, true>(P.col_w[1], P.col_b[1], a.c1, a.c2);
   float o3[3];
-  Lin::template fwd<C::COL_H, 3, false>(P.col_w[2], P.col_b[2], a.c2, o3);
+  colour_fwd<C, TC>(P, dir, geo, app, a.cin, a.c1, a.c2, o3);
 #pragma unroll
   for (int i = 0; i < 3; ++i) a.rgb[i] = sigmoidf_(o3[i]);
+}
+
+// The appearance vector of a point in the backward and export: its camera's embedding row (per-camera mode), else the
+// block's s_app.
+template <int APP>
+__device__ __forceinline__ void load_appearance(const KParams& P, int mode, int cam, const float* s_app, float (&appv)[APP]) {
+#pragma unroll
+  for (int i = 0; i < APP; ++i) appv[i] = (mode == FNR_APP_PER_CAMERA) ? __ldg(P.app_embedding + (size_t)cam * APP + i) : s_app[i];
 }
 
 // Mean appearance embedding into shared memory (fruit_field.py:217-219, 254-256).
@@ -279,6 +305,7 @@ __global__ void __launch_bounds__(kThreads) simt_field_forward_kernel(KField F, 
 #pragma unroll
       for (int i = 0; i < C::ENC / 4; ++i) st[i] = make_float4(enc[4 * i], enc[4 * i + 1], enc[4 * i + 2], enc[4 * i + 3]);
     }
+    // not load_appearance: selecting the source row once compiles to ~130 fewer instructions in this kernel
     const float* app = (F.appearance_mode == FNR_APP_PER_CAMERA)
                            ? P.app_embedding + (size_t)Rr.camera_indices[r] * C::APP
                            : s_app;
@@ -302,20 +329,6 @@ __global__ void __launch_bounds__(kThreads) simt_field_forward_kernel(KField F, 
 // ------------------------------------------------------------------------------------------
 // K2: per-ray compositing, one warp per ray (fruit_nerf.py:325-348).
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ float warp_incl_scan(float v, int lane) {
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const float t = __shfl_up_sync(kFull, v, o);
-    if (lane >= o) v += t;
-  }
-  return v;
-}
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-  return v;
-}
-
 __global__ void __launch_bounds__(kThreads) simt_composite_kernel(KRays Rr, KComposite Cm) {
   const int lane = threadIdx.x & 31;
   const int warps_per_block = blockDim.x >> 5;
@@ -324,23 +337,18 @@ __global__ void __launch_bounds__(kThreads) simt_composite_kernel(KRays Rr, KCom
     const size_t base = (size_t)r * S;
     float run_x = 0.f, run_w = 0.f;
     float acc = 0.f, cr = 0.f, cg = 0.f, cb = 0.f, sem = 0.f;
-    int median = S;  // first index with cumulative weight >= 0.5
+    int median = S - 1;
+    bool found = false;
     for (int c0 = 0; c0 < S; c0 += 32) {
       const int i = c0 + lane;
       const bool in = i < S;
-      float x = 0.f, w = 0.f;
+      float x = 0.f;
       if (in) {
         const float delta = Rr.ends[base + i] - Rr.starts[base + i];
         x = delta * Cm.sample_density[base + i];
       }
-      const float incl = warp_incl_scan(x, lane);
-      // exclusive prefix by shuffle, not `incl - x`: an infinite sigma*delta must give T = 1 in front of it (torch.cumsum semantics)
-      float excl = __shfl_up_sync(kFull, incl, 1);
-      if (lane == 0) excl = 0.f;
+      const float w = chunk_weight(x, in, lane, run_x);
       if (in) {
-        const float alpha = 1.0f - expf(-x);
-        const float T = expf(-(run_x + excl));
-        w = nan_to_num(alpha * T);
         if (Cm.weights) Cm.weights[base + i] = w;
         float c0r = Cm.sample_rgb[3 * (base + i)], c0g = Cm.sample_rgb[3 * (base + i) + 1], c0b = Cm.sample_rgb[3 * (base + i) + 2];
         if (Cm.clamp_rgb) {
@@ -354,12 +362,7 @@ __global__ void __launch_bounds__(kThreads) simt_composite_kernel(KRays Rr, KCom
         sem += w * Cm.sample_semantics[base + i];
         acc += w;
       }
-      const float wincl = warp_incl_scan(w, lane);
-      const bool hit = in && (run_w + wincl >= 0.5f);
-      const unsigned m = __ballot_sync(kFull, hit);
-      if (m && median == S) median = c0 + (__ffs(m) - 1);
-      run_x += __shfl_sync(kFull, incl, 31);
-      run_w += __shfl_sync(kFull, wincl, 31);
+      if (!found) found = median_chunk(w, in, c0, lane, run_w, median);
     }
     acc = warp_sum(acc);
     cr = warp_sum(cr);
@@ -386,9 +389,8 @@ __global__ void __launch_bounds__(kThreads) simt_composite_kernel(KRays Rr, KCom
       }
       if (Cm.accumulation) Cm.accumulation[r] = acc;
       if (Cm.semantics) Cm.semantics[r] = sem;
-      const int mi = median < S - 1 ? median : S - 1;
-      if (Cm.depth_index) Cm.depth_index[r] = mi;
-      if (Cm.depth) Cm.depth[r] = (Rr.starts[base + mi] + Rr.ends[base + mi]) / 2;
+      if (Cm.depth_index) Cm.depth_index[r] = median;
+      if (Cm.depth) Cm.depth[r] = (Rr.starts[base + median] + Rr.ends[base + median]) / 2;
     }
   }
 }
@@ -420,48 +422,23 @@ __global__ void __launch_bounds__(kThreads) simt_composite_backward_kernel(KRays
     const float gsem = B.d_semantics ? B.d_semantics[r] : 0.f;
     const float acc = B.accumulation[r];
     const float lr = B.sample_rgb[3 * (base + S - 1)], lg = B.sample_rgb[3 * (base + S - 1) + 1], lb = B.sample_rgb[3 * (base + S - 1) + 2];
-    // pass 1: total of G_i * w_i
-    float tot = 0.f;
-    for (int c0 = 0; c0 < S; c0 += 32) {
-      const int i = c0 + lane;
-      if (i < S) {
-        const float w = B.weights[base + i];
-        float G = gr * (B.sample_rgb[3 * (base + i)] - lr) + gg * (B.sample_rgb[3 * (base + i) + 1] - lg) +
-                  gb * (B.sample_rgb[3 * (base + i) + 2] - lb) + gacc;
-        if (B.d_weights) G += B.d_weights[base + i];
-        if (B.pass_semantic_gradients) G += gsem * B.sample_semantics[base + i];
-        tot += G * w;
-      }
-    }
-    tot = warp_sum(tot);
-    // suffix sums sum_{k>i} G_k w_k: for S <= 1024 from per-chunk totals + a reverse scan inside the chunk (no
-    // "total - prefix" cancellation on long rays); longer rays keep the prefix formulation
+    // G_i = dL/dw_i of sample i < S (rgb = sum w c + (1 - acc) c_last)
+    auto upstream = [&](int i) {
+      float G = gr * (B.sample_rgb[3 * (base + i)] - lr) + gg * (B.sample_rgb[3 * (base + i) + 1] - lg) +
+                gb * (B.sample_rgb[3 * (base + i) + 2] - lb) + gacc;
+      if (B.d_weights) G += B.d_weights[base + i];
+      if (B.pass_semantic_gradients) G += gsem * B.sample_semantics[base + i];
+      return G;
+    };
+    // suffix sums sum_{k>i} G_k w_k: exact (chunk_suffix) for S <= 1024; longer rays keep "total - prefix"
     const bool exact_suffix = S <= 1024;
-    float later_chunks = 0.f;
+    float later_chunks = 0.f, tot = 0.f;
     if (exact_suffix) {
-      float chunk_tot = 0.f;
-      for (int c0 = 0, ci = 0; c0 < S; c0 += 32, ++ci) {
-        const int i = c0 + lane;
-        float v = 0.f;
-        if (i < S) {
-          float G = gr * (B.sample_rgb[3 * (base + i)] - lr) + gg * (B.sample_rgb[3 * (base + i) + 1] - lg) +
-                    gb * (B.sample_rgb[3 * (base + i) + 2] - lb) + gacc;
-          if (B.d_weights) G += B.d_weights[base + i];
-          if (B.pass_semantic_gradients) G += gsem * B.sample_semantics[base + i];
-          v = G * B.weights[base + i];
-        }
-        const float t = warp_sum(v);
-        if (lane == ci) chunk_tot = t;
-      }
-      float rs = chunk_tot;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const float t = __shfl_down_sync(kFull, rs, o);
-        if (lane + o < 32) rs += t;
-      }
-      later_chunks = rs - chunk_tot;
+      later_chunks = later_chunks_sum(S, lane, [&](int i) { return upstream(i) * B.weights[base + i]; });
+    } else {
+      for (int i = lane; i < S; i += 32) tot += upstream(i) * B.weights[base + i];
+      tot = warp_sum(tot);
     }
-    // pass 2
     float run_x = 0.f, run_gw = 0.f;
     for (int c0 = 0, ci = 0; c0 < S; c0 += 32, ++ci) {
       const int i = c0 + lane;
@@ -471,25 +448,20 @@ __global__ void __launch_bounds__(kThreads) simt_composite_backward_kernel(KRays
         delta = Rr.ends[base + i] - Rr.starts[base + i];
         x = delta * B.sample_density[base + i];
         w = B.weights[base + i];
-        G = gr * (B.sample_rgb[3 * (base + i)] - lr) + gg * (B.sample_rgb[3 * (base + i) + 1] - lg) +
-            gb * (B.sample_rgb[3 * (base + i) + 2] - lb) + gacc;
-        if (B.d_weights) G += B.d_weights[base + i];
-        if (B.pass_semantic_gradients) G += gsem * B.sample_semantics[base + i];
+        G = upstream(i);
       }
       const float xin = warp_incl_scan(x, lane);
-      const float gwv = G * w;
-      const float gwin = warp_incl_scan(gwv, lane);
-      float rsfx = gwv;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const float t = __shfl_down_sync(kFull, rsfx, o);
-        if (lane + o < 32) rsfx += t;
+      const float gw = G * w;
+      float suffix;
+      if (exact_suffix) {
+        suffix = chunk_suffix(gw, later_chunks, ci, lane);
+      } else {
+        const float gwin = warp_incl_scan(gw, lane);
+        suffix = tot - (run_gw + gwin);
+        run_gw += __shfl_sync(kFull, gwin, 31);
       }
-      const float later = __shfl_sync(kFull, later_chunks, ci & 31);
       if (in) {
-        const float Tnext = expf(-(run_x + xin));
-        const float suffix = exact_suffix ? (rsfx - gwv) + later : tot - (run_gw + gwin);
-        float dsig = delta * (G * Tnext - suffix);
+        float dsig = weights_dsigma(delta, G, run_x, xin, suffix);
         if (B.d_sample_density) dsig += B.d_sample_density[base + i];
         float dr = w * gr, dg = w * gg, db = w * gb;
         if (i == S - 1) {
@@ -512,7 +484,6 @@ __global__ void __launch_bounds__(kThreads) simt_composite_backward_kernel(KRays
         out[4] = dl;
       }
       run_x += __shfl_sync(kFull, xin, 31);
-      run_gw += __shfl_sync(kFull, gwin, 31);
     }
   }
 }
@@ -613,9 +584,7 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
     }
     const int cam = (F.appearance_mode == FNR_APP_PER_CAMERA) ? Rr.camera_indices[r] : 0;
     float appv[C::APP];
-#pragma unroll
-    for (int i = 0; i < C::APP; ++i)
-      appv[i] = (F.appearance_mode == FNR_APP_PER_CAMERA) ? __ldg(P.app_embedding + (size_t)cam * C::APP + i) : s_app[i];
+    load_appearance(P, F.appearance_mode, cam, s_app, appv);
     // upstream per-point grads (zero for padding threads)
     const float* pg = B.point_grads + 5 * (size_t)pc;
     const float vm = valid ? 1.f : 0.f;
@@ -624,14 +593,10 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
     const float d_logit = pg[4] * vm;
     FNR_PHASE(kPhLoad);
 
-    // The forward is recomputed branch by branch (the same layer calls as field_mlps, so the same values), and each
-    // branch is back-propagated right after its forward: only the base MLP's activations live across the whole tile.
-    float h1[C::BASE_H], out[C::BASE_OUT];
-    Lin::template fwd<C::ENC, C::BASE_H, true>(P.base_w[0], P.base_b[0], enc, h1);
-    Lin::template fwd<C::BASE_H, C::BASE_OUT, false>(P.base_w[1], P.base_b[1], h1, out);
-    float geo[C::GEO];
-#pragma unroll
-    for (int i = 0; i < C::GEO; ++i) geo[i] = out[1 + i];
+    // The forward is recomputed branch by branch with field_mlps' branch functions, and each branch is back-propagated
+    // right after its forward: only the base MLP's activations live across the whole tile.
+    float h1[C::BASE_H], out[C::BASE_OUT], geo[C::GEO];
+    base_fwd<C, TC>(P, enc, h1, out, geo);
     FNR_PHASE(kPhRecompute);
 
     float d_geo[C::GEO];
@@ -642,13 +607,7 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
     {
       float z1[C::SEM_H], zo[C::SEM_OUT];
       float z2[C::SEM_LAYERS == 3 ? C::SEM_H : 1];
-      Lin::template fwd<C::GEO, C::SEM_H, true>(P.sem_w[0], P.sem_b[0], geo, z1);
-      if constexpr (C::SEM_LAYERS == 3) {
-        Lin::template fwd<C::SEM_H, C::SEM_H, true>(P.sem_w[1], P.sem_b[1], z1, z2);
-        Lin::template fwd<C::SEM_H, C::SEM_OUT, false>(P.sem_w[2], P.sem_b[2], z2, zo);
-      } else {
-        Lin::template fwd<C::SEM_H, C::SEM_OUT, false>(P.sem_w[1], P.sem_b[1], z1, zo);
-      }
+      semantic_fwd<C, TC>(P, geo, z1, z2, zo);
       FNR_PHASE(kPhRecompute);
       float dlg[1] = {d_logit};
       float dzo[C::SEM_OUT];
@@ -679,17 +638,8 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
     }
     // ---- colour branch ---------------------------------------------------------------------
     {
-      // cat[SH(dir), geo, appearance] -> MLP -> sigmoid (fruit_field.py:270-278)
-      float cin[C::COL_IN], c1[C::COL_H], c2[C::COL_H];
-      sh_degree4(d[0], d[1], d[2], cin);
-#pragma unroll
-      for (int i = 0; i < C::GEO; ++i) cin[C::SH + i] = geo[i];
-#pragma unroll
-      for (int i = 0; i < C::APP; ++i) cin[C::SH + C::GEO + i] = appv[i];
-      Lin::template fwd<C::COL_IN, C::COL_H, true>(P.col_w[0], P.col_b[0], cin, c1);
-      Lin::template fwd<C::COL_H, C::COL_H, true>(P.col_w[1], P.col_b[1], c1, c2);
-      float o3[3];
-      Lin::template fwd<C::COL_H, 3, false>(P.col_w[2], P.col_b[2], c2, o3);
+      float cin[C::COL_IN], c1[C::COL_H], c2[C::COL_H], o3[3];
+      colour_fwd<C, TC>(P, d, geo, appv, cin, c1, c2, o3);
       FNR_PHASE(kPhRecompute);
       float do3[3];
 #pragma unroll
@@ -752,19 +702,12 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
     }
     // ---- hash-table scatter -----------------------------------------------------------------
     if (valid) {
-      const uint32_t mask = (1u << F.log2T) - 1u;
       float2* gt = reinterpret_cast<float2*>(G.hash_table);
 #pragma unroll 1
       for (int l = 0; l < C::L; ++l) {
         const float g0 = denc[2 * l], g1 = denc[2 * l + 1];
         if (g0 == 0.f && g1 == 0.f) continue;
-        const LevelCell c = level_cell(pos, F.scalings[l]);
-        const uint32_t base = (uint32_t)l << F.log2T;
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const float w = corner_weight(c, k);
-          if (w != 0.f) atomicAdd(gt + corner_row(c, k, mask, base), make_float2(w * g0, w * g1));
-        }
+        level_scatter(gt, pos, F.scalings[l], l, F.log2T, g0, g1);
       }
     }
     FNR_PHASE(kPhScatter);
@@ -826,8 +769,7 @@ __global__ void __launch_bounds__(kThreads) simt_export_kernel(KField F, KParams
     float enc[C::ENC];
     hash_encode<C::L>(reinterpret_cast<const float2*>(P.hash_table), F.scalings, F.log2T, pos, enc);
     float appv[C::APP];
-#pragma unroll
-    for (int i = 0; i < C::APP; ++i) appv[i] = s_app[i];
+    load_appearance(P, FNR_APP_MEAN, 0, s_app, appv);
     Acts<C> a;
     field_mlps<C, TC>(P, enc, E.normal, appv, a);
     const float density = sel ? expf(a.out[0]) : 0.f;
@@ -903,13 +845,6 @@ __global__ void __launch_bounds__(kThreads) hash_indices_kernel(KField F, KRays 
 // ------------------------------------------------------------------------------------------
 // Launchers
 // ------------------------------------------------------------------------------------------
-static int grid_for(long long work_items, int per_block, int max_blocks) {
-  long long b = (work_items + per_block - 1) / per_block;
-  if (b < 1) b = 1;
-  if (b > max_blocks) b = max_blocks;
-  return (int)b;
-}
-
 int sm_count() {
   static int n = 0;
   if (!n) {
