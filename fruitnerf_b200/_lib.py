@@ -170,6 +170,17 @@ class AdamTensor(C.Structure):
     _fields_ = [("param", C.c_void_p), ("grad", C.c_void_p), ("exp_avg", C.c_void_p), ("exp_avg_sq", C.c_void_p), ("n", C.c_int64)]
 
 
+class FrameOutput(C.Structure):
+    _fields_ = [("image", C.c_void_p), ("kind", C.c_int32), ("auto_range", C.c_int32), ("near_plane", C.c_double),
+                ("far_plane", C.c_double)]
+
+
+FNR_CAMERA_PERSPECTIVE, FNR_CAMERA_FISHEYE, FNR_CAMERA_EQUIRECTANGULAR = 0, 1, 2
+FNR_FRAME_COLOR, FNR_FRAME_TURBO, FNR_FRAME_DEPTH = 0, 1, 2
+FNR_RANGE_AUTO_NEAR, FNR_RANGE_AUTO_FAR = 1, 2
+FNR_MAX_FRAME_OUTPUTS = 8
+FNR_COMPOSE_SCRATCH_FLOATS = FNR_MAX_FRAME_OUTPUTS * 256 * 2
+
 FNR_OPT_ADAM, FNR_OPT_RADAM = 0, 1
 FNR_MAX_ADAM_TENSORS = 48
 
@@ -206,6 +217,8 @@ EXPORTED_SYMBOLS = (
     "fnr_icp_scaled",
     "fnr_ward_cut",
     "fnr_hausdorff",
+    "fnr_camera_rays",
+    "fnr_compose_frame",
 )
 
 _lib = None
@@ -293,6 +306,10 @@ def load() -> C.CDLL:
     lib.fnr_ward_cut.argtypes = [vp, vp, i32, i32, vp, vp]
     lib.fnr_hausdorff.restype = C.c_int
     lib.fnr_hausdorff.argtypes = [vp, vp, vp, vp, i32, vp, vp]
+    lib.fnr_camera_rays.restype = C.c_int
+    lib.fnr_camera_rays.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i64, i32, vp, vp, vp]
+    lib.fnr_compose_frame.restype = C.c_int
+    lib.fnr_compose_frame.argtypes = [C.POINTER(FrameOutput), i32, vp, i32, i32, vp, vp, vp, vp]
     if lib.fnr_version() != ABI_VERSION:
         raise FruitNerfNativeError(f"ABI version mismatch: library reports {lib.fnr_version()}")
     _lib = lib

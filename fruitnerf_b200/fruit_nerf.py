@@ -240,7 +240,9 @@ class FruitModel(nn.Module):
         if self.colormap.device != semantic_labels.device:  # moved once, not per call (and never inside a graph capture)
             self.colormap = self.colormap.to(semantic_labels.device)
         cmap = self.colormap[semantic_labels]
-        outputs["semantics_colormap"] = cmap.repeat(1, 3) if self.test_mode == "inference" else cmap  # fruit_nerf.py:312 / 355
+        # fruit_nerf.py:312 / 355.  In inference mode the reference calls `.repeat(1, 3)` on this [R,1,3] gather, which raises
+        # (fewer repeat dims than tensor dims); its evident intent, an [R,3] colour per ray, is what inference mode returns here
+        outputs["semantics_colormap"] = cmap.reshape(R, -1) if self.test_mode == "inference" else cmap
         return outputs
 
     get_inference_outputs = get_outputs

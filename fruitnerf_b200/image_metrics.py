@@ -13,6 +13,7 @@ The reference takes these from third-party packages that are absent offline; wha
   normalised to its own min / max and faded to white by 1 - accumulation).  nerfstudio indexes matplotlib's 256-entry
   turbo table; matplotlib is absent here, so the table is rebuilt from the published degree-5 polynomial fit of turbo (close to
   the table in the interior, visibly off at the two ends): these are pictures for a viewer / logger, not parity outputs.
+  The `render` command's frame kernel (fnr_compose_frame) is handed this same table.
 * LPIPS needs the pretrained AlexNet weights torchmetrics downloads: not restated; the key is omitted.
 """
 from __future__ import annotations
@@ -92,8 +93,11 @@ def apply_colormap(image: Tensor) -> Tensor:
     return _turbo_table(image.device)[idx]
 
 
-def apply_depth_colormap(depth: Tensor, accumulation: Optional[Tensor] = None) -> Tensor:
-    near, far = float(torch.min(depth)), float(torch.max(depth))
+def apply_depth_colormap(depth: Tensor, accumulation: Optional[Tensor] = None, near_plane: Optional[float] = None,
+                         far_plane: Optional[float] = None) -> Tensor:
+    """``near_plane or min(depth)``, ``far_plane or max(depth)`` as nerfstudio writes it: a plane of 0 also means the
+    depth's own extreme."""
+    near, far = near_plane or float(torch.min(depth)), far_plane or float(torch.max(depth))
     d = torch.clip((depth - near) / (far - near + 1e-10), 0, 1)
     colored = apply_colormap(d)
     if accumulation is not None:

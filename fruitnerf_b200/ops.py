@@ -776,3 +776,88 @@ def hausdorff(a: Tensor, a_ranges, b: Tensor, b_ranges) -> Tensor:
     ra_d, rb_d = torch.from_numpy(np.ascontiguousarray(ra)).to(dev), torch.from_numpy(np.ascontiguousarray(rb)).to(dev)
     L.check(L.load().fnr_hausdorff(_ptr(pa), _ptr(ra_d), _ptr(pb), _ptr(rb_d), P, _ptr(out), _stream(dev)))
     return out
+
+
+# ======================================================================================================
+# Novel-view rendering (fnr_render.cu; nerfstudio ns-render, the reference's debug/render.py)
+# ======================================================================================================
+CAMERA_TYPES = {"perspective": L.FNR_CAMERA_PERSPECTIVE, "fisheye": L.FNR_CAMERA_FISHEYE, "equirectangular": L.FNR_CAMERA_EQUIRECTANGULAR}
+
+
+def camera_rays(c2w: Tensor, fx: Tensor, fy: Tensor, cx: Tensor, cy: Tensor, camera_type: str, height: int, width: int, frame: int,
+                pixel_start: int, num_pixels: int, out: Optional[Tuple[Tensor, Tensor]] = None) -> Tuple[Tensor, Tensor]:
+    """Origins and unit directions [n,3] of pixels [pixel_start, pixel_start + n) (row-major) of frame ``frame`` of a camera
+    set: c2w [F,3,4] (CUDA, fp32), per-frame fx / fy / cx / cy [F] (CUDA, taken as fp64).  ``out``: preallocated (origins, directions) with at
+    least n rows, of which the first n are written and returned."""
+    dev = _require_cuda(c2w, fx, fy, cx, cy)
+    if camera_type not in CAMERA_TYPES:
+        raise ValueError(f"camera_type must be one of {sorted(CAMERA_TYPES)}, got {camera_type!r}")
+    c2w = _f32c(c2w)
+    fx, fy, cx, cy = (t.to(torch.float64).contiguous() for t in (fx, fy, cx, cy))
+    F = c2w.shape[0]
+    if c2w.shape[1:] != (3, 4) or not (fx.numel() == fy.numel() == cx.numel() == cy.numel() == F):
+        raise ValueError(f"c2w must be [F,3,4] with F intrinsics each, got {tuple(c2w.shape)} and {fx.numel()} fx")
+    if out is None:
+        o = torch.empty((num_pixels, 3), dtype=torch.float32, device=dev)
+        d = torch.empty((num_pixels, 3), dtype=torch.float32, device=dev)
+    else:
+        _require_cuda(*out)
+        o, d = out[0][:num_pixels], out[1][:num_pixels]
+        if o.shape != (num_pixels, 3) or d.shape != (num_pixels, 3) or not (o.is_contiguous() and d.is_contiguous()):
+            raise ValueError("out buffers must be contiguous fp32 [>= n, 3]")
+    L.check(L.load().fnr_camera_rays(_ptr(c2w), _ptr(fx), _ptr(fy), _ptr(cx), _ptr(cy), F, CAMERA_TYPES[camera_type], int(height), int(width),
+                                     int(frame), int(pixel_start), int(num_pixels), _ptr(o), _ptr(d), _stream(dev)))
+    return o, d
+
+
+@dataclass
+class FrameImage:
+    """One requested output of a frame for ``compose_frame``: ``image`` [H*W, 3] (kind "color") or [H*W] / [H*W,1]
+    ("turbo", "depth"); depth ``near`` / ``far`` of None take the frame's own min / max."""
+
+    image: Tensor
+    kind: str
+    near: Optional[float] = None
+    far: Optional[float] = None
+
+
+_FRAME_KINDS = {"color": L.FNR_FRAME_COLOR, "turbo": L.FNR_FRAME_TURBO, "depth": L.FNR_FRAME_DEPTH}
+
+
+def compose_frame(images: Sequence[FrameImage], accumulation: Optional[Tensor], height: int, width: int, turbo: Tensor,
+                  scratch: Optional[Tensor] = None, out: Optional[Tensor] = None) -> Tensor:
+    """uint8 [H, W*k, 3] on the device: every image colour-mapped (nerfstudio apply_colormap / apply_depth_colormap),
+    side by side, quantised as uint8(clip(x, 0, 1) * 255 + 0.5).  ``turbo``: [256,3] CUDA fp32 table."""
+    k = len(images)
+    if not 1 <= k <= L.FNR_MAX_FRAME_OUTPUTS:
+        raise ValueError(f"compose_frame takes 1..{L.FNR_MAX_FRAME_OUTPUTS} images, got {k}")
+    dev = _require_cuda(turbo, accumulation, *[im.image for im in images])
+    P = height * width
+    arr = (L.FrameOutput * k)()
+    keep = []
+    any_auto = False
+    for j, im in enumerate(images):
+        if im.kind not in _FRAME_KINDS:
+            raise ValueError(f"unknown frame image kind {im.kind!r}")
+        t = _f32c(im.image)
+        want = 3 * P if im.kind == "color" else P
+        if t.numel() != want:
+            raise ValueError(f"{im.kind} image {j} has {t.numel()} values, expected {want} for {width}x{height}")
+        keep.append(t)
+        auto = (L.FNR_RANGE_AUTO_NEAR if im.near is None else 0) | (L.FNR_RANGE_AUTO_FAR if im.far is None else 0) if im.kind == "depth" else 0
+        any_auto |= auto != 0
+        arr[j] = L.FrameOutput(t.data_ptr(), _FRAME_KINDS[im.kind], auto, float(im.near or 0.0), float(im.far or 0.0))
+    acc = None if accumulation is None else _f32c(accumulation)
+    if acc is not None and acc.numel() != P:
+        raise ValueError(f"accumulation has {acc.numel()} values for {width}x{height}")
+    turbo = _f32c(turbo)
+    if turbo.numel() != 768:
+        raise ValueError("turbo table must be [256,3]")
+    if any_auto and scratch is None:
+        scratch = torch.empty(L.FNR_COMPOSE_SCRATCH_FLOATS, dtype=torch.float32, device=dev)
+    if out is None:
+        out = torch.empty((height, width * k, 3), dtype=torch.uint8, device=dev)
+    elif out.dtype != torch.uint8 or out.shape != (height, width * k, 3) or not out.is_contiguous():
+        raise ValueError(f"out must be contiguous uint8 [{height}, {width * k}, 3]")
+    L.check(L.load().fnr_compose_frame(arr, k, _ptr(acc), int(height), int(width), _ptr(turbo), _ptr(scratch), _ptr(out), _stream(dev)))
+    return out

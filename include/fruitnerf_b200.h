@@ -44,6 +44,9 @@
  *   fnr_icp_scaled, fnr_ward_cut, fnr_hausdorff
  *                        stage 3 of the fruit counting (clustering/clustering_base.py:261-429): scaled ICP of the fruit
  *                        template, Ward sub-centres for k = 2..6 and Hausdorff distances of each group to split
+ *   fnr_camera_rays, fnr_compose_frame
+ *                        the `render` command (debug/render.py, nerfstudio ns-render): camera-path rays and the
+ *                        per-frame colour-mapped uint8 image
  */
 #ifndef FRUITNERF_B200_H
 #define FRUITNERF_B200_H
@@ -443,6 +446,55 @@ int fnr_ward_cut(const double* points, const int64_t* offsets, int32_t num_segme
  * pair with an empty set. */
 int fnr_hausdorff(const double* a, const int64_t* a_ranges, const double* b, const int64_t* b_ranges, int32_t num_pairs, double* distances,
                   void* stream);
+
+/* ---- novel-view rendering (nerfstudio ns-render, the reference's debug/render.py launcher): camera rays of a camera
+ * path made on the device chunk by chunk, and the per-frame uint8 image of the requested outputs (fnr_render.cu). ---- */
+
+#define FNR_CAMERA_PERSPECTIVE 0
+#define FNR_CAMERA_FISHEYE 1
+#define FNR_CAMERA_EQUIRECTANGULAR 2
+
+/* Rays of pixels [pixel_start, pixel_start + num_pixels) (row-major, pixel centres) of frame `frame` of a camera set:
+ * c2w [num_frames,3,4] (OpenGL axes, DEVICE fp32), fx / fy / cx / cy [num_frames] (DEVICE fp64).  With
+ * (u, v) = ((x + 0.5 - cx) / fx, -(y + 0.5 - cy) / fy) the camera-space direction is
+ *   perspective      (u, v, -1)
+ *   fisheye          (u sin(t) / t, v sin(t) / t, -cos(t)), t = min(|(u, v)|, pi); (0, 0, -1) at t = 0
+ *   equirectangular  (-sin(a) sin(p), cos(p), -cos(a) sin(p)), a = -pi u, p = pi (0.5 - v)
+ * then rotated and normalised in fp32 without FMA.  cx / cy are rounded to fp32, the divisions by fx / fy are multiplies
+ * by fp32(1 / f) formed in fp64, and each 3-term sum is (a0 + a2) + a1: the op order torch's CUDA kernels give
+ * synthetic_scene.camera_rays with python-float intrinsics, so perspective
+ * rays are bit-identical to SyntheticCameras.generate_rays on the device.  origins / directions: DEVICE [num_pixels,3]
+ * fp32. */
+int fnr_camera_rays(const float* c2w, const double* fx, const double* fy, const double* cx, const double* cy, int32_t num_frames,
+                    int32_t camera_type, int32_t height, int32_t width, int32_t frame, int64_t pixel_start, int32_t num_pixels,
+                    float* origins, float* directions, void* stream);
+
+#define FNR_MAX_FRAME_OUTPUTS 8
+#define FNR_COMPOSE_PARTIALS 256
+/* floats of the DEVICE scratch fnr_compose_frame needs when a depth output takes its near / far from the frame */
+#define FNR_COMPOSE_SCRATCH_FLOATS (FNR_MAX_FRAME_OUTPUTS * FNR_COMPOSE_PARTIALS * 2)
+
+#define FNR_FRAME_COLOR 0 /* [H*W,3] image shown as is (nerfstudio apply_colormap of a 3-channel image) */
+#define FNR_FRAME_TURBO 1 /* [H*W] float through turbo: index long(clip(nan_to_num(v, 0), 0, 1) * 255) */
+#define FNR_FRAME_DEPTH 2 /* [H*W] depth: apply_depth_colormap, clip((d - near) * fp32(1 / (far - near + 1e-10)), 0, 1)
+                           * through turbo, then c * accumulation + (1 - accumulation) */
+#define FNR_RANGE_AUTO_NEAR 1
+#define FNR_RANGE_AUTO_FAR 2
+
+typedef struct fnr_frame_output {
+  const float* image;                /* DEVICE fp32, layout by kind */
+  int32_t kind;                      /* FNR_FRAME_* */
+  int32_t auto_range;                /* depth only, FNR_RANGE_AUTO_* bits: near / far taken from the frame's own min / max
+                                      * (NaN if any depth is NaN, as torch.min / torch.max) */
+  double near_plane, far_plane;      /* the others: near is rounded to fp32, far - near + 1e-10 is formed in fp64 */
+} fnr_frame_output;
+
+/* One frame of ns-render's _render_trajectory_video: the colour image of each output, side by side, quantised as
+ * uint8(clip(x, 0, 1) * 255 + 0.5) (NaN -> 0) into image: DEVICE [height, width * num_outputs, 3] uint8.  accumulation:
+ * DEVICE [H*W] fp32 (NULL: depth outputs are not blended).  turbo: DEVICE [256,3] fp32 colour table.  scratch: DEVICE
+ * float[FNR_COMPOSE_SCRATCH_FLOATS] (NULL when no output uses auto_range).  Exact: min / max do not depend on order. */
+int fnr_compose_frame(const fnr_frame_output* outputs, int32_t num_outputs, const float* accumulation, int32_t height, int32_t width,
+                      const float* turbo, float* scratch, uint8_t* image, void* stream);
 
 /* Hash-grid row indices (exact-integer parity hook): rows[N,L,8] in nerfstudio corner order for
  * the masked [0,1]^3 positions of the given samples; also writes positions[N,3] if non-NULL. */
