@@ -219,6 +219,8 @@ EXPORTED_SYMBOLS = (
     "fnr_hausdorff",
     "fnr_camera_rays",
     "fnr_compose_frame",
+    "fnr_pixel_batch_lens",
+    "fnr_camera_rays_lens",
 )
 
 _lib = None
@@ -310,6 +312,10 @@ def load() -> C.CDLL:
     lib.fnr_camera_rays.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i64, i32, vp, vp, vp]
     lib.fnr_compose_frame.restype = C.c_int
     lib.fnr_compose_frame.argtypes = [C.POINTER(FrameOutput), i32, vp, i32, i32, vp, vp, vp, vp]
+    lib.fnr_pixel_batch_lens.restype = C.c_int
+    lib.fnr_pixel_batch_lens.argtypes = [vp, vp, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]
+    lib.fnr_camera_rays_lens.restype = C.c_int
+    lib.fnr_camera_rays_lens.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i64, i32, vp, vp, vp]
     if lib.fnr_version() != ABI_VERSION:
         raise FruitNerfNativeError(f"ABI version mismatch: library reports {lib.fnr_version()}")
     _lib = lib

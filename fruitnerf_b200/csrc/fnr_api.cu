@@ -498,6 +498,25 @@ int fnr_pixel_batch(const float* rand, const float* c2w, const float* images, co
   return launch_pixel_batch(A, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int fnr_pixel_batch_lens(const float* rand, const float* c2w, const float* images, const float* masks, int32_t num_images, int32_t height,
+                         int32_t width, const float* fx, const float* fy, const float* cx, const float* cy, const float* distortion,
+                         int32_t camera_type, int32_t num_rays, float* origins, float* directions, int32_t* camera_indices, int64_t* indices,
+                         float* image, float* fruit_mask, void* stream) {
+  if (camera_type != FNR_CAMERA_PERSPECTIVE && camera_type != FNR_CAMERA_FISHEYE && camera_type != FNR_CAMERA_EQUIRECTANGULAR) {
+    set_error("fnr_pixel_batch_lens: unsupported camera_type %d", camera_type);
+    return FNR_ERR_UNSUPPORTED;
+  }
+  if (num_rays < 0 || num_images < 1 || height < 1 || width < 1 || !fx || !fy || !cx || !cy ||
+      (num_rays > 0 && (!rand || !c2w || !images || !masks || !origins || !directions || !camera_indices || !image || !fruit_mask))) {
+    set_error("invalid arguments to fnr_pixel_batch_lens (%d rays, %d images of %dx%d, intrinsics %s)", num_rays, num_images, width, height,
+              (fx && fy && cx && cy) ? "given" : "NULL");
+    return FNR_ERR_INVALID_ARGUMENT;
+  }
+  KPixelBatch A{num_rays, num_images, height, width, 0.f, 0.f, 0.f, 0.f, rand, c2w, images, masks, origins, directions, camera_indices,
+                indices, image, fruit_mask, fx, fy, cx, cy, distortion, camera_type};
+  return launch_pixel_batch(A, reinterpret_cast<cudaStream_t>(stream));
+}
+
 int fnr_spaced_bins(const float* base_bins, const float* t_rand, int32_t t_stride, const float* nears, const float* fars, int32_t num_rays,
                     int32_t num_samples, int32_t mode, float* bins, float* starts, float* ends, void* stream) {
   if (num_rays < 0 || num_samples < 1 || (mode != FNR_SPACING_UNIFORM && mode != FNR_SPACING_LINDISP_PIECEWISE) ||

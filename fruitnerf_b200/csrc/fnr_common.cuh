@@ -9,6 +9,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <math.h>
+#include <math_constants.h>
 #include "../../include/fruitnerf_b200.h"
 
 namespace fnr {
@@ -267,6 +268,96 @@ __device__ __forceinline__ bool median_chunk(float w, bool in, int c0, int lane,
   run_w += __shfl_sync(kFull, wincl, 31);
   if (m) median = c0 + __ffs(m) - 1;
   return m != 0;
+}
+
+// camera model ------------------------------------------------------------------------------
+// One definition of the lens for the training rays (pixel_batch_kernel) and the evaluation / render rays
+// (camera_rays_kernel); DESIGN.md section 4.3j.
+
+// [NS] camera_utils.radial_and_tangential_undistort(coords, [k1, k2, k3, k4, p1, p2], eps=1e-3, max_iterations=10):
+// Newton's method on the OpenCV model, exactly 10 steps and no convergence test, a zero step where |det| <= eps.  Run in
+// fp64 with every op rounded in the order of the expressions of data/camera_model.py, so that restatement reproduces it
+// bit for bit; (u, v) are rounded back to fp32.
+__device__ __forceinline__ void undistort_rt(const float* __restrict__ dist, float& u, float& v) {
+  const double k1 = dist[0], k2 = dist[1], k3 = dist[2], k4 = dist[3], p1 = dist[4], p2 = dist[5];
+  const double xd = u, yd = v;
+  const double tp1 = __dmul_rn(2.0, p1), tp2 = __dmul_rn(2.0, p2), sp1 = __dmul_rn(6.0, p1), sp2 = __dmul_rn(6.0, p2);
+  const double tk2 = __dmul_rn(2.0, k2), tk3 = __dmul_rn(3.0, k3);
+  double x = xd, y = yd;
+#pragma unroll 1
+  for (int it = 0; it < 10; ++it) {
+    const double r = __dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y));
+    const double d = __dadd_rn(1.0, __dmul_rn(r, __dadd_rn(k1, __dmul_rn(r, __dadd_rn(k2, __dmul_rn(r, __dadd_rn(k3, __dmul_rn(r, k4))))))));
+    const double x2 = __dmul_rn(2.0, x), y2 = __dmul_rn(2.0, y);
+    // residuals: x d + 2 p1 x y + p2 (r + 2 x^2) - xd and y d + 2 p2 x y + p1 (r + 2 y^2) - yd
+    const double fx = __dsub_rn(__dadd_rn(__dadd_rn(__dmul_rn(d, x), __dmul_rn(__dmul_rn(tp1, x), y)), __dmul_rn(p2, __dadd_rn(r, __dmul_rn(x2, x)))), xd);
+    const double fy = __dsub_rn(__dadd_rn(__dadd_rn(__dmul_rn(d, y), __dmul_rn(__dmul_rn(tp2, x), y)), __dmul_rn(p1, __dadd_rn(r, __dmul_rn(y2, y)))), yd);
+    // d'(r) = k1 + r (2 k2 + r (3 k3 + r 4 k4)) and the Jacobian of (fx, fy)
+    const double d_r = __dadd_rn(k1, __dmul_rn(r, __dadd_rn(tk2, __dmul_rn(r, __dadd_rn(tk3, __dmul_rn(__dmul_rn(r, 4.0), k4))))));
+    const double d_x = __dmul_rn(x2, d_r), d_y = __dmul_rn(y2, d_r);
+    const double fx_x = __dadd_rn(__dadd_rn(__dadd_rn(d, __dmul_rn(d_x, x)), __dmul_rn(tp1, y)), __dmul_rn(sp2, x));
+    const double fx_y = __dadd_rn(__dadd_rn(__dmul_rn(d_y, x), __dmul_rn(tp1, x)), __dmul_rn(tp2, y));
+    const double fy_x = __dadd_rn(__dadd_rn(__dmul_rn(d_x, y), __dmul_rn(tp2, y)), __dmul_rn(tp1, x));
+    const double fy_y = __dadd_rn(__dadd_rn(__dadd_rn(d, __dmul_rn(d_y, y)), __dmul_rn(tp2, x)), __dmul_rn(sp1, y));
+    const double den = __dsub_rn(__dmul_rn(fy_x, fx_y), __dmul_rn(fx_x, fy_y));
+    if (fabs(den) > 1e-3) {
+      x = __dadd_rn(x, __ddiv_rn(__dsub_rn(__dmul_rn(fx, fy_y), __dmul_rn(fy, fx_y)), den));
+      y = __dadd_rn(y, __ddiv_rn(__dsub_rn(__dmul_rn(fy, fx_x), __dmul_rn(fx, fy_x)), den));
+    }
+  }
+  u = __double2float_rn(x);
+  v = __double2float_rn(y);
+}
+
+// [NS] Cameras._generate_rays_from_coords: camera-space direction (OpenGL axes) of normalised image coordinates (u, v)
+__device__ __forceinline__ void camera_direction(int camera_type, float u, float v, float d[3]) {
+  if (camera_type == FNR_CAMERA_FISHEYE) {
+    // theta = clip(|(u, v)|, 0, pi); (u sin(theta) / theta, v sin(theta) / theta, -cos(theta)).  At theta = 0 the reference
+    // divides 0 by 0; that pixel is the optical axis (0, 0, -1) here.
+    const float theta = fminf(sqrtf(__fadd_rn(__fmul_rn(u, u), __fmul_rn(v, v))), CUDART_PI_F);
+    float s, c;
+    sincosf(theta, &s, &c);
+    const float k = theta > 0.f ? __fdiv_rn(s, theta) : 0.f;
+    d[0] = __fmul_rn(u, k);
+    d[1] = __fmul_rn(v, k);
+    d[2] = -c;
+  } else if (camera_type == FNR_CAMERA_EQUIRECTANGULAR) {
+    // theta = -pi u (azimuth), phi = pi (0.5 - v) (polar angle from +y)
+    const float theta = __fmul_rn(-CUDART_PI_F, u), phi = __fmul_rn(CUDART_PI_F, __fsub_rn(0.5f, v));
+    float st, ct, sp, cp;
+    sincosf(theta, &st, &ct);
+    sincosf(phi, &sp, &cp);
+    d[0] = -__fmul_rn(st, sp);
+    d[1] = cp;
+    d[2] = -__fmul_rn(ct, sp);
+  } else {
+    d[0] = u;
+    d[1] = v;
+    d[2] = -1.0f;
+  }
+}
+
+// The lens branch: pixel (x, y) of a camera with fp32 intrinsics and an optional [6] distortion -> camera-space direction.
+// The pixel step divides with __fdiv_rn, as the pinhole training rays do; equirectangular cameras are not undistorted.
+__device__ __forceinline__ void lens_direction(int x, int y, float fx, float fy, float cx, float cy, const float* __restrict__ dist,
+                                               int camera_type, float d[3]) {
+  float u = __fdiv_rn(__fsub_rn(__fadd_rn((float)x, 0.5f), cx), fx);
+  float v = -__fdiv_rn(__fsub_rn(__fadd_rn((float)y, 0.5f), cy), fy);
+  if (dist && camera_type != FNR_CAMERA_EQUIRECTANGULAR) undistort_rt(dist, u, v);
+  camera_direction(camera_type, u, v, d);
+}
+
+// origin and d = normalize(R d_cam) of a [3][4] row-major c2w: rounded products, 3-term sums left to right (the training rays)
+__device__ __forceinline__ void world_ray(const float* __restrict__ m, const float d[3], float* __restrict__ origin, float* __restrict__ dir) {
+  float w[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) w[k] = __fadd_rn(__fadd_rn(__fmul_rn(m[4 * k], d[0]), __fmul_rn(m[4 * k + 1], d[1])), __fmul_rn(m[4 * k + 2], d[2]));
+  const float n = fmaxf(sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(w[0], w[0]), __fmul_rn(w[1], w[1])), __fmul_rn(w[2], w[2]))), 1e-12f);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    origin[k] = m[4 * k + 3];
+    dir[k] = __fdiv_rn(w[k], n);
+  }
 }
 
 // host-side error plumbing -------------------------------------------------------------------

@@ -1,7 +1,8 @@
 // Small per-ray kernels around the fused field kernels -- the pieces of a training iteration that the reference
 // spreads over dozens of elementwise / reduction launches:
 //   pixel_batch_kernel     PixelSampler.sample + RayGenerator (fruit_nerf/data/fruit_datamanager.py:183-192; nerfstudio
-//                          pinhole Cameras.generate_rays): uniform (image, row, col) draws -> rays + targets
+//                          Cameras.generate_rays: a shared pinhole, or per-image intrinsics, lens distortion and the
+//                          fisheye / equirectangular models): uniform (image, row, col) draws -> rays + targets
 //   spaced_bins_kernel     SpacedSampler.generate_ray_samples: stratified bins in spacing space + the euclidean map
 //                          (UniformLinDispPiecewiseSampler / UniformSampler; fruit_nerf/components/ray_samplers.py:54-104)
 //   render_losses_kernel   MSELoss + BCEWithLogitsLoss(mean) + PSNR and their gradients (fruit_nerf.py:359-366, 396-399)
@@ -27,19 +28,17 @@ __global__ void __launch_bounds__(kThreads) pixel_batch_kernel(KPixelBatch A) {
     y = min(y, A.H - 1);
     x = min(x, A.W - 1);
     const float* m = A.c2w + 12 * (size_t)ci;  // [3][4] row-major
-    // pinhole, pixel centres: d_cam = ((x + 0.5 - cx) / fx, -(y + 0.5 - cy) / fy, -1); d = normalize(R d_cam)
-    const float dx = __fdiv_rn(__fsub_rn(__fadd_rn((float)x, 0.5f), A.cx), A.fx);
-    const float dy = -__fdiv_rn(__fsub_rn(__fadd_rn((float)y, 0.5f), A.cy), A.fy);
-    const float dz = -1.0f;
-    float v[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) v[k] = __fadd_rn(__fadd_rn(__fmul_rn(m[4 * k], dx), __fmul_rn(m[4 * k + 1], dy)), __fmul_rn(m[4 * k + 2], dz));
-    const float n = fmaxf(sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(v[0], v[0]), __fmul_rn(v[1], v[1])), __fmul_rn(v[2], v[2]))), 1e-12f);
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      A.origins[3 * r + k] = m[4 * k + 3];
-      A.directions[3 * r + k] = __fdiv_rn(v[k], n);
+    // pixel centres: d_cam = ((x + 0.5 - cx) / fx, -(y + 0.5 - cy) / fy, -1) for the pinhole; d = normalize(R d_cam)
+    float dc[3];
+    if (A.lens_fx) {
+      lens_direction(x, y, A.lens_fx[ci], A.lens_fy[ci], A.lens_cx[ci], A.lens_cy[ci], A.distortion ? A.distortion + 6 * (size_t)ci : nullptr,
+                     A.camera_type, dc);
+    } else {
+      dc[0] = __fdiv_rn(__fsub_rn(__fadd_rn((float)x, 0.5f), A.cx), A.fx);
+      dc[1] = -__fdiv_rn(__fsub_rn(__fadd_rn((float)y, 0.5f), A.cy), A.fy);
+      dc[2] = -1.0f;
     }
+    world_ray(m, dc, A.origins + 3 * r, A.directions + 3 * r);
     A.camera_indices[r] = ci;
     if (A.indices) {
       A.indices[3 * (size_t)r] = ci;

@@ -111,6 +111,10 @@ struct KPixelBatch {
   int64_t* indices;      // [R,3] (image, row, col) or NULL
   float* image;          // [R,3]
   float* fruit_mask;     // [R,1]
+  // lens cameras (fnr_pixel_batch_lens): per-image intrinsics in place of fx..cy, or all NULL for the shared pinhole
+  const float *lens_fx, *lens_fy, *lens_cx, *lens_cy;  // [N]
+  const float* distortion;  // [N,6] k1 k2 k3 k4 p1 p2, or NULL
+  int camera_type;
 };
 struct KSpacedBins {
   int R, S, mode;        // mode 0 = uniform, 1 = linear-in-disparity piecewise

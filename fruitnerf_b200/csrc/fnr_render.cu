@@ -1,6 +1,7 @@
 // Novel-view rendering of a trained model (the `render` command, nerfstudio ns-render):
 //   camera_rays_kernel     Cameras.generate_rays for a pixel range of one frame of a camera set (perspective, fisheye,
-//                          equirectangular; per-frame intrinsics), so a frame's rays are made chunk by chunk on the device
+//                          equirectangular; per-frame intrinsics; lens distortion), so a frame's rays are made chunk by
+//                          chunk on the device
 //   depth_range_kernel     per-block min / max of the depth outputs that take their near / far from the frame itself
 //   compose_frame_kernel   _render_trajectory_video's per-frame image: apply_colormap / apply_depth_colormap of every
 //                          requested output, concatenated side by side, quantised to uint8 as mediapy / PIL do
@@ -19,6 +20,9 @@ constexpr int kRangeBlocks = FNR_COMPOSE_PARTIALS;
 struct KCameraRays {
   const float* c2w;  // [F][3][4]
   const double *fx, *fy, *cx, *cy;  // [F]
+  // lens cameras (fnr_camera_rays_lens): fp32 intrinsics in place of fx..cy, or all NULL
+  const float *lens_fx, *lens_fy, *lens_cx, *lens_cy;  // [F]
+  const float* distortion;  // [F,6] or NULL
   int frame, camera_type, height, width;
   long long p0;
   int n;
@@ -32,6 +36,16 @@ __global__ void __launch_bounds__(kThreads) camera_rays_kernel(KCameraRays A) {
   const long long p = A.p0 + i;
   const int y = (int)(p / A.width), x = (int)(p % A.width);
   const float* m = A.c2w + 12 * (size_t)A.frame;  // [3][4] row-major
+  float d[3];
+  if (A.lens_fx) {
+    // the training rays' arithmetic throughout (pixel_batch_kernel), so the ray of pixel (frame, y, x) is bit-identical to
+    // the one a training batch draws for it
+    const int f = A.frame;
+    lens_direction(x, y, A.lens_fx[f], A.lens_fy[f], A.lens_cx[f], A.lens_cy[f], A.distortion ? A.distortion + 6 * (size_t)f : nullptr,
+                   A.camera_type, d);
+    world_ray(m, d, A.origins + 3 * (size_t)i, A.directions + 3 * (size_t)i);
+    return;
+  }
   // pixel centres: (u, v) = ((x + 0.5 - cx) / fx, -(y + 0.5 - cy) / fy) with python-float intrinsics, as torch's CUDA
   // kernels evaluate synthetic_scene.camera_rays: cx rounded to fp32 for the subtraction, the division a multiply by
   // fp32(1 / fx) formed in fp64
@@ -39,31 +53,7 @@ __global__ void __launch_bounds__(kThreads) camera_rays_kernel(KCameraRays A) {
   const float ifx = (float)(1.0 / A.fx[A.frame]), ify = (float)(1.0 / A.fy[A.frame]);
   const float u = __fmul_rn(__fsub_rn(__fadd_rn((float)x, 0.5f), cx), ifx);
   const float v = -__fmul_rn(__fsub_rn(__fadd_rn((float)y, 0.5f), cy), ify);
-  float d[3];
-  if (A.camera_type == FNR_CAMERA_FISHEYE) {
-    // theta = clip(|(u, v)|, 0, pi); (u sin(theta) / theta, v sin(theta) / theta, -cos(theta)).  At theta = 0 the reference
-    // divides 0 by 0; that pixel is the optical axis (0, 0, -1) here.
-    const float theta = fminf(sqrtf(__fadd_rn(__fmul_rn(u, u), __fmul_rn(v, v))), CUDART_PI_F);
-    float s, c;
-    sincosf(theta, &s, &c);
-    const float k = theta > 0.f ? __fdiv_rn(s, theta) : 0.f;
-    d[0] = __fmul_rn(u, k);
-    d[1] = __fmul_rn(v, k);
-    d[2] = -c;
-  } else if (A.camera_type == FNR_CAMERA_EQUIRECTANGULAR) {
-    // theta = -pi u (azimuth), phi = pi (0.5 - v) (polar angle from +y)
-    const float theta = __fmul_rn(-CUDART_PI_F, u), phi = __fmul_rn(CUDART_PI_F, __fsub_rn(0.5f, v));
-    float st, ct, sp, cp;
-    sincosf(theta, &st, &ct);
-    sincosf(phi, &sp, &cp);
-    d[0] = -__fmul_rn(st, sp);
-    d[1] = cp;
-    d[2] = -__fmul_rn(ct, sp);
-  } else {
-    d[0] = u;
-    d[1] = v;
-    d[2] = -1.0f;
-  }
+  camera_direction(A.camera_type, u, v, d);
   // d = normalize(R d_cam) as synthetic_scene.camera_rays runs on the device: rounded products, and torch's reduction of a
   // 3-long row (two lanes: elements 0 and 2 in one, 1 in the other) sums them as (a0 + a2) + a1, for the rotation and the norm
   float w[3];
@@ -200,24 +190,41 @@ using namespace fnr;
 
 extern "C" {
 
-int fnr_camera_rays(const float* c2w, const double* fx, const double* fy, const double* cx, const double* cy, int32_t num_frames,
-                    int32_t camera_type, int32_t height, int32_t width, int32_t frame, int64_t pixel_start, int32_t num_pixels,
-                    float* origins, float* directions, void* stream) {
+static int camera_rays(const char* name, const KCameraRays& A, int32_t num_frames, int32_t camera_type, int32_t height, int32_t width,
+                       int32_t frame, int64_t pixel_start, int32_t num_pixels, bool intrinsics, void* stream) {
   if (camera_type != FNR_CAMERA_PERSPECTIVE && camera_type != FNR_CAMERA_FISHEYE && camera_type != FNR_CAMERA_EQUIRECTANGULAR) {
-    set_error("fnr_camera_rays: unsupported camera_type %d", camera_type);
+    set_error("%s: unsupported camera_type %d", name, camera_type);
     return FNR_ERR_UNSUPPORTED;
   }
   if (num_frames < 1 || frame < 0 || frame >= num_frames || height < 1 || width < 1 || num_pixels < 0 || pixel_start < 0 ||
-      pixel_start + num_pixels > (int64_t)height * width ||
-      (num_pixels > 0 && (!c2w || !fx || !fy || !cx || !cy || !origins || !directions))) {
-    set_error("invalid arguments to fnr_camera_rays (frame %d of %d, %dx%d, pixels [%lld, %lld))", frame, num_frames, width, height,
+      pixel_start + num_pixels > (int64_t)height * width || (num_pixels > 0 && (!A.c2w || !intrinsics || !A.origins || !A.directions))) {
+    set_error("invalid arguments to %s (frame %d of %d, %dx%d, pixels [%lld, %lld))", name, frame, num_frames, width, height,
               (long long)pixel_start, (long long)pixel_start + num_pixels);
     return FNR_ERR_INVALID_ARGUMENT;
   }
   if (num_pixels == 0) return FNR_OK;
-  KCameraRays A{c2w, fx, fy, cx, cy, frame, camera_type, height, width, pixel_start, num_pixels, origins, directions};
   camera_rays_kernel<<<(num_pixels + kThreads - 1) / kThreads, kThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(A);
   return check_launch("camera_rays_kernel");
+}
+
+int fnr_camera_rays(const float* c2w, const double* fx, const double* fy, const double* cx, const double* cy, int32_t num_frames,
+                    int32_t camera_type, int32_t height, int32_t width, int32_t frame, int64_t pixel_start, int32_t num_pixels,
+                    float* origins, float* directions, void* stream) {
+  KCameraRays A{c2w, fx, fy, cx, cy, nullptr, nullptr, nullptr, nullptr, nullptr, frame, camera_type, height, width, pixel_start, num_pixels,
+                origins, directions};
+  return camera_rays("fnr_camera_rays", A, num_frames, camera_type, height, width, frame, pixel_start, num_pixels, fx && fy && cx && cy, stream);
+}
+
+int fnr_camera_rays_lens(const float* c2w, const float* fx, const float* fy, const float* cx, const float* cy, const float* distortion,
+                         int32_t num_frames, int32_t camera_type, int32_t height, int32_t width, int32_t frame, int64_t pixel_start,
+                         int32_t num_pixels, float* origins, float* directions, void* stream) {
+  if (!fx || !fy || !cx || !cy) {
+    set_error("fnr_camera_rays_lens: NULL intrinsics");
+    return FNR_ERR_INVALID_ARGUMENT;
+  }
+  KCameraRays A{c2w, nullptr, nullptr, nullptr, nullptr, fx, fy, cx, cy, distortion, frame, camera_type, height, width, pixel_start, num_pixels,
+                origins, directions};
+  return camera_rays("fnr_camera_rays_lens", A, num_frames, camera_type, height, width, frame, pixel_start, num_pixels, true, stream);
 }
 
 int fnr_compose_frame(const fnr_frame_output* outputs, int32_t num_outputs, const float* accumulation, int32_t height, int32_t width,

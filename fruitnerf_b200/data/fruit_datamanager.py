@@ -113,6 +113,8 @@ class FruitDataManager(nn.Module):
         from .synthetic_scene import camera_rays
 
         cams = ds.cameras
+        if cams.has_lens:
+            return self._lens_pixel_batch(ds, num_rays)
         N, H, W = len(ds), cams.height, cams.width
         dev = ds.images.device
         if dev.type == "cuda":  # one launch (fnr_pixel_batch) after the draw, instead of ~25 indexing / elementwise kernels
@@ -139,6 +141,37 @@ class FruitDataManager(nn.Module):
                            pixel_area=torch.full((num_rays, 1), 1.0 / (cams.fx * cams.fy), device=o.device), camera_indices=ci[:, None])
         batch = {"image": ds.images[ci, ys, xs], "fruit_mask": ds.fruit_masks[ci, ys, xs], "indices": idx}
         return bundle, batch
+
+    def _lens_pixel_batch(self, ds, num_rays: int) -> Tuple[RayBundle, Dict]:
+        """``_pixel_batch`` for lens cameras (per-image intrinsics, distortion, fisheye / equirectangular): the same draws, rays
+        from ``fnr_pixel_batch_lens`` on the device or from data/camera_model.py on the host.  pixel_area is 1 / (fx fy) of
+        each ray's camera."""
+        cams = ds.cameras
+        N, H, W = len(ds), cams.height, cams.width
+        dev = ds.images.device
+        fx, fy, cx, cy = cams.intrinsics()  # already [N] fp32 on the device after .to(device): no copy in the step
+        area = self.__dict__.setdefault("_lens_area_cache", {})
+        key = (id(ds), str(dev))
+        if key not in area:
+            area[key] = (ds, (1.0 / (fx.double() * fy.double())).float())  # ds held so that its id stays unique
+        inv_area = area[key][1]
+        if dev.type == "cuda":
+            from .. import ops
+
+            r = torch.rand((num_rays, 3), device=dev)
+            o, d, cam, idx, image, mask = ops.pixel_batch_lens(r, cams.camera_to_worlds, ds.images, ds.fruit_masks, fx, fy, cx, cy,
+                                                               cams.distortion_params, cams.camera_type)
+            bundle = RayBundle(origins=o, directions=d, pixel_area=inv_area[cam.long()][:, None], camera_indices=cam[:, None])
+            return bundle, {"image": image, "fruit_mask": mask, "indices": idx}
+        from .camera_model import lens_rays
+
+        r = torch.rand((num_rays, 3), device=dev, generator=self._generator())
+        idx = torch.minimum(torch.floor(r * torch.tensor([N, H, W], dtype=torch.float32)).long(), torch.tensor([N - 1, H - 1, W - 1]))
+        ci, ys, xs = idx[:, 0], idx[:, 1], idx[:, 2]
+        dist = cams.distortion_params
+        o, d = lens_rays(cams.camera_to_worlds[ci], fx[ci], fy[ci], cx[ci], cy[ci], None if dist is None else dist[ci], cams.camera_type, ys, xs)
+        bundle = RayBundle(origins=o.contiguous(), directions=d.contiguous(), pixel_area=inv_area[ci][:, None], camera_indices=ci[:, None])
+        return bundle, {"image": ds.images[ci, ys, xs], "fruit_mask": ds.fruit_masks[ci, ys, xs], "indices": idx}
 
     def next_train(self, step: int) -> Tuple[RayBundle, Dict]:
         self.train_count += 1

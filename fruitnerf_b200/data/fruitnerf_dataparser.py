@@ -8,8 +8,11 @@ train split with the remaining frames for eval) -> an in-memory data set (images
 ``scene_box``, ``metadata['semantics']``) that ``FruitDataManager`` keeps resident on the GPU.  Image decoding is host
 I/O done once at start-up; nothing here is on the per-iteration path.
 
-The kernels generate rays for ONE shared pinhole camera model (``fnr_pixel_batch``): per-frame intrinsics and non-zero
-distortion coefficients are rejected with a clear error instead of being silently ignored.
+By default the parser keeps to ONE shared pinhole camera model (``fnr_pixel_batch``): per-frame intrinsics and non-zero
+distortion coefficients are rejected with a clear error instead of being silently ignored.  With ``lens_distortion=True``
+it reads what the reference passes to nerfstudio's ``Cameras`` (fruitnerf_dataparser.py:86-137, 225-246): shared or
+per-frame intrinsics and distortion and the ``camera_model``, which ``fnr_pixel_batch_lens`` / ``fnr_camera_rays_lens``
+model on the device (DESIGN.md section 4.3j).
 """
 from __future__ import annotations
 
@@ -24,6 +27,7 @@ import torch
 from torch import Tensor
 
 from ..compat import InstantiateConfig, SceneBox, Semantics
+from .camera_model import CAMERA_MODEL_TO_TYPE, get_distortion_params
 from .synthetic_scene import SyntheticCameras, SyntheticFruitDataset
 
 MAX_AUTO_RESOLUTION = 1200  # fruitnerf_dataparser.py:39
@@ -42,6 +46,9 @@ class FruitNerfDataParserConfig(InstantiateConfig):
     center_method: Literal["poses", "focus", "none"] = "poses"
     auto_scale_poses: bool = True
     train_split_fraction: float = 0.9
+    lens_distortion: bool = False
+    """Read ``camera_model``, per-frame intrinsics and distortion coefficients (captured data sets).  Off: one shared
+    distortion-free pinhole, anything else refused, ``camera_model`` ignored."""
 
 
 @dataclass
@@ -204,10 +211,12 @@ class FruitNerf:
         assert len(semantic_filenames) == 0 or len(semantic_filenames) == len(image_filenames), (
             "Different number of image and semantic filenames. "
             "You should check that mask_path is specified for every frame (or zero frames) in transforms.json.")
-        for k in ("k1", "k2", "k3", "k4", "p1", "p2"):
-            vals = [float(meta[k])] if k in meta else [float(f[k]) for f in meta["frames"] if k in f]
-            if any(v != 0.0 for v in vals):
-                raise NotImplementedError(f"non-zero distortion coefficient {k}: the device ray generator is a pinhole model")
+        lens = self.config.lens_distortion
+        if not lens:
+            for k in ("k1", "k2", "k3", "k4", "p1", "p2"):
+                vals = [float(meta[k])] if k in meta else [float(f[k]) for f in meta["frames"] if k in f]
+                if any(v != 0.0 for v in vals):
+                    raise NotImplementedError(f"non-zero distortion coefficient {k}: the device ray generator is a pinhole model")
 
         # ---- split (fruitnerf_dataparser.py:155-187)
         has_split_files_spec = any(f"{s}_filenames" in meta for s in ("train", "val", "test"))
@@ -255,13 +264,23 @@ class FruitNerf:
                 return float(meta[k])
             vals = {per_frame[i][k] for i in indices}
             if len(vals) != 1:
+                if k in ("h", "w") and lens:
+                    raise NotImplementedError(f"per-frame image sizes ({k} differs between frames): the pixel sampler draws from one [N,H,W] image stack")
                 raise NotImplementedError(f"per-frame intrinsics ({k} differs between frames): the device ray generator takes one shared pinhole camera")
             return vals.pop()
 
         assert self.downscale_factor is not None
         r = 1.0 / self.downscale_factor  # Cameras.rescale_output_resolution
-        fx, fy, cx, cy = (intrinsic(k) * r for k in ("fl_x", "fl_y", "cx", "cy"))
         height, width = int(intrinsic("h") * r), int(intrinsic("w") * r)
+        if lens:
+            # fruitnerf_dataparser.py:225-246: shared values as python floats, per-frame ones as fp32 tensors of the split
+            idx_np = np.asarray(indices, dtype=np.int64)
+            fx, fy, cx, cy = (float(meta[k]) * r if shared[k] else torch.tensor([f[k] for f in per_frame], dtype=torch.float32)[idx_np] * r
+                              for k in ("fl_x", "fl_y", "cx", "cy"))
+            camera_type, distortion = _lens_model(meta, idx_np)
+        else:
+            fx, fy, cx, cy = (intrinsic(k) * r for k in ("fl_x", "fl_y", "cx", "cy"))
+            camera_type, distortion = "perspective", None
 
         metadata = {}
         if semantic_filenames:
@@ -284,7 +303,7 @@ class FruitNerf:
             masks = torch.stack([read_fruit_mask(p) for p in semantic_filenames])
         else:
             masks = torch.zeros(images.shape[0], height, width, 1)
-        cams = SyntheticCameras(poses_t[:, :3, :4].contiguous(), fx, fy, cx, cy, height, width)
+        cams = SyntheticCameras(poses_t[:, :3, :4].contiguous(), fx, fy, cx, cy, height, width, camera_type, distortion)
         return DataparserOutputs(image_filenames=image_filenames, cameras=cams, scene_box=scene_box, dataparser_scale=scale,
                                  dataparser_transform=transform, metadata=metadata, images=images, fruit_masks=masks)
 
@@ -311,6 +330,28 @@ class FruitNerf:
         if self.downscale_factor > 1:
             return data_dir / f"{downsample_folder_prefix}{self.downscale_factor}" / filepath.name
         return data_dir / filepath
+
+
+def _lens_model(meta: Dict, indices: np.ndarray) -> Tuple[str, Optional[Tensor]]:
+    """camera_type and the [N,6] distortion of the split ``indices`` (None when every coefficient is zero: the undistortion
+    is then the identity).  fruitnerf_dataparser.py:92-137, 236-246, including its test for shared coefficients: only
+    k1, k2, k3, p1, p2 at the top level make them shared (k4 alone does not), and then all six are read from the top."""
+    model = meta.get("camera_model", "OPENCV")
+    if model not in CAMERA_MODEL_TO_TYPE:
+        if model.startswith(("OMNIDIRECTIONALSTEREO", "VR180")):
+            raise NotImplementedError(f"camera_model {model!r}: stereo cameras are not supported")
+        raise ValueError(f"unknown camera_model {model!r} (known: {sorted(CAMERA_MODEL_TO_TYPE)})")
+    camera_type = CAMERA_MODEL_TO_TYPE[model]
+    keys = ("k1", "k2", "k3", "k4", "p1", "p2")
+    if any(k in meta for k in ("k1", "k2", "k3", "p1", "p2")):
+        dist = get_distortion_params(**{k: float(meta[k]) if k in meta else 0.0 for k in keys}).expand(len(indices), 6).contiguous()
+    else:
+        dist = torch.stack([get_distortion_params(**{k: float(f[k]) if k in f else 0.0 for k in keys}) for f in meta["frames"]])[indices]
+    if len(indices) == 0 or not bool((dist != 0).any()):
+        return camera_type, None
+    if not bool(torch.isfinite(dist).all()):
+        raise ValueError("distortion coefficients must be finite")
+    return camera_type, dist
 
 
 def load_fruit_datasets(config: FruitNerfDataParserConfig) -> Tuple[SyntheticFruitDataset, SyntheticFruitDataset, DataparserOutputs]:

@@ -16,7 +16,7 @@ import json
 import math
 import pathlib
 from dataclasses import dataclass, field
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, Optional, Tuple, Union
 
 import torch
 from torch import Tensor
@@ -131,28 +131,86 @@ def trace(geom: SceneGeometry, origins: Tensor, dirs: Tensor) -> Tuple[Tensor, T
 
 @dataclass
 class SyntheticCameras:
+    """Cameras of a data set.  ``fx`` / ``fy`` / ``cx`` / ``cy`` are python floats shared by every image (the pinhole the
+    synthetic scene and most captures use) or per-image [N] tensors; ``camera_type`` and ``distortion_params`` ([N,6] =
+    k1 k2 k3 k4 p1 p2, or None) describe the lens (data/camera_model.py)."""
+
     camera_to_worlds: Tensor  # [N,3,4]
-    fx: float
-    fy: float
-    cx: float
-    cy: float
+    fx: Union[float, Tensor]
+    fy: Union[float, Tensor]
+    cx: Union[float, Tensor]
+    cy: Union[float, Tensor]
     height: int
     width: int
+    camera_type: str = "perspective"
+    distortion_params: Optional[Tensor] = None
 
     def __len__(self):
         return int(self.camera_to_worlds.shape[0])
 
+    @property
+    def has_lens(self) -> bool:
+        """Anything but one shared distortion-free pinhole: these rays come from the lens kernels / camera_model."""
+        return self.camera_type != "perspective" or self.distortion_params is not None or any(
+            torch.is_tensor(v) for v in (self.fx, self.fy, self.cx, self.cy))
+
+    def intrinsics(self) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
+        """Per-image fx, fy, cx, cy [N] in fp32 on the cameras' device."""
+        N, dev = len(self), self.camera_to_worlds.device
+        return tuple(torch.as_tensor(v, dtype=torch.float32, device=dev).reshape(-1).expand(N).contiguous()
+                     for v in (self.fx, self.fy, self.cx, self.cy))
+
+    def subset(self, index) -> "SyntheticCameras":
+        pick = lambda v: v[index] if torch.is_tensor(v) else v  # noqa: E731
+        return SyntheticCameras(self.camera_to_worlds[index], pick(self.fx), pick(self.fy), pick(self.cx), pick(self.cy), self.height, self.width,
+                                self.camera_type, pick(self.distortion_params))
+
     def to(self, device):
-        return SyntheticCameras(self.camera_to_worlds.to(device), self.fx, self.fy, self.cx, self.cy, self.height, self.width)
+        if not self.has_lens:
+            return SyntheticCameras(self.camera_to_worlds.to(device), self.fx, self.fy, self.cx, self.cy, self.height, self.width)
+        # lens cameras keep per-image fp32 arrays on the device for the ray kernels; their values are checked here, once,
+        # because the training step (captured in a CUDA graph) must not read device memory back
+        from .camera_model import TYPE_TO_CAMERA_MODEL
+
+        N = len(self)
+        if self.camera_type not in TYPE_TO_CAMERA_MODEL:
+            raise ValueError(f"camera_type must be one of {sorted(TYPE_TO_CAMERA_MODEL)}, got {self.camera_type!r}")
+        fx, fy, cx, cy = (t.to(device) for t in self.intrinsics())
+        dist = self.distortion_params
+        if dist is not None:
+            dist = dist.to(device=device, dtype=torch.float32).contiguous()
+            if tuple(dist.shape) != (N, 6):
+                raise ValueError(f"distortion_params must be [{N},6], got {tuple(dist.shape)}")
+        checked = torch.stack([fx, fy, cx, cy], 1) if dist is None else torch.cat([torch.stack([fx, fy, cx, cy], 1), dist], 1)
+        if not bool(torch.isfinite(checked).all()) or not bool(((fx != 0) & (fy != 0)).all()):
+            raise ValueError("camera intrinsics and distortion must be finite, with non-zero focal lengths")
+        return SyntheticCameras(self.camera_to_worlds.to(device), fx, fy, cx, cy, self.height, self.width, self.camera_type, dist)
 
     def generate_rays(self, camera_index: int) -> RayBundle:
         """Full-image bundle [H,W] for evaluation (nerfstudio Cameras.generate_rays(camera_indices=i))."""
         dev = self.camera_to_worlds.device
-        ys, xs = torch.meshgrid(torch.arange(self.height, device=dev), torch.arange(self.width, device=dev), indexing="ij")
-        o, d = camera_rays(self.camera_to_worlds[camera_index], self.fx, self.fy, self.cx, self.cy, ys.reshape(-1), xs.reshape(-1))
         H, W = self.height, self.width
+        if self.has_lens:
+            fx, fy, cx, cy = self.intrinsics()
+            dist = self.distortion_params
+            if dev.type == "cuda":
+                from .. import ops
+
+                o, d = ops.camera_rays_lens(self.camera_to_worlds, fx, fy, cx, cy, dist, self.camera_type, H, W, camera_index, 0, H * W)
+            else:
+                from .camera_model import lens_rays
+
+                ys, xs = torch.meshgrid(torch.arange(H, device=dev), torch.arange(W, device=dev), indexing="ij")
+                i = camera_index
+                o, d = lens_rays(self.camera_to_worlds[i], fx[i], fy[i], cx[i], cy[i], None if dist is None else dist[i], self.camera_type,
+                                 ys.reshape(-1), xs.reshape(-1))
+            area = 1.0 / (float(fx[camera_index]) * float(fy[camera_index]))
+        else:
+            ys, xs = torch.meshgrid(torch.arange(H, device=dev), torch.arange(W, device=dev), indexing="ij")
+            o, d = camera_rays(self.camera_to_worlds[camera_index], self.fx, self.fy, self.cx, self.cy, ys.reshape(-1), xs.reshape(-1))
+            area = 1.0 / (self.fx * self.fy)
         return RayBundle(origins=o.reshape(H, W, 3).contiguous(), directions=d.reshape(H, W, 3).contiguous(),
-                         pixel_area=torch.full((H, W, 1), 1.0 / (self.fx * self.fy), device=dev),
+                         pixel_area=torch.full((H, W, 1), area, device=dev),
                          camera_indices=torch.full((H, W, 1), camera_index, dtype=torch.int64, device=dev))
 
 
@@ -178,9 +236,15 @@ class SyntheticFruitDataset:
 
 
 def make_apple_scene(num_images: int = 40, height: int = 160, width: int = 160, num_fruits: int = 12, seed: int = 0, radius: float = 1.0,
-                     elevations=(12.0, 30.0, 50.0), noise_std: float = 0.02, device="cpu") -> Tuple[SyntheticFruitDataset, SyntheticFruitDataset]:
+                     elevations=(12.0, 30.0, 50.0), noise_std: float = 0.02, device="cpu", camera_type: str = "perspective",
+                     distortion: Optional[Tensor] = None, intrinsics_jitter: float = 0.0) -> Tuple[SyntheticFruitDataset, SyntheticFruitDataset]:
     """(train, eval) data sets of the synthetic apple tree.  Cameras orbit at ``radius`` (inside the +/-1 box after the
-    dataparser's auto-scaling) on three elevation rings; every 10th image goes to the eval split (train_split_fraction 0.9)."""
+    dataparser's auto-scaling) on three elevation rings; every 10th image goes to the eval split (train_split_fraction 0.9).
+
+    A lens: ``camera_type`` ("perspective", "fisheye", "equirectangular"), ``distortion`` (k1 k2 k3 k4 p1 p2, shared [6]
+    or per image [N,6]) and ``intrinsics_jitter`` (each image's fx / fy / cx / cy scaled by 1 + jitter * U(-1, 1), seeded)
+    make lens cameras whose images are traced along the rays of data/camera_model.py.  The defaults give the shared
+    pinhole and the same scene bit for bit."""
     geom = make_geometry(num_fruits, seed)
     target = torch.tensor([0.0, 0.0, 0.02])
     poses = []
@@ -192,6 +256,14 @@ def make_apple_scene(num_images: int = 40, height: int = 160, width: int = 160, 
     c2w = torch.stack(poses).to(torch.float32)
     fx = fy = 1.1 * width
     cams = SyntheticCameras(c2w.to(device), fx, fy, width / 2.0, height / 2.0, height, width)
+    if camera_type != "perspective" or distortion is not None or intrinsics_jitter:
+        intr = torch.tensor([fx, fy, width / 2.0, height / 2.0], dtype=torch.float32).expand(num_images, 4)
+        if intrinsics_jitter:
+            gj = torch.Generator().manual_seed(seed + 777)
+            intr = intr * (1.0 + intrinsics_jitter * (2.0 * torch.rand(num_images, 4, generator=gj) - 1.0))
+        dist = None if distortion is None else torch.as_tensor(distortion, dtype=torch.float32).reshape(-1, 6).expand(num_images, 6).contiguous()
+        cams = SyntheticCameras(c2w.to(device), *(intr[:, k].contiguous().to(device) for k in range(4)), height, width, camera_type,
+                                None if dist is None else dist.to(device))
     imgs, masks = [], []
     for i in range(num_images):
         rb = cams.generate_rays(i)
@@ -212,9 +284,9 @@ def make_apple_scene(num_images: int = 40, height: int = 160, width: int = 160, 
     def subset(ix):
         sem = Semantics(filenames=[f"semantics/frame_{int(i):05d}.png" for i in ix], classes=["apple", "stuff"],
                         colors=torch.tensor([[255, 0, 0], [0, 0, 0]], dtype=torch.float32) / 255.0, mask_classes=["apple", "stuff"])
-        return SyntheticFruitDataset(images[ix], fruit_masks[ix],
-                                     SyntheticCameras(cams.camera_to_worlds[ix], fx, fy, cams.cx, cams.cy, height, width), scene_box,
-                                     {"semantics": sem}, geom, 1.0)
+        cam_ix = cams.subset(ix.to(cams.camera_to_worlds.device)) if cams.has_lens else SyntheticCameras(
+            cams.camera_to_worlds[ix], fx, fy, cams.cx, cams.cy, height, width)
+        return SyntheticFruitDataset(images[ix], fruit_masks[ix], cam_ix, scene_box, {"semantics": sem}, geom, 1.0)
 
     return subset(train_idx), subset(eval_idx)
 
@@ -235,7 +307,20 @@ def write_dataset(ds: SyntheticFruitDataset, out_dir) -> pathlib.Path:
         m[:3, :4] = ds.cameras.camera_to_worlds[i].cpu()
         frames.append({"file_path": f"images/frame_{i:05d}.png", "semantic_path": f"semantics/frame_{i:05d}.png",
                        "transform_matrix": m.tolist()})
-    meta = {"fl_x": ds.cameras.fx, "fl_y": ds.cameras.fy, "cx": ds.cameras.cx, "cy": ds.cameras.cy, "w": ds.cameras.width,
-            "h": ds.cameras.height, "camera_model": "OPENCV", "k1": 0.0, "k2": 0.0, "p1": 0.0, "p2": 0.0, "frames": frames}
+    cams = ds.cameras
+    if cams.has_lens:
+        # per-frame intrinsics and distortion, and the camera model, so that the lens survives the round trip
+        from .camera_model import TYPE_TO_CAMERA_MODEL
+
+        fxs, fys, cxs, cys = (t.cpu().tolist() for t in cams.intrinsics())
+        dist = None if cams.distortion_params is None else cams.distortion_params.cpu().tolist()
+        for i, f in enumerate(frames):
+            f.update({"fl_x": fxs[i], "fl_y": fys[i], "cx": cxs[i], "cy": cys[i]})
+            if dist is not None:
+                f.update(dict(zip(("k1", "k2", "k3", "k4", "p1", "p2"), dist[i])))
+        meta = {"w": cams.width, "h": cams.height, "camera_model": TYPE_TO_CAMERA_MODEL[cams.camera_type], "frames": frames}
+    else:
+        meta = {"fl_x": cams.fx, "fl_y": cams.fy, "cx": cams.cx, "cy": cams.cy, "w": cams.width,
+                "h": cams.height, "camera_model": "OPENCV", "k1": 0.0, "k2": 0.0, "p1": 0.0, "p2": 0.0, "frames": frames}
     (out / "transforms.json").write_text(json.dumps(meta, indent=1))
     return out / "transforms.json"

@@ -488,6 +488,32 @@ def pixel_batch(rand: Tensor, c2w: Tensor, images: Tensor, masks: Tensor, fx: fl
     return o, d, cam, idx, img, m
 
 
+def pixel_batch_lens(rand: Tensor, c2w: Tensor, images: Tensor, masks: Tensor, fx: Tensor, fy: Tensor, cx: Tensor, cy: Tensor,
+                     distortion: Optional[Tensor], camera_type: str):
+    """``pixel_batch`` for lens cameras (DESIGN.md section 4.3j): per-image fx / fy / cx / cy [N] and distortion [N,6] (k1 k2 k3 k4
+    p1 p2, or None), all fp32 on the device, and a camera type of ``CAMERA_TYPES``.  Same outputs as ``pixel_batch``.  Nothing
+    here reads device memory, so the call can be captured in a CUDA graph: the values are checked when the data set is
+    moved to the device (``SyntheticCameras.to``)."""
+    dev = _require_cuda(rand, c2w, images, masks, fx, fy, cx, cy, distortion)
+    if camera_type not in CAMERA_TYPES:
+        raise ValueError(f"camera_type must be one of {sorted(CAMERA_TYPES)}, got {camera_type!r}")
+    R = rand.shape[0]
+    N, H, W = images.shape[0], images.shape[1], images.shape[2]
+    fx, fy, cx, cy = (_f32c(t.reshape(-1)) for t in (fx, fy, cx, cy))
+    if not (fx.numel() == fy.numel() == cx.numel() == cy.numel() == N) or (distortion is not None and tuple(distortion.shape) != (N, 6)):
+        raise ValueError(f"lens cameras need [N] intrinsics and [N,6] distortion for N = {N} images")
+    distortion = None if distortion is None else _f32c(distortion)
+    rand, c2w, images, masks = _f32c(rand), _f32c(c2w), _f32c(images), _f32c(masks)
+    f32 = dict(dtype=torch.float32, device=dev)
+    o, d, img, m = torch.empty((R, 3), **f32), torch.empty((R, 3), **f32), torch.empty((R, 3), **f32), torch.empty((R, 1), **f32)
+    cam = torch.empty((R,), dtype=torch.int32, device=dev)
+    idx = torch.empty((R, 3), dtype=torch.int64, device=dev)
+    L.check(L.load().fnr_pixel_batch_lens(rand.data_ptr(), c2w.data_ptr(), images.data_ptr(), masks.data_ptr(), N, H, W, fx.data_ptr(),
+                                          fy.data_ptr(), cx.data_ptr(), cy.data_ptr(), _ptr(distortion), CAMERA_TYPES[camera_type], R,
+                                          o.data_ptr(), d.data_ptr(), cam.data_ptr(), idx.data_ptr(), img.data_ptr(), m.data_ptr(), _stream(dev)))
+    return o, d, cam, idx, img, m
+
+
 def spaced_bins(base_bins: Tensor, t_rand: Optional[Tensor], nears: Tensor, fars: Tensor, num_samples: int, mode: int):
     """SpacedSampler bins (spacing space) + euclidean starts / ends.  base_bins [S+1] (host-made linspace, already on the device)."""
     dev = _require_cuda(base_bins, nears, fars)
@@ -807,6 +833,27 @@ def camera_rays(c2w: Tensor, fx: Tensor, fy: Tensor, cx: Tensor, cy: Tensor, cam
             raise ValueError("out buffers must be contiguous fp32 [>= n, 3]")
     L.check(L.load().fnr_camera_rays(_ptr(c2w), _ptr(fx), _ptr(fy), _ptr(cx), _ptr(cy), F, CAMERA_TYPES[camera_type], int(height), int(width),
                                      int(frame), int(pixel_start), int(num_pixels), _ptr(o), _ptr(d), _stream(dev)))
+    return o, d
+
+
+def camera_rays_lens(c2w: Tensor, fx: Tensor, fy: Tensor, cx: Tensor, cy: Tensor, distortion: Optional[Tensor], camera_type: str, height: int,
+                     width: int, frame: int, pixel_start: int, num_pixels: int) -> Tuple[Tensor, Tensor]:
+    """``camera_rays`` for lens cameras: fp32 fx / fy / cx / cy [F] and distortion [F,6] or None on the device.  The ray of pixel
+    (frame, y, x) is bit-identical to the one ``pixel_batch_lens`` draws for it."""
+    dev = _require_cuda(c2w, fx, fy, cx, cy, distortion)
+    if camera_type not in CAMERA_TYPES:
+        raise ValueError(f"camera_type must be one of {sorted(CAMERA_TYPES)}, got {camera_type!r}")
+    c2w = _f32c(c2w)
+    F = c2w.shape[0]
+    fx, fy, cx, cy = (_f32c(t.reshape(-1)) for t in (fx, fy, cx, cy))
+    if c2w.shape[1:] != (3, 4) or not (fx.numel() == fy.numel() == cx.numel() == cy.numel() == F) or (
+            distortion is not None and tuple(distortion.shape) != (F, 6)):
+        raise ValueError(f"c2w must be [F,3,4] with F intrinsics each and [F,6] distortion, got {tuple(c2w.shape)} and {fx.numel()} fx")
+    distortion = None if distortion is None else _f32c(distortion)
+    o = torch.empty((num_pixels, 3), dtype=torch.float32, device=dev)
+    d = torch.empty((num_pixels, 3), dtype=torch.float32, device=dev)
+    L.check(L.load().fnr_camera_rays_lens(_ptr(c2w), _ptr(fx), _ptr(fy), _ptr(cx), _ptr(cy), _ptr(distortion), F, CAMERA_TYPES[camera_type],
+                                          int(height), int(width), int(frame), int(pixel_start), int(num_pixels), _ptr(o), _ptr(d), _stream(dev)))
     return o, d
 
 

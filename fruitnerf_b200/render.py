@@ -70,9 +70,10 @@ class CameraSet:
 
     @staticmethod
     def from_cameras(cams, indices: Optional[Sequence[int]] = None) -> "CameraSet":
-        """The pinhole cameras of a data set (``SyntheticCameras``), all of them or ``indices``."""
-        c2w = cams.camera_to_worlds if indices is None else cams.camera_to_worlds[list(indices)]
-        return CameraSet(c2w, cams.fx, cams.fy, cams.cx, cams.cy, cams.height, cams.width)
+        """Perspective, distortion-free cameras with the poses and intrinsics of a data set's cameras (``SyntheticCameras``,
+        shared or per-image intrinsics), all of them or ``indices``, as nerfstudio's camera paths build them."""
+        pick = (lambda v: v) if indices is None else (lambda v: v[list(indices)] if torch.is_tensor(v) else v)
+        return CameraSet(pick(cams.camera_to_worlds), pick(cams.fx), pick(cams.fy), pick(cams.cx), pick(cams.cy), cams.height, cams.width)
 
     def rescale_output_resolution(self, scale: float) -> "CameraSet":
         """nerfstudio Cameras.rescale_output_resolution: intrinsics times ``scale`` (fp32), sizes truncated."""

@@ -3,6 +3,12 @@ train -> held-out PSNR / fruit IoU -> uniform-volume export -> fruit count.  (Th
 against the CPU oracle lives in tests/test_gpu_training.py: the product never imports the oracle.)
 
     python -m fruitnerf_b200.scripts.train --steps 3000 --json gpurun_out/train_synthetic.json
+
+With ``--data`` it trains on a captured data folder (``transforms.json`` + images + fruit masks, with the lens model of
+its cameras) and evaluates on the folder's eval split, then leaves the run folder for ``ns-export-semantics``, ``count``
+and ``render``:
+
+    python -m fruitnerf_b200.scripts.train --data DATA --steps 30000 --output-dir RUN
 """
 from __future__ import annotations
 
@@ -11,6 +17,7 @@ import copy
 import json
 import os
 import time
+from pathlib import Path
 from typing import Dict, Optional
 
 import numpy as np
@@ -37,6 +44,38 @@ def synthetic_spec(method: str = "fruit_nerf", num_images: int = 40, image_size:
     if rays_per_batch:
         dm.train_num_rays_per_batch = rays_per_batch
     return spec
+
+
+def data_spec(data, method: str = "fruit_nerf", downscale_factor: Optional[int] = None, seed: int = 0,
+              schedule_steps: Optional[int] = None):
+    """The method's TrainerSpec pointed at a data folder (or its transforms.json), read with the lens model of its cameras."""
+    from ..data.fruitnerf_dataparser import FruitNerfDataParserConfig
+
+    spec = synthetic_spec(method, seed=seed, schedule_steps=schedule_steps)
+    dm = spec.pipeline.datamanager
+    dm.synthetic_scene = None
+    dm.dataparser = FruitNerfDataParserConfig(data=Path(data).resolve(), downscale_factor=downscale_factor, lens_distortion=True)
+    return spec
+
+
+def train_data(data, output_dir: str, steps: int = 3000, method: str = "fruit_nerf", device: str = "cuda:0", downscale_factor: Optional[int] = None,
+               log_every: int = 250, eval_every: int = 500, seed: int = 0, use_cuda_graph: bool = True, short_schedule: bool = True):
+    """Train on a data folder, evaluate on its eval split and write the run folder (config.yml, checkpoint)."""
+    torch.manual_seed(seed)
+    spec = data_spec(data, method, downscale_factor, seed, schedule_steps=steps if short_schedule else None)
+    trainer = Trainer(spec, device=device, output_dir=output_dir, use_cuda_graph=use_cuda_graph)
+    torch.cuda.synchronize()
+    t0 = time.time()
+    history = trainer.train(steps, log_every=log_every, eval_every=eval_every)
+    torch.cuda.synchronize()
+    train_s = time.time() - t0
+    cams = trainer.pipeline.datamanager.train_dataset.cameras
+    res = {"method": method, "data": str(Path(data).resolve()), "steps": steps, "cuda_graph": bool(trainer.use_cuda_graph),
+           "camera_type": cams.camera_type, "lens_distortion": cams.distortion_params is not None, "train_seconds": train_s,
+           "ms_per_iteration": 1e3 * train_s / steps, "history": history,
+           "eval": trainer.pipeline.get_average_eval_image_metrics(trainer.step), "checkpoint": str(trainer.save_checkpoint()),
+           "config": str(Path(output_dir) / "config.yml")}
+    return res
 
 
 def export_and_count(trainer: Trainer, points_per_side: int = 256, half_extent: float = 0.3) -> Dict:
@@ -148,10 +187,19 @@ def main(argv=None):
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--no-graph", action="store_true", help="enqueue every iteration op by op instead of replaying CUDA graphs")
     ap.add_argument("--json", default=None)
+    ap.add_argument("--data", default=None, help="train on a data folder (or its transforms.json) instead of the synthetic scene; "
+                    "needs --output-dir")
+    ap.add_argument("--downscale-factor", type=int, default=None, help="with --data: read the images_N folders (default: automatic)")
     a = ap.parse_args(argv)
-    res = train_synthetic(a.steps, a.method, image_size=a.image_size, num_images=a.num_images, num_fruits=a.num_fruits,
-                          points_per_side=a.points_per_side, output_dir=a.output_dir, use_cuda_graph=not a.no_graph,
-                          short_schedule=not a.stock_schedule, seed=a.seed)
+    if a.data is not None:
+        if a.output_dir is None:
+            ap.error("--data needs --output-dir: the run folder is what export, count and render read")
+        res = train_data(a.data, a.output_dir, a.steps, a.method, downscale_factor=a.downscale_factor, seed=a.seed,
+                         use_cuda_graph=not a.no_graph, short_schedule=not a.stock_schedule)
+    else:
+        res = train_synthetic(a.steps, a.method, image_size=a.image_size, num_images=a.num_images, num_fruits=a.num_fruits,
+                              points_per_side=a.points_per_side, output_dir=a.output_dir, use_cuda_graph=not a.no_graph,
+                              short_schedule=not a.stock_schedule, seed=a.seed)
     print(json.dumps({k: v for k, v in res.items() if k != "history"}))
     if a.json:
         os.makedirs(os.path.dirname(a.json) or ".", exist_ok=True)

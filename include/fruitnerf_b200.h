@@ -47,6 +47,9 @@
  *   fnr_camera_rays, fnr_compose_frame
  *                        the `render` command (debug/render.py, nerfstudio ns-render): camera-path rays and the
  *                        per-frame colour-mapped uint8 image
+ *   fnr_pixel_batch_lens, fnr_camera_rays_lens
+ *                        training and evaluation rays of captured data sets (fruit_nerf/data/fruitnerf_dataparser.py
+ *                        cameras): per-frame intrinsics, OpenCV lens distortion, fisheye and equirectangular models
  */
 #ifndef FRUITNERF_B200_H
 #define FRUITNERF_B200_H
@@ -279,6 +282,17 @@ int fnr_pixel_batch(const float* rand, const float* c2w, const float* images, co
                     float* directions, int32_t* camera_indices, int64_t* indices, float* image, float* fruit_mask,
                     void* stream);
 
+/* fnr_pixel_batch for captured cameras (DESIGN.md section 4.3j): the same draws, gathers and outputs, with per-image
+ * fx / fy / cx / cy [num_images] (DEVICE fp32, not NULL), optional distortion [num_images,6] = k1 k2 k3 k4 p1 p2 (DEVICE
+ * fp32, or NULL for none) and camera_type FNR_CAMERA_* (defined below).  With (u, v) = ((x + 0.5 - cx) / fx,
+ * -(y + 0.5 - cy) / fy) (fp32, correctly rounded divisions), (u, v) is undistorted by nerfstudio's
+ * radial_and_tangential_undistort (10 Newton steps in fp64; not for equirectangular) and mapped to a direction as
+ * fnr_camera_rays does.  Inputs are not checked for finiteness here: that is done once when the data set is loaded. */
+int fnr_pixel_batch_lens(const float* rand, const float* c2w, const float* images, const float* masks, int32_t num_images,
+                         int32_t height, int32_t width, const float* fx, const float* fy, const float* cx, const float* cy,
+                         const float* distortion, int32_t camera_type, int32_t num_rays, float* origins, float* directions,
+                         int32_t* camera_indices, int64_t* indices, float* image, float* fruit_mask, void* stream);
+
 #define FNR_SPACING_UNIFORM 0
 #define FNR_SPACING_LINDISP_PIECEWISE 1
 /* SpacedSampler.generate_ray_samples (components/ray_samplers.py:54-104; nerfstudio UniformLinDispPiecewiseSampler):
@@ -468,6 +482,13 @@ int fnr_hausdorff(const double* a, const int64_t* a_ranges, const double* b, con
 int fnr_camera_rays(const float* c2w, const double* fx, const double* fy, const double* cx, const double* cy, int32_t num_frames,
                     int32_t camera_type, int32_t height, int32_t width, int32_t frame, int64_t pixel_start, int32_t num_pixels,
                     float* origins, float* directions, void* stream);
+
+/* fnr_camera_rays for the lens cameras of a data set: fx / fy / cx / cy [num_frames] (DEVICE fp32, not NULL), distortion
+ * [num_frames,6] (DEVICE fp32, or NULL).  The arithmetic is fnr_pixel_batch_lens's (the pixel step a correctly rounded
+ * division, 3-term sums left to right), so the ray of pixel (frame, y, x) is bit-identical to the training ray drawn for it. */
+int fnr_camera_rays_lens(const float* c2w, const float* fx, const float* fy, const float* cx, const float* cy, const float* distortion,
+                         int32_t num_frames, int32_t camera_type, int32_t height, int32_t width, int32_t frame, int64_t pixel_start,
+                         int32_t num_pixels, float* origins, float* directions, void* stream);
 
 #define FNR_MAX_FRAME_OUTPUTS 8
 #define FNR_COMPOSE_PARTIALS 256
