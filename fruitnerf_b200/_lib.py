@@ -210,6 +210,7 @@ EXPORTED_SYMBOLS = (
     "fnr_radius_count",
     "fnr_voxel_down_sample",
     "fnr_dbscan",
+    "fnr_radius_count_multi",
     "fnr_cluster_sums",
     "fnr_knn_mean_distance",
     "fnr_estimate_normals",
@@ -294,6 +295,9 @@ def load() -> C.CDLL:
     lib.fnr_voxel_down_sample.argtypes = [vp, i64, f64p, f64p, f64, vp, vp, vp, sz, vp]
     lib.fnr_dbscan.restype = C.c_int
     lib.fnr_dbscan.argtypes = [vp, i64, f64p, f64p, f64, i32, vp, vp, vp, sz, vp]
+    i32p = C.POINTER(C.c_int32)
+    lib.fnr_radius_count_multi.restype = C.c_int
+    lib.fnr_radius_count_multi.argtypes = [vp, i64, f64p, f64p, f64p, i32p, i32, vp, vp, sz, vp]
     lib.fnr_cluster_sums.restype = C.c_int
     lib.fnr_cluster_sums.argtypes = [vp, vp, i64, i32, vp, vp, vp, sz, vp]
     lib.fnr_knn_mean_distance.restype = C.c_int

@@ -17,7 +17,7 @@ Where each stage runs depends on the input:
 """
 from __future__ import annotations
 
-from typing import Dict, List, Optional, Sequence, Tuple
+from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -589,6 +589,64 @@ def split_clusters(groups: Sequence[np.ndarray], template: np.ndarray, seed: int
             "icp_iterations": its}
 
 
+def load_obj_centres(path) -> np.ndarray:
+    """Ground-truth fruit centres from an OBJ file with one object per fruit (the synthetic trees' ``fruits.obj``,
+    clustering_base.py:67-111 load_obj_file): an ``o`` line starts a new object, each ``v`` line adds a vertex to the
+    current object, and a fruit's centre is the mean of its object's vertices.  [K,3] float64 in object order.
+
+    A file without any ``o`` line, a vertex before the first ``o`` line or an object without vertices raises
+    ValueError.  The reference crashes on the first (its vertex list does not exist yet), silently counts the vertices
+    before the first ``o`` as part of the first object, and takes the mean of an empty object as NaN."""
+    objects: List[List[List[float]]] = []
+    stray = 0  # line of the first vertex before any 'o' line
+    with open(path, "r") as f:
+        for num, line in enumerate(f, 1):
+            parts = line.split()
+            if not parts:
+                continue
+            if parts[0] == "o":
+                objects.append([])
+            elif parts[0] == "v":
+                if len(parts) < 4:
+                    raise ValueError(f"{path}:{num}: vertex with fewer than 3 coordinates")
+                if not objects:
+                    stray = stray or num
+                    continue
+                objects[-1].append([float(v) for v in parts[1:4]])
+    if not objects:
+        raise ValueError(f"{path}: no 'o' line: the file holds no fruit objects")
+    if stray:
+        raise ValueError(f"{path}:{stray}: vertex before the first 'o' line")
+    empty = [i for i, o in enumerate(objects) if not o]
+    if empty:
+        raise ValueError(f"{path}: object {empty[0]} has no vertices")
+    return np.stack([np.asarray(o, dtype=np.float64).mean(axis=0) for o in objects])
+
+
+def load_gt_centres(path) -> np.ndarray:
+    """Ground-truth fruit centres [K,3] float64 in the reference's formats, by file suffix:
+    - ``.obj``: one object per fruit (``load_obj_centres``);
+    - ``.ply``: a line set of 8-corner boxes as open3d writes it (Fuji's ``lineset_aligned.ply``), ascii or binary; the
+      centres are the means of each 8 consecutive vertices (clustering_base.py:459-462).  A vertex count that is not a
+      multiple of 8 raises ValueError;
+    - ``.npy``: an array of centres, as ``count --gt-centers`` reads it."""
+    from pathlib import Path
+
+    suffix = Path(path).suffix.lower()
+    if suffix == ".obj":
+        return load_obj_centres(path)
+    if suffix == ".ply":
+        from .export.exporter_utils import read_line_set_points
+
+        pts = read_line_set_points(path)
+        if pts.shape[0] % 8:
+            raise ValueError(f"{path}: {pts.shape[0]} line-set vertices are not whole 8-corner boxes")
+        return pts.reshape(-1, 8, 3).mean(axis=1)
+    if suffix == ".npy":
+        return np.load(path).astype(np.float64).reshape(-1, 3)
+    raise ValueError(f"{path}: ground truth must be .obj (fruit objects), .ply (line set of boxes) or .npy (centres)")
+
+
 def evaluate_count(centres: np.ndarray, gt_centres: np.ndarray, max_distance: float = 0.15) -> Dict:
     """The reference's score of a count (clustering_base.py:464-506): centres are visited in order and each takes the
     nearest remaining ground-truth centre if that is closer than ``max_distance`` (a true positive; the ground-truth
@@ -610,3 +668,223 @@ def evaluate_count(centres: np.ndarray, gt_centres: np.ndarray, max_distance: fl
     recall = tp / (tp + fn) if tp + fn else 0.0
     f1 = 2 * precision * recall / (precision + recall) if precision + recall else 0.0
     return {"TP": tp, "FP": fp, "FN": fn, "precision": precision, "recall": recall, "F1": f1}
+
+
+# ---- parameter sweeps: many counts of one cloud (clustering/run_clustering_sweep.py) -----------------------------------
+
+COUNT_ARGS = ("eps", "min_samples", "cluster_merge_distance", "down_sample", "remove_outliers_nb_points", "remove_outliers_radius", "seed")
+_COUNT_DEFAULTS = {"down_sample": 0.0, "remove_outliers_nb_points": 0, "remove_outliers_radius": 0.0, "seed": 0}
+MAX_RADIUS_RATIO, MAX_RADII = 4.0, 16  # what one ops.radius_count_multi call accepts
+
+
+def count_sweep(points, configs: Sequence[Dict], templates: Optional[Sequence[Optional[np.ndarray]]] = None,
+                on_stage: Optional[Callable[[str], None]] = None) -> List[Dict]:
+    """``count_fruits(points, **configs[i], template=templates[i])`` for every i: each result is exactly what that call
+    returns alone.  ``configs``: dicts of count_fruits' keyword arguments (``COUNT_ARGS``); ``templates``: one fruit
+    template (or None: no stage 3) per config, all None when omitted.
+
+    numpy input runs that loop.  A CUDA tensor shares the work the configs have in common: the radius counts of each
+    distinct outlier radius (one multi-radius walk, cap = the largest nb_points + 1), the voxel down-sampling of each
+    distinct filtered set, DBSCAN once per distinct (set, eps, min_samples), stage 2 once per distinct (set, eps,
+    min_samples, merge distance); stage 3's alpha shapes once per group content, its surface sample
+    once per (content, seed, group index), and one ICP launch per template, one Ward launch over every distinct sample
+    and one Hausdorff launch over every (template, sample) pair.  ``on_stage`` (device path only) is called with the
+    name of each stage as it ends: 'radius_count', 'voxel', 'dbscan', 'merge', 'alpha', 'match'."""
+    configs = [dict(c) for c in configs]
+    templates = [None] * len(configs) if templates is None else list(templates)
+    if len(templates) != len(configs):
+        raise ValueError(f"{len(templates)} templates for {len(configs)} configs")
+    for c in configs:
+        unknown = sorted(set(c) - set(COUNT_ARGS))
+        if unknown:
+            raise ValueError(f"count_sweep: unknown count_fruits arguments {unknown}")
+    if not _on_device(points):
+        return [count_fruits(points, **c, template=t) for c, t in zip(configs, templates)]
+    return _device_count_sweep(points, [{**_COUNT_DEFAULTS, **c} for c in configs], templates, on_stage or (lambda stage: None))
+
+
+def _radius_chunks(values: Sequence) -> List[List]:
+    """Ascending radii cut into runs one ``ops.radius_count_multi`` call accepts: at most MAX_RADII entries, the largest at
+    most MAX_RADIUS_RATIO times the first."""
+    chunks: List[List] = []
+    for r in sorted(values):
+        if chunks and len(chunks[-1]) < MAX_RADII and not r > MAX_RADIUS_RATIO * chunks[-1][0]:
+            chunks[-1].append(r)
+        else:
+            chunks.append([r])
+    return chunks
+
+
+def _device_count_sweep(points, configs: List[Dict], templates: List, on_stage) -> List[Dict]:
+    pts = ops.cluster_points(points)
+    if pts.shape[0] == 0:
+        return [_device_count_fruits(pts, c["eps"], c["min_samples"], c["cluster_merge_distance"], c["down_sample"],
+                                     c["remove_outliers_nb_points"], c["remove_outliers_radius"], t, c["seed"])
+                for c, t in zip(configs, templates)]
+
+    def outlier_key(c):  # None: no outlier removal
+        nb, r = c["remove_outliers_nb_points"], c["remove_outliers_radius"]
+        return (int(nb), float(r)) if nb > 0 and r > 0 else None
+
+    # radius counts: each distinct radius once, saturated at the largest nb_points + 1 it is used with
+    caps: Dict[float, int] = {}
+    for c in configs:
+        k = outlier_key(c)
+        if k is not None:
+            caps[k[1]] = max(caps.get(k[1], 0), k[0] + 1)
+    counts = {}
+    for chunk in _radius_chunks(list(caps)):
+        rows = ops.radius_count_multi(pts, chunk, [caps[r] for r in chunk])
+        counts.update({r: rows[i] for i, r in enumerate(chunk)})
+    filtered = {None: pts}
+    for c in configs:
+        k = outlier_key(c)
+        if k is not None and k not in filtered:
+            filtered[k] = pts[counts[k[1]] - 1 >= k[0]]  # = _device_remove_radius_outliers: min(count, cap) - 1 >= nb
+    on_stage("radius_count")
+
+    down = {}
+    for c in configs:
+        key = (outlier_key(c), float(c["down_sample"]))
+        if key not in down:
+            down[key] = ops.voxel_down_sample(filtered[key[0]], key[1])
+    on_stage("voxel")
+
+    # one DBSCAN per distinct (set, eps, min_samples); separate calls beat one shared-grid walk over several eps (DESIGN 4.3k)
+    labels = {}
+    for c in configs:
+        key = (outlier_key(c), float(c["down_sample"]))
+        prob = (float(c["eps"]), int(c["min_samples"]))
+        if down[key].shape[0] and (key, prob) not in labels:
+            labels[(key, prob)] = ops.dbscan(down[key], *prob)
+    on_stage("dbscan")
+
+    stage2, results, jobs = {}, [None] * len(configs), []
+    for i, (c, t) in enumerate(zip(configs, templates)):
+        key = (outlier_key(c), float(c["down_sample"]))
+        prob = (float(c["eps"]), int(c["min_samples"]))
+        s2 = (key, prob, float(c["cluster_merge_distance"]))
+        if s2 not in stage2:
+            dpts = down[key]
+            if dpts.shape[0] == 0:
+                stage2[s2] = [{"count": 0, "count_before_merge": 0, "centers": np.zeros((0, 3)), "num_points": 0}, None, []]
+            else:
+                lab, k = labels[(key, prob)]
+                sums, cnt = ops.cluster_sums(dpts, lab, k)
+                res, group_of = _merge_groups(sums.cpu().numpy(), cnt.cpu().numpy(), s2[2])
+                res["num_points"] = int(dpts.shape[0])
+                stage2[s2] = [res, (dpts, lab, group_of), None]
+        entry = stage2[s2]
+        if t is None:
+            results[i] = {**entry[0], "centers": entry[0]["centers"].copy()}  # as independent as separate calls
+            continue
+        if entry[2] is None:
+            entry[2] = _device_groups(*entry[1])
+        jobs.append((i, entry[0], entry[2], np.asarray(t, dtype=np.float64), int(c["seed"])))
+    on_stage("merge")
+    if jobs:
+        for i, res in _sweep_stage3(jobs, pts.device, on_stage):
+            results[i] = res
+    else:
+        on_stage("alpha")
+        on_stage("match")
+    return results
+
+
+def _sweep_stage3(jobs, device, on_stage):
+    """``_with_stage3`` for every job (index, stage-2 result, groups, template, seed), sharing the alpha shapes, the
+    surface samples and the device launches between the jobs.  Yields (index, result)."""
+    template_vol, shapes, samples = {}, {}, {}  # template bytes -> V_t; content -> (volumes, boundary); (content, seed, g) -> sample
+    plans = []
+    for i, res, groups, tmpl, seed in jobs:
+        tkey = tmpl.tobytes()
+        if tkey not in template_vol:
+            template_vol[tkey] = float(alpha_shape(tmpl, (ALPHA_VOLUME,))[0][0])
+        vt = template_vol[tkey]
+        decisions, picks = [], {}
+        for g, grp in enumerate(groups):
+            p64 = np.asarray(grp, dtype=np.float64).reshape(-1, 3)
+            content = (p64.shape[0], p64.tobytes())
+            skey = (content, seed, g)
+            if content not in shapes:
+                volumes, boundaries, sample = alpha_shape(p64, (ALPHA_VOLUME, ALPHA_SURFACE), seed=seed, group=g)
+                shapes[content] = (volumes, boundaries[-1])
+                samples[skey] = sample
+            elif skey not in samples:
+                samples[skey] = _surface_sample(p64, shapes[content][1], SURFACE_SAMPLES, seed, g)
+            volumes, sample = shapes[content][0], samples[skey]
+            if sample is None:  # as alpha_stage
+                decisions.append("one")
+            elif vt < SPLIT_RATIO * volumes[0]:
+                decisions.append("split")
+                picks[g] = skey
+            elif PRUNE_RATIO * vt > abs(volumes[0]):
+                decisions.append("prune")
+            else:
+                decisions.append("one")
+        plans.append((i, res, groups, tmpl, tkey, decisions, picks))
+    on_stage("alpha")
+
+    # the distinct samples to split (Ward: template-free) and, per template, the samples it is fitted to (ICP)
+    sample_keys = list(dict.fromkeys(k for p in plans for _, k in sorted(p[6].items())))
+    per_template: Dict[bytes, Tuple[np.ndarray, Dict]] = {}  # template -> (template, {sample key: None}), in first-use order
+    for p in plans:
+        per_template.setdefault(p[4], (p[3], {}))[1].update(dict.fromkeys(k for _, k in sorted(p[6].items())))
+    matched = _device_match_sweep([samples[k] for k in sample_keys], sample_keys, per_template, device) if sample_keys else {}
+    on_stage("match")
+
+    for i, res, groups, tmpl, tkey, decisions, picks in plans:
+        centers, per_group = [], np.zeros(len(groups), dtype=np.int64)
+        for g, (grp, dec) in enumerate(zip(groups, decisions)):  # split_clusters' assembly
+            if dec == "one":
+                centers.append(np.asarray(grp, dtype=np.float64).mean(axis=0)[None])
+                per_group[g] = 1
+            elif dec == "split":
+                T, cuts, d = matched[(tkey, picks[g])]
+                k = int(np.argmin(d)) + 1
+                per_group[g] = k
+                centers.append(transform_points(tmpl, T).mean(axis=0)[None] if k == 1 else cuts[CUT_OFFSETS[k - 2]:CUT_OFFSETS[k - 1]])
+        split = per_group[np.array([dec == "split" for dec in decisions], dtype=bool)]
+        extra, pruned = int((split - 1).sum()), int(sum(dec == "prune" for dec in decisions))
+        yield i, {**res, "count_after_merge": res["count"], "count": res["count"] + extra - pruned, "num_split_extra": extra,
+                  "num_pruned": pruned, "centers": np.concatenate(centers) if centers else np.zeros((0, 3))}
+
+
+def _device_match_sweep(sample_list: List[np.ndarray], sample_keys: List, per_template: Dict, device) -> Dict:
+    """``_device_match`` over several templates: one ICP launch per template on the samples it is fitted to, one Ward
+    launch over all samples, one Hausdorff launch over every (template, sample) pair.  ``per_template``: {template key:
+    (template, ordered sample keys)}.  Returns {(template key, sample
+    key): (T [4,4], sub-centres [20,3], distances [6])}."""
+    f64 = dict(dtype=torch.float64, device=device)
+    offsets = np.concatenate([[0], np.cumsum([s.shape[0] for s in sample_list])])
+    row = {k: j for j, k in enumerate(sample_keys)}
+    targets = torch.from_numpy(np.concatenate(sample_list)).to(**f64)
+    cuts = ops.ward_cut(targets, offsets)
+    fits, hyp, sizes, a_ranges, pairs = {}, [], [], [], []
+    for tkey, (tmpl, keys) in per_template.items():
+        if not keys:
+            continue
+        t = torch.from_numpy(tmpl).to(**f64)
+        sub = [sample_list[row[k]] for k in keys]
+        sub_offsets = np.concatenate([[0], np.cumsum([s.shape[0] for s in sub])])
+        inits = np.stack([s.mean(axis=0) for s in sub])  # match_candidates' initial translations
+        T, _, _, _ = ops.icp_scaled(t, torch.from_numpy(np.concatenate(sub)).to(**f64), sub_offsets, torch.from_numpy(inits).to(**f64))
+        x, y, z = t[:, 0], t[:, 1], t[:, 2]
+        R = T[:, :3, :]
+        fitted = torch.stack([((R[:, r, 0:1] * x + R[:, r, 1:2] * y) + R[:, r, 2:3] * z) + R[:, r, 3:4] for r in range(3)], dim=2)
+        T_host = T.cpu().numpy()
+        for b, k in enumerate(keys):
+            j = row[k]
+            pairs.append((tkey, k, T_host[b], j))
+            hyp.append(fitted[b])
+            sizes.append(t.shape[0])
+            for kk in range(2, MAX_FRUIT_PER_GROUP + 1):
+                centres = cuts[j, CUT_OFFSETS[kk - 2]:CUT_OFFSETS[kk - 1]]
+                hyp.append((t[None, :, :] + centres[:, None, :]).reshape(-1, 3))
+                sizes.append(kk * t.shape[0])
+            a_ranges.extend([[offsets[j], offsets[j + 1]]] * MAX_FRUIT_PER_GROUP)
+    b_offsets = np.concatenate([[0], np.cumsum(sizes)])
+    d = ops.hausdorff(targets, np.asarray(a_ranges, dtype=np.int64), torch.cat(hyp), np.stack([b_offsets[:-1], b_offsets[1:]], axis=1))
+    d = d.view(-1, MAX_FRUIT_PER_GROUP).cpu().numpy()
+    cuts_host = cuts.cpu().numpy()
+    return {(tkey, k): (T, cuts_host[j], d[p]) for p, (tkey, k, T, j) in enumerate(pairs)}

@@ -9,6 +9,15 @@
 // h = (15/16) r / sqrt(3): every pair of points inside one cell is closer than r, and a pair within r is at most two cells
 // apart on each axis (r / h = 1.85).  The 1/16 margin absorbs the rounding of the key arithmetic.
 //
+// The multi-radius call (fnr_radius_count_multi) answers R radii r_1..r_R on one grid whose side comes
+// from the smallest radius, h = cell_side(r_min): the own cell is still within every radius, and a larger radius walks
+// more rings.  The ring of radius r is ring(r) = floor(r/h + 1/16) + 1.  Derivation: the keys are floor(q) with q the
+// computed (p - lo) / h; check_extent bounds |p| / h by 2^40 and the extent by 2^21 cells, so each q is within 2^-12 of
+// its exact value and two points' q differ by at most r/h + 2^-11 < r/h + 1/16 when |dp| <= r on that axis (the fp64
+// predicate d2 <= r*r admits |dp| only 2^-50 r beyond r).  Two integers floor(q1) <= floor(q2) then differ by
+// D < r/h + 1/16 + 1, so D <= floor(r/h + 1/16) + 1.  For r = r_min this is the +-2 above (floor(1.85 + 0.06) + 1); the
+// call accepts r_max / r_min <= 4, i.e. r_max / h <= 7.4 and at most 8 rings.
+//
 // Distances are fp64 with explicit round-to-nearest intrinsics in x, y, z order, d2 = (dx*dx + dy*dy) + dz*dz <= r*r:
 // scikit-learn's KD-tree radius predicate bit for bit.  No host synchronisation; data-dependent sizes (cells, voxels,
 // clusters) stay in device memory.
@@ -66,21 +75,22 @@ __device__ __forceinline__ int lower_bound(const uint64_t* __restrict__ a, int n
   return lo;
 }
 
-// Calls f(cell, ring) for every occupied cell within +-2 cells of `key` on each axis, ring = Chebyshev distance in cells
-// (0 = the cell itself).  f returns false to stop the walk.
+// Calls f(cell, ring) for every occupied cell within +-reach cells of `key` on each axis, ring = Chebyshev distance in
+// cells (0 = the cell itself).  f returns false to stop the walk.  The single-radius kernels walk +-2; the multi-radius
+// count passes the ring of its largest radius (header comment).
 template <class F>
-__device__ __forceinline__ void for_each_near_cell(const Grid& g, int nc, uint64_t key, F&& f) {
+__device__ __forceinline__ void for_each_near_cell(const Grid& g, int nc, uint64_t key, F&& f, int reach = 2) {
   const long long cx = (long long)(key >> (2 * kAxisBits)), cy = (long long)((key >> kAxisBits) & kAxisMask),
                   cz = (long long)(key & kAxisMask);
-  for (int dx = -2; dx <= 2; ++dx) {
+  for (int dx = -reach; dx <= reach; ++dx) {
     const long long x = cx + dx;
     if (x < 0 || x >= kAxisCells) continue;
-    for (int dy = -2; dy <= 2; ++dy) {
+    for (int dy = -reach; dy <= reach; ++dy) {
       const long long y = cy + dy;
       if (y < 0 || y >= kAxisCells) continue;
-      const uint64_t hi = pack_key(x, y, cz + 2 < kAxisCells ? cz + 2 : kAxisCells - 1);
+      const uint64_t hi = pack_key(x, y, cz + reach < kAxisCells ? cz + reach : kAxisCells - 1);
       const int dxy = max(abs(dx), abs(dy));
-      for (int c = lower_bound(g.ukeys, nc, pack_key(x, y, cz > 2 ? cz - 2 : 0)); c < nc; ++c) {
+      for (int c = lower_bound(g.ukeys, nc, pack_key(x, y, cz > reach ? cz - reach : 0)); c < nc; ++c) {
         const uint64_t k = g.ukeys[c];
         if (k > hi) break;
         const int ring = max(dxy, (int)llabs((long long)(k & kAxisMask) - cz));
@@ -155,6 +165,52 @@ __global__ void __launch_bounds__(kThreads) radius_count_kernel(Grid g, double r
   cnt = min(cnt, cap);
   if (counts) counts[g.perm[j]] = cnt;
   if (core_sorted) core_sorted[j] = cnt >= cap;
+}
+
+// The radii of one multi-radius walk, passed by value (constant bank).  ring[k] = ring(r_k) of the header comment.
+constexpr int kMaxRadii = 16;
+struct Radii {
+  double r2[kMaxRadii];
+  int cap[kMaxRadii];
+  int ring[kMaxRadii];
+  int num;
+  int reach;  // the largest ring
+};
+
+// radius_count_kernel for R <= kR radii on one grid: each pair's d2 is computed once and compared with every r_k^2 whose
+// ring reaches its cell.  A point stops once every count has reached its cap.  counts: [R,n] rows in input order.
+template <int kR>
+__global__ void __launch_bounds__(kThreads) radius_count_multi_kernel(Grid g, Radii rs, int* __restrict__ counts) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= g.n) return;
+  const int own = g.cell_of[j];
+  const int whole = g.cstart[own + 1] - g.cstart[own];
+  int cnt[kR];
+  int open = 0;  // counts still below their cap
+#pragma unroll
+  for (int k = 0; k < kR; ++k) {
+    cnt[k] = whole;
+    if (k < rs.num && whole < rs.cap[k]) ++open;
+  }
+  if (open) {
+    const double px = g.x[j], py = g.y[j], pz = g.z[j];
+    for_each_near_cell(g, *g.ncells, g.keys[j], [&](int c, int ring) {
+      if (ring == 0) return true;
+      for (int m = g.cstart[c], e = g.cstart[c + 1]; m < e; ++m) {
+        const double d2 = dist2(px, py, pz, g.x[m], g.y[m], g.z[m]);
+#pragma unroll
+        for (int k = 0; k < kR; ++k)
+          if (k < rs.num && ring <= rs.ring[k] && cnt[k] < rs.cap[k] && d2 <= rs.r2[k] && ++cnt[k] == rs.cap[k]) --open;
+        if (!open) return false;
+      }
+      return true;
+    }, rs.reach);
+  }
+  const size_t n = (size_t)g.n;
+#pragma unroll
+  for (int k = 0; k < kR; ++k) {
+    if (k < rs.num) counts[k * n + g.perm[j]] = min(cnt[k], rs.cap[k]);
+  }
 }
 
 // ---- DBSCAN ---------------------------------------------------------------------------------------------------------
@@ -844,6 +900,57 @@ int build_grid(const double* pts, int n, const double* lo, double h, const Scrat
 
 double cell_side(double r) { return kCellShrink * r / std::sqrt(3.0); }
 
+// ---- multi-radius count ---------------------------------------------------------------------------------------------
+constexpr double kMaxRadiusRatio = 4.0;  // r_max / r_min: at most 8 rings (header comment)
+
+// Checks R radii (`what_r`: their name) and caps and fills the walk parameters for the grid of side
+// h = cell_side(r_min); *r_min receives r_min.
+int make_radii(const char* what, const char* what_r, const double* radii, const int32_t* caps, int32_t num, Radii* rs, double* r_min) {
+  if (num < 1 || !radii || !caps) {
+    set_error("%s: %d radii with %s radii / caps; at least one, with non-NULL host arrays, is needed", what, num,
+              radii && caps ? "" : "NULL ");
+    return FNR_ERR_INVALID_ARGUMENT;
+  }
+  if (num > kMaxRadii) {
+    set_error("%s: %d radii; at most %d are supported", what, num, kMaxRadii);
+    return FNR_ERR_UNSUPPORTED;
+  }
+  double lo = radii[0], hi = radii[0];
+  for (int k = 0; k < num; ++k) {
+    if (!(radii[k] > 0.0) || !std::isfinite(radii[k]) || caps[k] < 1) {
+      set_error("%s: %s %d is %g with cap %d; %s must be positive and finite and caps >= 1", what, what_r, k, radii[k], caps[k], what_r);
+      return FNR_ERR_INVALID_ARGUMENT;
+    }
+    lo = std::fmin(lo, radii[k]);
+    hi = std::fmax(hi, radii[k]);
+  }
+  if (hi > kMaxRadiusRatio * lo) {
+    set_error("%s: largest %s %g is %g times the smallest %g; at most %g is supported", what, what_r, hi, hi / lo, lo, kMaxRadiusRatio);
+    return FNR_ERR_UNSUPPORTED;
+  }
+  const double h = cell_side(lo);
+  *rs = Radii{};
+  rs->num = num;
+  for (int k = 0; k < num; ++k) {
+    rs->r2[k] = radii[k] * radii[k];
+    rs->cap[k] = caps[k];
+    rs->ring[k] = (int)std::floor(radii[k] / h + 1.0 / 16.0) + 1;
+    rs->reach = std::max(rs->reach, rs->ring[k]);
+  }
+  *r_min = lo;
+  return FNR_OK;
+}
+
+int launch_radius_count_multi(const Grid& g, int n, const Radii& rs, int* counts, cudaStream_t st) {
+  const int nb = grid_for(n, kThreads, INT_MAX);
+  if (rs.num <= 1) radius_count_multi_kernel<1><<<nb, kThreads, 0, st>>>(g, rs, counts);
+  else if (rs.num <= 2) radius_count_multi_kernel<2><<<nb, kThreads, 0, st>>>(g, rs, counts);
+  else if (rs.num <= 4) radius_count_multi_kernel<4><<<nb, kThreads, 0, st>>>(g, rs, counts);
+  else if (rs.num <= 8) radius_count_multi_kernel<8><<<nb, kThreads, 0, st>>>(g, rs, counts);
+  else radius_count_multi_kernel<kMaxRadii><<<nb, kThreads, 0, st>>>(g, rs, counts);
+  return check_launch("radius_count_multi_kernel");
+}
+
 // Cell side of the kNN grid, from n, k and the bounds alone (no device read-back): the side at which k points would
 // share a cell if the n points filled the bounding box evenly, taken over the box itself and over its largest face and
 // longest edge (the largest of the three, so flat and thin clouds get cells sized for their own dimension).  It is then
@@ -997,6 +1104,29 @@ int fnr_dbscan(const double* points, int64_t num_points, const double* lo, const
   if (int rc = check_cuda(cub::DeviceScan::ExclusiveSum(s.cub, tb, s.flag, s.cid, n, st), "cub ExclusiveSum (cluster ids)")) return rc;
   label_kernel<<<nb, kThreads, 0, st>>>(g, s.core, s.cmin, s.parent, s.cid, s.flag, e2, labels, num_clusters);
   return check_launch("label_kernel");
+}
+
+int fnr_radius_count_multi(const double* points, int64_t num_points, const double* lo, const double* hi, const double* radii,
+                           const int32_t* caps, int32_t num_radii, int32_t* counts, void* scratch, size_t scratch_bytes, void* stream) {
+  const char* what = "fnr_radius_count_multi";
+  if (int rc = check_points(what, points, num_points, lo, hi)) return rc;
+  Radii rs;
+  double r_min = 0.0;
+  if (int rc = make_radii(what, "radius", radii, caps, num_radii, &rs, &r_min)) return rc;
+  if (num_points > 0 && !counts) {
+    set_error("%s: NULL counts", what);
+    return FNR_ERR_INVALID_ARGUMENT;
+  }
+  const int n = (int)num_points;
+  if (n == 0) return FNR_OK;
+  const double h = cell_side(r_min);
+  if (int rc = check_extent(what, "smallest radius", r_min, h, lo, hi)) return rc;
+  Scratch s;
+  if (int rc = bind_scratch(what, n, scratch, scratch_bytes, &s)) return rc;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  Grid g;
+  if (int rc = build_grid(points, n, lo, h, s, st, &g)) return rc;
+  return launch_radius_count_multi(g, n, rs, counts, st);
 }
 
 int fnr_cluster_sums(const double* points, const int32_t* labels, int64_t num_points, int32_t num_clusters, double* sums,

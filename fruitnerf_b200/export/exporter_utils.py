@@ -241,3 +241,65 @@ def read_ply(path):
     if {"red", "green", "blue"} <= set(vertex.dtype.names):
         colors = np.stack([vertex["red"], vertex["green"], vertex["blue"]], axis=1).astype(np.float64) / 255.0
     return points, colors
+
+
+def read_line_set_points(path) -> np.ndarray:
+    """The vertices of a PLY line set as open3d's write_line_set produces it -> [N,3] float64.
+
+    A ``vertex`` element with float or double x/y/z (other scalar vertex properties are skipped by their declared type)
+    and any further elements (open3d's ``edge`` element, list properties included), which are not read.  Both ``ascii``
+    and ``binary_little_endian`` files are read.  ``read_ply`` keeps refusing such files: they are no point cloud."""
+    with open(path, "rb") as f:
+        if f.readline().strip() != b"ply":
+            raise ValueError(f"{path}: not a PLY file")
+        fmt, elements = None, []
+        while True:
+            line = f.readline()
+            if not line:
+                raise ValueError(f"{path}: PLY header has no end_header")
+            tok = line.decode("ascii", "replace").split()
+            if not tok or tok[0] in ("comment", "obj_info"):
+                continue
+            if tok[0] == "end_header":
+                break
+            if tok[0] == "format":
+                fmt = tok[1]
+            elif tok[0] == "element":
+                elements.append((tok[1], int(tok[2]), []))
+            elif tok[0] == "property":
+                if not elements:
+                    raise ValueError(f"{path}: property before any element")
+                kind = "list" if tok[1] == "list" else _PLY_TYPES.get(tok[1])
+                if kind is None:
+                    raise ValueError(f"{path}: unknown PLY type '{tok[1]}'")
+                elements[-1][2].append((tok[-1], kind))
+        if fmt not in ("ascii", "binary_little_endian"):
+            raise ValueError(f"{path}: only ascii and binary_little_endian PLY are supported, got {fmt}")
+        vertex = None
+        for name, count, props in elements:  # the elements before the vertices are skipped row by row
+            if name == "vertex" or count:
+                if any(kind == "list" for _, kind in props):
+                    if name == "vertex":
+                        raise ValueError(f"{path}: list property in the vertex element")
+                    raise ValueError(f"{path}: element '{name}' with list properties before the vertices")
+            if fmt == "ascii":
+                rows = [f.readline().split() for _ in range(count)]
+                if name != "vertex":
+                    continue
+                if any(len(r) != len(props) for r in rows):
+                    raise ValueError(f"{path}: vertex rows do not have {len(props)} values")
+                table = np.array(rows, dtype=np.float64).reshape(count, len(props))
+                vertex = {p: table[:, i] for i, (p, _) in enumerate(props)}
+            else:
+                dt = np.dtype(props)
+                data = f.read(count * dt.itemsize)
+                if name != "vertex":
+                    continue
+                if len(data) != count * dt.itemsize:
+                    raise ValueError(f"{path}: file ends inside the vertex element")
+                rec = np.frombuffer(data, dtype=dt, count=count)
+                vertex = {p: rec[p] for p in dt.names}
+            break
+    if vertex is None or not {"x", "y", "z"} <= set(vertex):
+        raise ValueError(f"{path}: no vertex x/y/z")
+    return np.stack([vertex["x"], vertex["y"], vertex["z"]], axis=1).astype(np.float64)

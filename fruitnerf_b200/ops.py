@@ -654,6 +654,27 @@ def dbscan(points: Tensor, eps: float, min_samples: int) -> Tuple[Tensor, int]:
     return labels, int(num.item())
 
 
+def _host_radii(radii, caps, what: str):
+    """(double[R], int32[R], R) host arrays of the multi-radius calls; the library checks the values."""
+    r, c = [float(v) for v in radii], [int(v) for v in caps]
+    if len(r) != len(c):
+        raise ValueError(f"{what}: {len(r)} radii for {len(c)} caps")
+    return (C.c_double * max(len(r), 1))(*r), (C.c_int32 * max(len(c), 1))(*c), len(r)
+
+
+def radius_count_multi(points: Tensor, radii: Sequence[float], caps: Sequence[int]) -> Tensor:
+    """int32 [R,n]: row k is ``radius_count(points, radii[k], caps[k])``, bit for bit, from one grid walk (1 <= R <= 16,
+    max(radii) <= 4 min(radii))."""
+    pts = cluster_points(points)
+    n, dev = pts.shape[0], pts.device
+    r, c, R = _host_radii(radii, caps, "radius_count_multi")
+    counts = torch.empty((R, n), dtype=torch.int32, device=dev)
+    lo, hi = _bounds(pts)
+    scratch = _cluster_scratch(n, dev)
+    L.check(L.load().fnr_radius_count_multi(_ptr(pts), n, lo, hi, r, c, R, _ptr(counts), _ptr(scratch), scratch.numel(), _stream(dev)))
+    return counts
+
+
 def cluster_sums(points: Tensor, labels: Tensor, num_clusters: int) -> Tuple[Tensor, Tensor]:
     """(fp64 coordinate sums [K,3], int32 point counts [K]) of the labels 0..K-1 (deterministic)."""
     pts = cluster_points(points)

@@ -2,12 +2,14 @@
 (clustering/run_clustering.py with clustering/clustering_base.py), i.e. radius-outlier removal, voxel down-sampling,
 DBSCAN and the merge of cluster centres closer than ``--cluster-merge-distance``, then, with ``--template``, the split of
 groups of touching fruit and the pruning of fragments by template matching (stage 3).  ``--gt-centers`` scores the
-centres against ground truth (TP / FP / FN, precision, recall, F1).  The defaults are the reference's real-tree
+centres against ground truth (TP / FP / FN, precision, recall, F1); ``--gt-cluster`` reads the reference's ground-truth
+files (an OBJ of fruit objects or a PLY line set of boxes) as well as .npy.  The defaults are the reference's real-tree
 parameters (clustering/config_real.py).
 
     python -m fruitnerf_b200.scripts.count --pcd OUT/semantic_colormap.ply --json OUT/count.json
     python -m fruitnerf_b200.scripts.count --pcd OUT/semantic_colormap.ply --template apple.ply --template-size 0.7 \
         --gt-centers gt_centers.npy
+    python -m fruitnerf_b200.scripts.count --pcd OUT/semantic_colormap.ply --gt-cluster fruits.obj
 
 The kernels need a CUDA device; without one the script fails (there is no CPU fallback).
 """
@@ -20,7 +22,7 @@ import os
 import numpy as np
 import torch
 
-from ..clustering import count_fruits, evaluate_count, load_template
+from ..clustering import count_fruits, evaluate_count, load_gt_centres, load_template
 from ..export.exporter_utils import read_ply
 
 
@@ -39,9 +41,14 @@ def parse_args(argv=None) -> argparse.Namespace:
                     "e.g. 0.7 for apples and 1.1 for pears)")
     ap.add_argument("--gt-centers", default=None, help=".npy of ground-truth fruit centres [K,3]: adds TP / FP / FN / precision / "
                     "recall / F1 (a centre matches the nearest unmatched one closer than 0.15)")
+    ap.add_argument("--gt-cluster", default=None, help="ground truth in the reference's formats (clustering.load_gt_centres): "
+                    ".obj (one object per fruit), .ply (line set of 8-corner boxes) or .npy (centres); scored as --gt-centers")
     ap.add_argument("--device", default="cuda:0", help="CUDA device to count on (cuda or cuda:N)")
     ap.add_argument("--json", default=None, help="also write the result to this file")
-    return ap.parse_args(argv)
+    a = ap.parse_args(argv)
+    if a.gt_centers is not None and a.gt_cluster is not None:
+        ap.error("--gt-centers and --gt-cluster are alternatives: give one ground truth")
+    return a
 
 
 def count_cloud(a: argparse.Namespace) -> dict:
@@ -52,6 +59,8 @@ def count_cloud(a: argparse.Namespace) -> dict:
     points, _ = read_ply(a.pcd)
     template = load_template(a.template, a.template_size) if a.template else None
     gt = np.load(a.gt_centers).astype(np.float64).reshape(-1, 3) if a.gt_centers else None
+    if a.gt_cluster:
+        gt = load_gt_centres(a.gt_cluster)
     res = count_fruits(torch.from_numpy(points).to(a.device), eps=a.eps, min_samples=a.min_samples,
                        cluster_merge_distance=a.cluster_merge_distance, down_sample=a.down_sample,
                        remove_outliers_nb_points=a.remove_outliers_nb_points, remove_outliers_radius=a.remove_outliers_radius,

@@ -38,6 +38,9 @@
  *   fnr_radius_count, fnr_voxel_down_sample, fnr_dbscan, fnr_cluster_sums
  *                        stages 1-2 of the fruit counting (clustering/clustering_base.py:138-143, 183-259):
  *                        radius-outlier removal, voxel down-sampling, DBSCAN, the sums of the centre merge
+ *   fnr_radius_count_multi
+ *                        radius counts for several radii on one grid: the parameter sweeps of
+ *                        clustering/run_clustering_sweep.py
  *   fnr_backproject_select, fnr_knn_mean_distance, fnr_estimate_normals
  *                        the `pointcloud` export (fruit_nerf/scripts/exporter.py:124-129, nerfstudio ExportPointCloud):
  *                        back-projection and selection of rendered rays, statistical outlier removal, normal estimation
@@ -396,6 +399,15 @@ int fnr_voxel_down_sample(const double* points, int64_t num_points, const double
  * labels: DEVICE [n] int32; *num_clusters: DEVICE int32. */
 int fnr_dbscan(const double* points, int64_t num_points, const double* lo, const double* hi, double eps, int32_t min_samples,
                int32_t* labels, int32_t* num_clusters, void* scratch, size_t scratch_bytes, void* stream);
+
+/* counts[k*n + i] = fnr_radius_count(radius = radii[k], cap = caps[k]) counts[i], bit for bit, for k < num_radii, from
+ * one grid whose cell side comes from the smallest radius (a larger radius walks the rings it needs): the outlier counts
+ * of parameter sweeps (clustering.count_sweep).  radii / caps: HOST arrays of 1 <= num_radii <= 16 entries, every
+ * radius positive and finite, every cap >= 1 (FNR_ERR_INVALID_ARGUMENT otherwise; more than 16 entries or a largest
+ * radius more than 4 times the smallest return FNR_ERR_UNSUPPORTED).  The 2^21-cells-per-axis limit applies to the
+ * smallest radius.  counts: DEVICE [num_radii, n] int32.  Scratch: fnr_cluster_scratch_bytes(n). */
+int fnr_radius_count_multi(const double* points, int64_t num_points, const double* lo, const double* hi, const double* radii,
+                           const int32_t* caps, int32_t num_radii, int32_t* counts, void* scratch, size_t scratch_bytes, void* stream);
 
 /* Per-cluster fp64 coordinate sums [num_clusters,3] and point counts [num_clusters] of labels in [0, num_clusters) -- the
  * inputs of the centre merge (clustering_base.py:209-259).  Deterministic: the same input gives the same bits. */
