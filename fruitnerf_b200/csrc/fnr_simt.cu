@@ -143,9 +143,14 @@ __device__ __forceinline__ void tile_weight_grad(float* __restrict__ sX, float* 
 
 constexpr int cmax(int a, int b) { return a > b ? a : b; }
 
-// How the field kernels evaluate a Linear layer W [N][K]: forward y = act(W x + b), input gradient dx = W^T dy and
-// weight gradient dW = dY^T X over the CTA's tile.  TC = false: per thread in fp32 on the CUDA cores (the exact device
-// reference).  TC = true: block-wide on the tensor cores (fnr_wgmma.cuh; every thread of the 128-thread CTA must take part).
+// The field's Linear layers.  The first six are the small family's tensor-core layers in the order of its resident
+// weight image; kSem2 exists in the big family only.
+enum Slot { kBase0, kBase1, kSem0, kSem1, kCol0, kCol1, kHead, kCol2, kSem2 };
+
+// How the field kernels evaluate a Linear layer W [N][K] (SLOT: which one): forward y = act(W x + b), input gradient
+// dx = W^T dy and weight gradient dW = dY^T X over the tile.  TC = false: per thread in fp32 on the CUDA cores (the exact
+// device reference).  TC = true: warpgroup-wide on the tensor cores with the weight tile staged from global memory at
+// every step (fnr_wgmma.cuh; every thread of the 128-thread CTA must take part).
 template <class C, bool TC>
 struct Layers {
   // the 1- and 3-wide output heads (64 MACs per point) stay in exact fp32 on the CUDA cores on both paths
@@ -161,14 +166,14 @@ struct Layers {
     extern __shared__ __align__(128) uint8_t wg_smem[];
     return wg_smem;
   }
-  template <int K, int N, bool RELU>
+  template <int SLOT, int K, int N, bool RELU>
   static __device__ __forceinline__ void fwd(const float* __restrict__ W, const float* __restrict__ b, const float (&x)[K], float (&y)[N]) {
     if constexpr (tensor(N))
       wg::linear<C::MAXW, C::MAXW, K, N, RELU>(dyn_smem(), W, b, x, y);
     else
       linear_fwd<K, N, RELU>(W, b, x, y);
   }
-  template <int K, int N>
+  template <int SLOT, int K, int N>
   static __device__ __forceinline__ void dx(const float* __restrict__ W, const float (&dy)[N], float (&dxv)[K]) {
     if constexpr (tensor(N))
       wg::linear_dx<C::MAXW, C::MAXW, K, N>(dyn_smem(), W, dy, dxv);
@@ -176,12 +181,169 @@ struct Layers {
       linear_bwd_input<K, N>(W, dy, dxv);
     FNR_PHASE(kPhDx);
   }
-  template <int K, int N>
+  template <int SLOT, int K, int N>
   static __device__ __forceinline__ void dw(float* sX, float* sY, const float (&x)[K], const float (&dy)[N], float* gW, float* gb) {
     if constexpr (tensor(N))
       wg::weight_grad<K, N>(dyn_smem(), x, dy, gW, gb);
     else
       tile_weight_grad<K, N>(sX, sY, x, dy, gW, gb);
+    FNR_PHASE(kPhDw);
+  }
+};
+
+// The small family's tensor-core backward: CTAs of two warpgroups, each taking its own 128-point tiles.  Per CTA, the six
+// tensor-core layers are split once into a resident bf16 hi / lo image (the K-major tiles rowgemm stages, so the recompute
+// runs the forward's bytes and MMA sequence; dx reads the same image MN-major), and the weight gradients of all eight
+// layers are accumulated in fp32 in shared memory and added to the global gradient once, when the CTA ends.
+// Dynamic shared memory: weight image | accumulators | locks | per-warpgroup step tiles | per-warpgroup warp partials.
+// The resident plan of the small family: shape of every slot, offsets of its weight image (six tensor-core layers) and of
+// its fp32 gradient accumulator (all eight; wg::DwAcc layout for the tensor-core layers, [N][K] then [N] for the heads).
+namespace resident {
+using C = CfgSmall;
+static_assert(C::SEM_LAYERS == 2, "resident plan of the two-layer semantic MLP");
+constexpr int kSlots = 8;  // kBase0 .. kCol2
+constexpr int kImageSlots = 6;
+constexpr int K(int s) {
+  return s == kBase0 ? C::ENC : s == kBase1 ? C::BASE_H : s == kSem0 ? C::GEO : s == kSem1 ? C::SEM_H : s == kCol0 ? C::COL_IN
+                                                                                                      : s == kHead ? C::SEM_OUT : C::COL_H;
+}
+constexpr int N(int s) {
+  return s == kBase0 ? C::BASE_H : s == kBase1 ? C::BASE_OUT : s == kSem0 ? C::SEM_H : s == kSem1 ? C::SEM_OUT : s == kHead ? 1
+                                                                                                      : s == kCol2 ? 3 : C::COL_H;
+}
+constexpr bool tensor(int n) { return n >= 8; }
+constexpr int img_bytes(int s) { return 2 * wg::padn(N(s)) * wg::pad16(K(s)) * 2; }
+constexpr int img_off(int s) { return s == 0 ? 0 : img_off(s - 1) + img_bytes(s - 1); }
+constexpr int acc_floats(int s) { return tensor(N(s)) ? (N(s) + 15) / 16 * 32 * (wg::padn(K(s)) / 2) + N(s) : N(s) * K(s) + N(s); }
+constexpr int acc_off(int s) { return s == 0 ? 0 : acc_off(s - 1) + (acc_floats(s - 1) + 3) / 4 * 4; }  // float4-aligned
+constexpr int align128(int b) { return (b + 127) / 128 * 128; }
+}  // namespace resident
+
+struct ResidentLayers {
+  using C = CfgSmall;
+  static constexpr int kGroups = 2;
+  static constexpr int kSlots = resident::kSlots;
+  static constexpr int K(int s) { return resident::K(s); }
+  static constexpr int N(int s) { return resident::N(s); }
+  static constexpr bool tensor(int n) { return resident::tensor(n); }
+  static constexpr int img_off(int s) { return resident::img_off(s); }
+  static constexpr int acc_off(int s) { return resident::acc_off(s); }
+  static constexpr int kImageBytes = resident::img_off(resident::kImageSlots);
+  static constexpr int kAccOff = kImageBytes;
+  static constexpr int kLockOff = kAccOff + resident::acc_off(kSlots) * 4;
+  static constexpr int kStepOff = resident::align128(kLockOff + kSlots * 4);
+  static constexpr int kPartOff = kStepOff + kGroups * wg::kResidentStepBytes;
+  static constexpr int kBytes = kPartOff + kGroups * 4 * wg::kWarpPartial * 4;
+  static_assert(kImageBytes == 64 * 1024, "16384 split weights");
+
+  static __device__ __forceinline__ uint8_t* smem() {
+    extern __shared__ __align__(128) uint8_t wg_smem[];
+    return wg_smem;
+  }
+  static __device__ __forceinline__ uint8_t* step() { return smem() + kStepOff + wg::group() * wg::kResidentStepBytes; }
+  static __device__ __forceinline__ float* part() { return reinterpret_cast<float*>(smem() + kPartOff) + wg::group() * 4 * wg::kWarpPartial; }
+  template <int S>
+  static __device__ __forceinline__ float* acc() {
+    constexpr int off = acc_off(S);
+    return reinterpret_cast<float*>(smem() + kAccOff) + off;
+  }
+  static __device__ __forceinline__ int* lock(int s) { return reinterpret_cast<int*>(smem() + kLockOff) + s; }
+  static __device__ __forceinline__ const float* weight(const KParams& P, int s) {
+    return s == kBase0 ? P.base_w[0] : s == kBase1 ? P.base_w[1] : s == kSem0 ? P.sem_w[0] : s == kSem1 ? P.sem_w[1]
+         : s == kCol0 ? P.col_w[0] : s == kCol1 ? P.col_w[1] : s == kHead ? P.head_w : P.col_w[2];
+  }
+  static __device__ __forceinline__ const float* bias(const KParams& P, int s) {
+    return s == kBase0 ? P.base_b[0] : s == kBase1 ? P.base_b[1] : s == kSem0 ? P.sem_b[0] : s == kSem1 ? P.sem_b[1]
+         : s == kCol0 ? P.col_b[0] : s == kCol1 ? P.col_b[1] : s == kHead ? P.head_b : P.col_b[2];
+  }
+
+  // Split slot S's weights into the image exactly as rowgemm stages them (getw(n, k) = W[n][k], zero padding).
+  template <int S>
+  static __device__ __forceinline__ void split_image(const KParams& P) {
+    constexpr int NP = wg::padn(N(S)), KP = wg::pad16(K(S)), kChunks = NP * KP / 8;
+    const float* __restrict__ W = weight(P, S);
+    uint8_t* hi = smem() + img_off(S);
+    for (int i = threadIdx.x; i < kChunks; i += blockDim.x) {
+      const int n = i % NP, kc = i / NP;
+      float v[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[j] = (n < N(S) && 8 * kc + j < K(S)) ? __ldg(W + (size_t)n * K(S) + 8 * kc + j) : 0.f;
+      wg::split_store8(hi, hi + NP * KP * 2, kc * (NP * 16) + n * 16, v);
+    }
+  }
+  // Once per CTA, before the first tile: the weight image, zero accumulators and free locks.
+  static __device__ __forceinline__ void prepare(const KParams& P) {
+    split_image<kBase0>(P);
+    split_image<kBase1>(P);
+    split_image<kSem0>(P);
+    split_image<kSem1>(P);
+    split_image<kCol0>(P);
+    split_image<kCol1>(P);
+    constexpr int kAccFloats = acc_off(kSlots);
+    float* a = acc<0>();
+    for (int i = threadIdx.x; i < kAccFloats; i += blockDim.x) a[i] = 0.f;
+    if (threadIdx.x < kSlots) *lock(threadIdx.x) = 0;
+    wg::fence_proxy_async();
+    __syncthreads();
+  }
+  // Slot S's accumulator added to the global gradient (reds: G may be a buffer other GPUs add into); after a CTA barrier.
+  template <int S>
+  static __device__ __forceinline__ void flush(const KParams& G) {
+    constexpr int Kv = K(S), Nv = N(S);
+    float* gW = const_cast<float*>(weight(G, S));
+    float* gb = const_cast<float*>(bias(G, S));
+    const float* a = acc<S>();
+    constexpr int kW = tensor(Nv) ? wg::DwAcc<Kv, Nv>::kW : Nv * Kv;
+    for (int e = threadIdx.x; e < kW; e += blockDim.x) {
+      int n = e / Kv, k = e % Kv;
+      if constexpr (tensor(Nv)) wg::DwAcc<Kv, Nv>::at(e, n, k);
+      const float v = a[e];
+      if (n < Nv && k < Kv && v != 0.f) atomicAdd(gW + (size_t)n * Kv + k, v);
+    }
+    for (int n = threadIdx.x; n < Nv; n += blockDim.x)
+      if (a[kW + n] != 0.f) atomicAdd(gb + n, a[kW + n]);
+  }
+  static __device__ __forceinline__ void flush_all(const KParams& G) {
+    flush<kBase0>(G);
+    flush<kBase1>(G);
+    flush<kSem0>(G);
+    flush<kSem1>(G);
+    flush<kCol0>(G);
+    flush<kCol1>(G);
+    flush<kHead>(G);
+    flush<kCol2>(G);
+  }
+
+  template <int SLOT, int Kv, int Nv, bool RELU>
+  static __device__ __forceinline__ void fwd(const float* __restrict__ W, const float* __restrict__ b, const float (&x)[Kv], float (&y)[Nv]) {
+    static_assert(K(SLOT) == Kv && N(SLOT) == Nv, "slot shape");
+    if constexpr (tensor(Nv)) {
+      wg::resident_rowgemm<wg::padn(Nv), wg::pad16(Kv), false>(step(), smem() + img_off(SLOT), x, y);
+#pragma unroll
+      for (int n = 0; n < Nv; ++n) {  // as wg::linear
+        const float v = y[n] + __ldg(b + n);
+        y[n] = RELU ? fmaxf(v, 0.f) : v;
+      }
+    } else {
+      linear_fwd<Kv, Nv, RELU>(W, b, x, y);
+    }
+  }
+  template <int SLOT, int Kv, int Nv>
+  static __device__ __forceinline__ void dx(const float* __restrict__ W, const float (&dy)[Nv], float (&dxv)[Kv]) {
+    static_assert(K(SLOT) == Kv && N(SLOT) == Nv, "slot shape");
+    if constexpr (tensor(Nv))
+      wg::resident_rowgemm<wg::padn(Nv), wg::pad16(Kv), true>(step(), smem() + img_off(SLOT), dy, dxv);
+    else
+      linear_bwd_input<Kv, Nv>(W, dy, dxv);
+    FNR_PHASE(kPhDx);
+  }
+  template <int SLOT, int Kv, int Nv>
+  static __device__ __forceinline__ void dw(float*, float*, const float (&x)[Kv], const float (&dy)[Nv], float*, float*) {
+    static_assert(K(SLOT) == Kv && N(SLOT) == Nv, "slot shape");
+    if constexpr (tensor(Nv))
+      wg::weight_grad_acc<Kv, Nv>(step(), part(), x, dy, acc<SLOT>(), lock(SLOT));
+    else
+      wg::head_weight_grad_acc<Kv, Nv>(part(), x, dy, acc<SLOT>(), lock(SLOT));
     FNR_PHASE(kPhDw);
   }
 };
@@ -202,58 +364,58 @@ struct Acts {
 // The field's branch forwards.  field_mlps and the backward's recompute both run these, so the recompute gives the
 // forward's pre-activations bit for bit and its ReLU masks agree with the forward that ran.
 //
+// Lin: how the layers are evaluated (Layers<C, TC> or ResidentLayers).
+//
 // base MLP: enc -> [h0, geo...]; geo = out[1:]
-template <class C, bool TC>
+template <class C, class Lin>
 __device__ __forceinline__ void base_fwd(const KParams& P, const float (&enc)[C::ENC], float (&h1)[C::BASE_H],
                                          float (&out)[C::BASE_OUT], float (&geo)[C::GEO]) {
-  using Lin = Layers<C, TC>;
-  Lin::template fwd<C::ENC, C::BASE_H, true>(P.base_w[0], P.base_b[0], enc, h1);
-  Lin::template fwd<C::BASE_H, C::BASE_OUT, false>(P.base_w[1], P.base_b[1], h1, out);
+  Lin::template fwd<kBase0, C::ENC, C::BASE_H, true>(P.base_w[0], P.base_b[0], enc, h1);
+  Lin::template fwd<kBase1, C::BASE_H, C::BASE_OUT, false>(P.base_w[1], P.base_b[1], h1, out);
 #pragma unroll
   for (int i = 0; i < C::GEO; ++i) geo[i] = out[1 + i];
 }
 
 // semantic branch up to the logit head: mlp_semantics(detach(geo)) (fruit_field.py:263-268)
-template <class C, bool TC>
+template <class C, class Lin>
 __device__ __forceinline__ void semantic_fwd(const KParams& P, const float (&geo)[C::GEO], float (&z1)[C::SEM_H],
                                              float (&z2)[C::SEM_LAYERS == 3 ? C::SEM_H : 1], float (&zo)[C::SEM_OUT]) {
-  using Lin = Layers<C, TC>;
-  Lin::template fwd<C::GEO, C::SEM_H, true>(P.sem_w[0], P.sem_b[0], geo, z1);
+  Lin::template fwd<kSem0, C::GEO, C::SEM_H, true>(P.sem_w[0], P.sem_b[0], geo, z1);
   if constexpr (C::SEM_LAYERS == 3) {
-    Lin::template fwd<C::SEM_H, C::SEM_H, true>(P.sem_w[1], P.sem_b[1], z1, z2);
-    Lin::template fwd<C::SEM_H, C::SEM_OUT, false>(P.sem_w[2], P.sem_b[2], z2, zo);
+    Lin::template fwd<kSem1, C::SEM_H, C::SEM_H, true>(P.sem_w[1], P.sem_b[1], z1, z2);
+    Lin::template fwd<kSem2, C::SEM_H, C::SEM_OUT, false>(P.sem_w[2], P.sem_b[2], z2, zo);
   } else {
-    Lin::template fwd<C::SEM_H, C::SEM_OUT, false>(P.sem_w[1], P.sem_b[1], z1, zo);
+    Lin::template fwd<kSem1, C::SEM_H, C::SEM_OUT, false>(P.sem_w[1], P.sem_b[1], z1, zo);
   }
 }
 
 // colour branch up to the sigmoid: cat[SH(dir), geo, appearance] -> MLP (fruit_field.py:270-278)
-template <class C, bool TC>
+template <class C, class Lin>
 __device__ __forceinline__ void colour_fwd(const KParams& P, const float* __restrict__ dir, const float (&geo)[C::GEO],
                                            const float (&app)[C::APP], float (&cin)[C::COL_IN], float (&c1)[C::COL_H],
                                            float (&c2)[C::COL_H], float (&o3)[3]) {
-  using Lin = Layers<C, TC>;
   sh_degree4(dir[0], dir[1], dir[2], cin);
 #pragma unroll
   for (int i = 0; i < C::GEO; ++i) cin[C::SH + i] = geo[i];
 #pragma unroll
   for (int i = 0; i < C::APP; ++i) cin[C::SH + C::GEO + i] = app[i];
-  Lin::template fwd<C::COL_IN, C::COL_H, true>(P.col_w[0], P.col_b[0], cin, c1);
-  Lin::template fwd<C::COL_H, C::COL_H, true>(P.col_w[1], P.col_b[1], c1, c2);
-  Lin::template fwd<C::COL_H, 3, false>(P.col_w[2], P.col_b[2], c2, o3);
+  Lin::template fwd<kCol0, C::COL_IN, C::COL_H, true>(P.col_w[0], P.col_b[0], cin, c1);
+  Lin::template fwd<kCol1, C::COL_H, C::COL_H, true>(P.col_w[1], P.col_b[1], c1, c2);
+  Lin::template fwd<kCol2, C::COL_H, 3, false>(P.col_w[2], P.col_b[2], c2, o3);
 }
 
 template <class C, bool TC>
 __device__ __forceinline__ void field_mlps(const KParams& P, const float (&enc)[C::ENC], const float* __restrict__ dir,
                                            const float (&app)[C::APP], Acts<C>& a) {
+  using Lin = Layers<C, TC>;
   float geo[C::GEO];
-  base_fwd<C, TC>(P, enc, a.h1, a.out, geo);
-  semantic_fwd<C, TC>(P, geo, a.z1, a.z2, a.zo);
+  base_fwd<C, Lin>(P, enc, a.h1, a.out, geo);
+  semantic_fwd<C, Lin>(P, geo, a.z1, a.z2, a.zo);
   float lg[1];
-  Layers<C, TC>::template fwd<C::SEM_OUT, 1, false>(P.head_w, P.head_b, a.zo, lg);
+  Lin::template fwd<kHead, C::SEM_OUT, 1, false>(P.head_w, P.head_b, a.zo, lg);
   a.logit = lg[0];
   float o3[3];
-  colour_fwd<C, TC>(P, dir, geo, app, a.cin, a.c1, a.c2, o3);
+  colour_fwd<C, Lin>(P, dir, geo, app, a.cin, a.c1, a.c2, o3);
 #pragma unroll
   for (int i = 0; i < 3; ++i) a.rgb[i] = sigmoidf_(o3[i]);
 }
@@ -489,9 +651,11 @@ __global__ void __launch_bounds__(kThreads) simt_composite_backward_kernel(KRays
 }
 
 // ------------------------------------------------------------------------------------------
-// K4: per-point field backward.  Weight gradients: the CTA's 128 points form one tile; for every
-// layer the tile's inputs X[128,K] and output grads dY[128,N] go to shared memory and each thread
-// reduces a 4x4 block of dW = dY^T X over the tile, then adds it to the global gradient.
+// K4: per-point field backward.  Weight gradients: a warpgroup's 128 points form one tile; for every
+// layer the tile's inputs X[128,K] and output grads dY[128,N] go to shared memory.  simt: each thread
+// reduces a 4x4 block of dW = dY^T X over the tile, then adds it to the global gradient.  Tensor cores:
+// the tile's dW is one MMA, added to the global gradient per tile (Layers<C, true>) or to accumulators in
+// shared memory that the CTA flushes once (ResidentLayers, small family).
 // ------------------------------------------------------------------------------------------
 template <int K, int N>
 __device__ __forceinline__ void tile_weight_grad(float* __restrict__ sX, float* __restrict__ sY, const float (&x)[K],
@@ -543,24 +707,34 @@ __device__ unsigned long long g_bwd_phase_cycles[kBwdPhases];
 #endif
 
 template <class C, bool TC>
-__global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F, KParams P, KParams G, KRays Rr,
-                                                                      KFieldBwd B) {
-  using Lin = Layers<C, TC>;
+constexpr bool resident_backward() { return TC && std::is_same<C, CfgSmall>::value; }
+template <class C, bool TC>
+constexpr int backward_threads() { return resident_backward<C, TC>() ? ResidentLayers::kGroups * kThreads : kThreads; }
+
+template <class C, bool TC>
+__global__ void __launch_bounds__(backward_threads<C, TC>()) simt_field_backward_kernel(KField F, KParams P, KParams G, KRays Rr,
+                                                                                       KFieldBwd B) {
+  constexpr bool kResident = resident_backward<C, TC>();
+  constexpr int kGroups = backward_threads<C, TC>() / kThreads;  // warpgroups (tiles in flight) per CTA
+  using Lin = std::conditional_t<kResident, ResidentLayers, Layers<C, TC>>;
   extern __shared__ __align__(16) float smem[];
   constexpr int TP = ((C::MAXW + 3) & ~3) + 4;
   float* sX = smem;
   float* sY = smem + kThreads * TP;
   __shared__ float s_app[C::APP];
   block_mean_embedding(P, F.num_images, C::APP, F.appearance_mode, s_app);
+  if constexpr (kResident) ResidentLayers::prepare(P);
 #ifdef FNR_BWD_PHASE_TIMERS
-  if (threadIdx.x < kBwdPhases) phase::cycles[threadIdx.x] = 0;
-  if (threadIdx.x == 0) phase::last = clock64();
+  if (threadIdx.x < 2 * kBwdPhases) phase::cycles[threadIdx.x / kBwdPhases][threadIdx.x % kBwdPhases] = 0;
+  if (wg::tid() == 0) phase::last[wg::group()] = clock64();
+  __syncthreads();
 #endif
   const long long N = (long long)Rr.R * Rr.S;
   const long long tiles = (N + kThreads - 1) / kThreads;
   const int lane = threadIdx.x & 31;
-  for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-    const long long p = tile * kThreads + threadIdx.x;
+  // warpgroup g of CTA b takes tiles b * kGroups + g, strided over all warpgroups of the grid
+  for (long long tile = (long long)blockIdx.x * kGroups + wg::group(); tile < tiles; tile += (long long)gridDim.x * kGroups) {
+    const long long p = tile * kThreads + wg::tid();
     const bool valid = p < N;
     const long long pc = valid ? p : N - 1;
     const int r = (int)(pc / Rr.S);
@@ -596,7 +770,7 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
     // The forward is recomputed branch by branch with field_mlps' branch functions, and each branch is back-propagated
     // right after its forward: only the base MLP's activations live across the whole tile.
     float h1[C::BASE_H], out[C::BASE_OUT], geo[C::GEO];
-    base_fwd<C, TC>(P, enc, h1, out, geo);
+    base_fwd<C, Lin>(P, enc, h1, out, geo);
     FNR_PHASE(kPhRecompute);
 
     float d_geo[C::GEO];
@@ -607,31 +781,31 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
     {
       float z1[C::SEM_H], zo[C::SEM_OUT];
       float z2[C::SEM_LAYERS == 3 ? C::SEM_H : 1];
-      semantic_fwd<C, TC>(P, geo, z1, z2, zo);
+      semantic_fwd<C, Lin>(P, geo, z1, z2, zo);
       FNR_PHASE(kPhRecompute);
       float dlg[1] = {d_logit};
       float dzo[C::SEM_OUT];
-      Lin::template dx<C::SEM_OUT, 1>(P.head_w, dlg, dzo);
-      Lin::template dw<C::SEM_OUT, 1>(sX, sY, zo, dlg, G.head_w, G.head_b);
+      Lin::template dx<kHead, C::SEM_OUT, 1>(P.head_w, dlg, dzo);
+      Lin::template dw<kHead, C::SEM_OUT, 1>(sX, sY, zo, dlg, G.head_w, G.head_b);
       float dz1[C::SEM_H];
       if constexpr (C::SEM_LAYERS == 3) {
         float dz2[C::SEM_H];
-        Lin::template dx<C::SEM_H, C::SEM_OUT>(P.sem_w[2], dzo, dz2);
-        Lin::template dw<C::SEM_H, C::SEM_OUT>(sX, sY, z2, dzo, G.sem_w[2], G.sem_b[2]);
+        Lin::template dx<kSem2, C::SEM_H, C::SEM_OUT>(P.sem_w[2], dzo, dz2);
+        Lin::template dw<kSem2, C::SEM_H, C::SEM_OUT>(sX, sY, z2, dzo, G.sem_w[2], G.sem_b[2]);
 #pragma unroll
         for (int i = 0; i < C::SEM_H; ++i) dz2[i] = z2[i] > 0.f ? dz2[i] : 0.f;
-        Lin::template dx<C::SEM_H, C::SEM_H>(P.sem_w[1], dz2, dz1);
-        Lin::template dw<C::SEM_H, C::SEM_H>(sX, sY, z1, dz2, G.sem_w[1], G.sem_b[1]);
+        Lin::template dx<kSem1, C::SEM_H, C::SEM_H>(P.sem_w[1], dz2, dz1);
+        Lin::template dw<kSem1, C::SEM_H, C::SEM_H>(sX, sY, z1, dz2, G.sem_w[1], G.sem_b[1]);
       } else {
-        Lin::template dx<C::SEM_H, C::SEM_OUT>(P.sem_w[1], dzo, dz1);
-        Lin::template dw<C::SEM_H, C::SEM_OUT>(sX, sY, z1, dzo, G.sem_w[1], G.sem_b[1]);
+        Lin::template dx<kSem1, C::SEM_H, C::SEM_OUT>(P.sem_w[1], dzo, dz1);
+        Lin::template dw<kSem1, C::SEM_H, C::SEM_OUT>(sX, sY, z1, dzo, G.sem_w[1], G.sem_b[1]);
       }
 #pragma unroll
       for (int i = 0; i < C::SEM_H; ++i) dz1[i] = z1[i] > 0.f ? dz1[i] : 0.f;
-      Lin::template dw<C::GEO, C::SEM_H>(sX, sY, geo, dz1, G.sem_w[0], G.sem_b[0]);
+      Lin::template dw<kSem0, C::GEO, C::SEM_H>(sX, sY, geo, dz1, G.sem_w[0], G.sem_b[0]);
       if (F.pass_semantic_gradients) {
         float dg[C::GEO];
-        Lin::template dx<C::GEO, C::SEM_H>(P.sem_w[0], dz1, dg);
+        Lin::template dx<kSem0, C::GEO, C::SEM_H>(P.sem_w[0], dz1, dg);
 #pragma unroll
         for (int i = 0; i < C::GEO; ++i) d_geo[i] += dg[i];
       }
@@ -639,7 +813,7 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
     // ---- colour branch ---------------------------------------------------------------------
     {
       float cin[C::COL_IN], c1[C::COL_H], c2[C::COL_H], o3[3];
-      colour_fwd<C, TC>(P, d, geo, appv, cin, c1, c2, o3);
+      colour_fwd<C, Lin>(P, d, geo, appv, cin, c1, c2, o3);
       FNR_PHASE(kPhRecompute);
       float do3[3];
 #pragma unroll
@@ -648,16 +822,16 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
         do3[i] = d_rgb[i] * rgb * (1.0f - rgb);
       }
       float dc2[C::COL_H], dc1[C::COL_H], dcin[C::COL_IN];
-      Lin::template dx<C::COL_H, 3>(P.col_w[2], do3, dc2);
-      Lin::template dw<C::COL_H, 3>(sX, sY, c2, do3, G.col_w[2], G.col_b[2]);
+      Lin::template dx<kCol2, C::COL_H, 3>(P.col_w[2], do3, dc2);
+      Lin::template dw<kCol2, C::COL_H, 3>(sX, sY, c2, do3, G.col_w[2], G.col_b[2]);
 #pragma unroll
       for (int i = 0; i < C::COL_H; ++i) dc2[i] = c2[i] > 0.f ? dc2[i] : 0.f;
-      Lin::template dx<C::COL_H, C::COL_H>(P.col_w[1], dc2, dc1);
-      Lin::template dw<C::COL_H, C::COL_H>(sX, sY, c1, dc2, G.col_w[1], G.col_b[1]);
+      Lin::template dx<kCol1, C::COL_H, C::COL_H>(P.col_w[1], dc2, dc1);
+      Lin::template dw<kCol1, C::COL_H, C::COL_H>(sX, sY, c1, dc2, G.col_w[1], G.col_b[1]);
 #pragma unroll
       for (int i = 0; i < C::COL_H; ++i) dc1[i] = c1[i] > 0.f ? dc1[i] : 0.f;
-      Lin::template dx<C::COL_IN, C::COL_H>(P.col_w[0], dc1, dcin);
-      Lin::template dw<C::COL_IN, C::COL_H>(sX, sY, cin, dc1, G.col_w[0], G.col_b[0]);
+      Lin::template dx<kCol0, C::COL_IN, C::COL_H>(P.col_w[0], dc1, dcin);
+      Lin::template dw<kCol0, C::COL_IN, C::COL_H>(sX, sY, cin, dc1, G.col_w[0], G.col_b[0]);
 #pragma unroll
       for (int i = 0; i < C::GEO; ++i) d_geo[i] += dcin[C::SH + i];
       // appearance-embedding gradient (only the per-camera rows are parameters of the graph;
@@ -693,12 +867,12 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
 #pragma unroll
       for (int i = 0; i < C::GEO; ++i) dout[1 + i] = d_geo[i];
       float dh1[C::BASE_H];
-      Lin::template dx<C::BASE_H, C::BASE_OUT>(P.base_w[1], dout, dh1);
-      Lin::template dw<C::BASE_H, C::BASE_OUT>(sX, sY, h1, dout, G.base_w[1], G.base_b[1]);
+      Lin::template dx<kBase1, C::BASE_H, C::BASE_OUT>(P.base_w[1], dout, dh1);
+      Lin::template dw<kBase1, C::BASE_H, C::BASE_OUT>(sX, sY, h1, dout, G.base_w[1], G.base_b[1]);
 #pragma unroll
       for (int i = 0; i < C::BASE_H; ++i) dh1[i] = h1[i] > 0.f ? dh1[i] : 0.f;
-      Lin::template dx<C::ENC, C::BASE_H>(P.base_w[0], dh1, denc);
-      Lin::template dw<C::ENC, C::BASE_H>(sX, sY, enc, dh1, G.base_w[0], G.base_b[0]);
+      Lin::template dx<kBase0, C::ENC, C::BASE_H>(P.base_w[0], dh1, denc);
+      Lin::template dw<kBase0, C::ENC, C::BASE_H>(sX, sY, enc, dh1, G.base_w[0], G.base_b[0]);
     }
     // ---- hash-table scatter -----------------------------------------------------------------
     if (valid) {
@@ -712,9 +886,21 @@ __global__ void __launch_bounds__(kThreads) simt_field_backward_kernel(KField F,
     }
     FNR_PHASE(kPhScatter);
   }
+  if constexpr (kResident) {
+    // every warpgroup, with tiles or without, ends here: one flush of the CTA's weight gradients
+    __syncthreads();
+#ifdef FNR_BWD_PHASE_TIMERS
+    const long long f0 = clock64();
+#endif
+    ResidentLayers::flush_all(G);
+#ifdef FNR_BWD_PHASE_TIMERS
+    __syncthreads();
+    if (threadIdx.x == 0) phase::cycles[0][kPhDwFlush] += (unsigned long long)(clock64() - f0);
+#endif
+  }
 #ifdef FNR_BWD_PHASE_TIMERS
   __syncthreads();  // thread 0's update of the last phase is visible to the threads that flush the counters
-  if (threadIdx.x < kBwdPhases) atomicAdd(g_bwd_phase_cycles + threadIdx.x, phase::cycles[threadIdx.x]);
+  if (threadIdx.x < kBwdPhases) atomicAdd(g_bwd_phase_cycles + threadIdx.x, phase::cycles[0][threadIdx.x] + phase::cycles[1][threadIdx.x]);
 #endif
 }
 
@@ -909,6 +1095,17 @@ int launch_field_backward(Family fam, bool tc, const KField& F, const KParams& P
   return with_layers(fam, tc, [&](auto c, auto t) {
     using C = decltype(c);
     constexpr bool TC = decltype(t)::value;
+    if constexpr (resident_backward<C, TC>()) {
+      // one CTA of two warpgroups per SM (its shared memory is most of the SM's), as many warpgroups as there are tiles
+      const long long N = (long long)Rr.R * Rr.S;
+      if (N == 0) return FNR_OK;
+      auto kernel = simt_field_backward_kernel<C, TC>;
+      constexpr int threads = backward_threads<C, TC>();
+      cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ResidentLayers::kBytes);
+      if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute");
+      kernel<<<grid_for(N, threads, sm_count()), threads, ResidentLayers::kBytes, st>>>(F, P, G, Rr, B);
+      return check_launch("simt_field_backward_kernel<wgmma>");
+    }
     return launch_field_kernel(simt_field_backward_kernel<C, TC>, Layers<C, TC>::kBwdSmemBytes, (long long)Rr.R * Rr.S,
                                TC ? "simt_field_backward_kernel<wgmma>" : "simt_field_backward_kernel", st, F, P, G, Rr, B);
   });

@@ -1,36 +1,47 @@
 // Hopper (sm_90a) warpgroup MMA layer: the MLP layers of the tensor-core field forward and backward (fnr_simt.cu,
-// Layers<C, true>): y = W x + b, dx = W^T dy and dW = dY^T X of a 128-point tile.
+// Layers<C, true> and ResidentLayers): y = W x + b, dx = W^T dy and dW = dY^T X of a 128-point tile.
 //
-// One CTA of 128 threads = one warpgroup = one tile of 128 sample points, thread t owning point t.  A layer
-// y = W x + b is one block-wide step: every thread writes its row x[K] into shared memory as a bf16 hi/lo split
+// One warpgroup (128 threads) = one tile of 128 sample points, thread t of the warpgroup owning point t.  A layer
+// y = W x + b is one warpgroup-wide step: every thread writes its row x[K] into shared memory as a bf16 hi/lo split
 // (x ~= hi + lo, 16 mantissa bits), the weights W[N][K] are split the same way, and the warpgroup runs
 // D[128, N] = Xhi Whi^T + Xlo Whi^T + Xhi Wlo^T + Xlo Wlo^T with fp32 accumulation (wgmma m64nNk16, two M halves);
 // the accumulator fragments go back to shared memory in fp32 and every thread reads its row.  Relative error of a
-// product ~2^-17 (the rounding of the lo halves), fp32-class for the parity bar of the tests.
+// product ~2^-17 (the rounding of the lo halves), fp32-class for the parity bar of the tests.  The forward and export
+// kernels (one warpgroup per CTA) stage the weight tile from global memory at every step; the small family's backward
+// (two warpgroups per CTA) splits its weights once per CTA into a resident image and accumulates dW / db in shared memory.
 //
-// Operand layout (no swizzle, K-major core matrices of 8 rows x 16 bytes): element (row, k) of a ROWS x KP tile is at
+// Operand layout (no swizzle, core matrices of 8 rows x 16 bytes).  K-major: element (row, k) of a ROWS x KP tile is at
 //     (k / 8) * (ROWS * 16) + row * 16 + (k % 8) * 2
-// so the descriptor's leading byte offset (between the two K core matrices of one k16 step) is ROWS * 16 and its
-// stride byte offset (between 8-row groups) is 128.
+// MN-major (read with the wgmma transpose bit): element (row, k) is at (row / 8) * MN_STRIDE + k * 16 + (row % 8) * 2.
+// In both, a descriptor's leading byte offset is the stride between core matrices along K and its stride byte offset
+// the stride between core matrices along M / N (K-major: ROWS * 16 and 128; MN-major: 128 and MN_STRIDE).
 #pragma once
 #include <cuda_bf16.h>
 #include <stdint.h>
 
-// Diagnostic build of the backward (-DFNR_BWD_PHASE_TIMERS, tools/bench_backward.py --phases; never set by the normal
-// build): FNR_PHASE(i) closes phase i of the current tile.  Every thread of the CTA calls it; after a barrier, thread 0
-// adds the clock64() cycles since the previous mark to the CTA's counter of phase i.
 namespace fnr {
+namespace wg {
+// Index of the thread in its warpgroup, the warpgroup in the CTA, and the warpgroup's named barrier (id 1 + warpgroup;
+// id 0 is __syncthreads).  A CTA of one warpgroup sees threadIdx.x and a barrier over the whole CTA.
+__device__ __forceinline__ int tid() { return threadIdx.x & 127; }
+__device__ __forceinline__ int group() { return threadIdx.x >> 7; }
+__device__ __forceinline__ void sync() { asm volatile("bar.sync %0, 128;" ::"r"(1 + group()) : "memory"); }
+}  // namespace wg
+
+// Diagnostic build of the backward (-DFNR_BWD_PHASE_TIMERS, tools/bench_backward.py --phases; never set by the normal
+// build): FNR_PHASE(i) closes phase i of the current tile.  Every thread of the warpgroup calls it; after the warpgroup's
+// barrier, its thread 0 adds the clock64() cycles since the previous mark to the warpgroup's counter of phase i.
 enum BwdPhase { kPhLoad, kPhRecompute, kPhDx, kPhDw, kPhDwFlush, kPhScatter, kBwdPhases };
 #ifdef FNR_BWD_PHASE_TIMERS
 namespace phase {
-__shared__ unsigned long long cycles[kBwdPhases];
-__shared__ long long last;
+__shared__ unsigned long long cycles[2][kBwdPhases];
+__shared__ long long last[2];
 __device__ __forceinline__ void mark(int i) {
-  __syncthreads();
-  if (threadIdx.x == 0) {
+  wg::sync();
+  if (wg::tid() == 0) {
     const long long now = clock64();
-    cycles[i] += (unsigned long long)(now - last);
-    last = now;
+    cycles[wg::group()][i] += (unsigned long long)(now - last[wg::group()]);
+    last[wg::group()] = now;
   }
 }
 }  // namespace phase
@@ -56,40 +67,36 @@ __device__ __forceinline__ void wait_all() { asm volatile("wgmma.wait_group.sync
 // generic-proxy shared-memory stores -> visible to the async proxy that wgmma reads operands through
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// D[64, N] (+)= A[64, 16] B[N, 16]^T, bf16 operands from shared memory, fp32 accumulators in registers.
-template <int N>
-__device__ __forceinline__ void mma_m64k16(float (&d)[N / 2], uint64_t a, uint64_t b, int scale_d);
-template <>
-__device__ __forceinline__ void mma_m64k16<16>(float (&d)[8], uint64_t a, uint64_t b, int scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-      : "l"(a), "l"(b), "r"(scale_d));
-}
-template <>
-__device__ __forceinline__ void mma_m64k16<32>(float (&d)[16], uint64_t a, uint64_t b, int scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(a), "l"(b), "r"(scale_d));
-}
-template <>
-__device__ __forceinline__ void mma_m64k16<64>(float (&d)[32], uint64_t a, uint64_t b, int scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(a), "l"(b), "r"(scale_d));
-}
-template <>
-__device__ __forceinline__ void mma_m64k16<128>(float (&d)[64], uint64_t a, uint64_t b, int scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(a), "l"(b), "r"(scale_d));
+// D[64, N] (+)= A[64, 16] B[N, 16]^T, bf16 operands from shared memory, fp32 accumulators in registers.  TA / TB: the
+// operand is MN-major (the transpose bit).
+template <int N, int TA = 0, int TB = 0>
+__device__ __forceinline__ void mma_m64k16(float (&d)[N / 2], uint64_t a, uint64_t b, int scale_d) {
+  if constexpr (N == 16) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
+  } else if constexpr (N == 32) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
+  } else if constexpr (N == 64) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
+  } else {
+    static_assert(N == 128, "wgmma tile width");
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
+  }
 }
 
 __device__ __forceinline__ void split_store(uint8_t* hi, uint8_t* lo, int off, float x) {
@@ -113,10 +120,19 @@ __device__ __forceinline__ void split_store8(uint8_t* hi, uint8_t* lo, int off, 
   *reinterpret_cast<uint4*>(lo + off) = make_uint4(l[0], l[1], l[2], l[3]);
 }
 
+// hi / lo split of values [8 c, 8 c + 8) of a register vector (zero past R) into one core-matrix row.
+template <int R>
+__device__ __forceinline__ void split_store_chunk(uint8_t* hi, uint8_t* lo, int off, const float (&x)[R], int c) {
+  float v[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) v[j] = 8 * c + j < R ? x[8 * c + j < R ? 8 * c + j : 0] : 0.f;
+  split_store8(hi, lo, off, v);
+}
+
 constexpr int pad16(int k) { return (k + 15) / 16 * 16; }
 constexpr int padn(int n) { return n <= 16 ? 16 : n <= 32 ? 32 : n <= 64 ? 64 : 128; }
 
-// Shared memory of one layer step: X tile (hi | lo), W tile (hi | lo), fp32 result rows.
+// Shared memory of one staged layer step: X tile (hi | lo), W tile (hi | lo), fp32 result rows.
 template <int KMAX, int NMAX>
 struct Smem {
   static constexpr int kX = 2 * 128 * pad16(KMAX) * 2;
@@ -125,8 +141,74 @@ struct Smem {
   static constexpr int kBytes = kX + kW + 128 * kYStride * 4;
 };
 
+// Shared memory of one resident layer step (ResidentLayers): the X tile, with the fp32 result rows stored over it as
+// they are produced.  Result element (row, c) is at float (c / 4) * 512 + row * 4 + c % 4: column group c / 4 takes the
+// 2 KiB of one 8-k chunk of the tile (hi or lo), and M half h writes rows [64 h, 64 h + 64), the 1 KiB of each chunk
+// that its MMAs have just consumed.  The fragment stores and the row reads are free of bank conflicts.
+constexpr int kResidentStepBytes = 2 * 128 * 64 * 2;
+constexpr int kRowsGroupStride = 512;
+
+// B operand of a layer step: W [NP outputs] x [KP reduction], hi at `hi`, lo `lo` bytes further; lbo / sbo as in the
+// descriptor, `kstep` bytes between k16 steps.
+struct BOperand {
+  uint32_t hi, lo, lbo, sbo, kstep;
+};
+
+// The MMA sequence of a layer step and its write-back: D[128, NP] = X W^T over the X tile at `ax` (K-major, lo `xlo`
+// bytes further) as hi.hi, lo.hi, hi.lo, lo.lo per k16 step, M half by M half, each half's fragments stored as fp32 at
+// ys + row * row_stride + (c / 4) * group_stride + c % 4.  ALIAS: ys lies over the X tile, so the warpgroup waits for
+// all of a half's MMAs before any of its rows is stored.  Every thread of the warpgroup must call it.
+template <int KP, int NP, int TB, bool ALIAS>
+__device__ __forceinline__ void layer_mma(uint32_t ax, uint32_t xlo, const BOperand& w, float* ys, int row_stride, int group_stride) {
+  const int t = tid(), warp = t >> 5, lane = t & 31;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float d[NP / 2];
+#pragma unroll
+    for (int i = 0; i < NP / 2; ++i) d[i] = 0.f;
+    fence_operands();
+#pragma unroll
+    for (int ks = 0; ks < KP / 16; ++ks) {
+      const uint32_t xa = ax + ks * 2 * (128 * 16) + h * 64 * 16, wa = w.hi + ks * w.kstep;
+      const uint64_t dxh = desc(xa, 128 * 16, 128), dxl = desc(xa + xlo, 128 * 16, 128);
+      const uint64_t dwh = desc(wa, w.lbo, w.sbo), dwl = desc(wa + w.lo, w.lbo, w.sbo);
+      mma_m64k16<NP, 0, TB>(d, dxh, dwh, ks > 0);
+      mma_m64k16<NP, 0, TB>(d, dxl, dwh, 1);
+      mma_m64k16<NP, 0, TB>(d, dxh, dwl, 1);
+      mma_m64k16<NP, 0, TB>(d, dxl, dwl, 1);
+    }
+    commit();
+    wait_all();
+    if (ALIAS) sync();
+    // fragment (i, j): row 16 * warp + lane / 4 (+8 for j >= 2), column 8 * i + 2 * (lane % 4) + (j & 1)
+    const int r0 = h * 64 + 16 * warp + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+    for (int i = 0; i < NP / 8; ++i) {
+      float* y = ys + (2 * i + (c0 >> 2)) * group_stride + (c0 & 3);
+      *reinterpret_cast<float2*>(y + r0 * row_stride) = make_float2(d[4 * i], d[4 * i + 1]);
+      *reinterpret_cast<float2*>(y + (r0 + 8) * row_stride) = make_float2(d[4 * i + 2], d[4 * i + 3]);
+    }
+  }
+}
+
+// This thread's result row of layer_mma (16-byte aligned groups of 4), after a warpgroup barrier.
+template <int NO>
+__device__ __forceinline__ void read_row(const float* ys, int row_stride, int group_stride, float (&y)[NO]) {
+  const float* r = ys + tid() * row_stride;
+#pragma unroll
+  for (int n = 0; n < NO / 4 * 4; n += 4) {
+    const float4 v = *reinterpret_cast<const float4*>(r + (n / 4) * group_stride);
+    y[n] = v.x;
+    y[n + 1] = v.y;
+    y[n + 2] = v.z;
+    y[n + 3] = v.w;
+  }
+#pragma unroll
+  for (int n = NO / 4 * 4; n < NO; ++n) y[n] = r[(n / 4) * group_stride + n % 4];
+}
+
 // Per-thread-row GEMM y[NO] = sum_r x[r] * getw(no, r) for the point of this thread (getw: fp32 weight of output no,
-// reduction index r); every thread of the CTA (one warpgroup) must call it.
+// reduction index r), with the weight tile staged from getw; every thread of the CTA (one warpgroup) must call it.
 template <int KMAX, int NMAX, int R, int NO, class GetW>
 __device__ __forceinline__ void rowgemm(uint8_t* smem, const float (&x)[R], float (&y)[NO], GetW getw) {
   constexpr int KP = pad16(R), NP = padn(NO);
@@ -137,15 +219,10 @@ __device__ __forceinline__ void rowgemm(uint8_t* smem, const float (&x)[R], floa
   uint8_t* whi = smem + S::kX;
   uint8_t* wlo = whi + NP * KP * 2;
   float* ys = reinterpret_cast<float*>(smem + S::kX + S::kW);
-  const int t = threadIdx.x;
+  const int t = tid();
   __syncthreads();  // the previous step's readers are done with every buffer
 #pragma unroll
-  for (int kc = 0; kc < KP / 8; ++kc) {
-    float v[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) v[j] = 8 * kc + j < R ? x[8 * kc + j < R ? 8 * kc + j : 0] : 0.f;
-    split_store8(xhi, xlo, kc * (128 * 16) + t * 16, v);
-  }
+  for (int kc = 0; kc < KP / 8; ++kc) split_store_chunk(xhi, xlo, kc * (128 * 16) + t * 16, x, kc);
   // weight tile in (row, 8-k chunk) units, consecutive threads on consecutive rows of one chunk column
   constexpr int kChunks = NP * KP / 8;
 #pragma unroll 1
@@ -160,47 +237,34 @@ __device__ __forceinline__ void rowgemm(uint8_t* smem, const float (&x)[R], floa
   }
   fence_proxy_async();
   __syncthreads();
-  const uint32_t ax = smem_u32(xhi), aw = smem_u32(whi);
-  constexpr uint32_t XLO = 128 * KP * 2, WLO = NP * KP * 2;
-  const int warp = t >> 5, lane = t & 31;
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    float d[NP / 2];
-#pragma unroll
-    for (int i = 0; i < NP / 2; ++i) d[i] = 0.f;
-    fence_operands();
-#pragma unroll
-    for (int ks = 0; ks < KP / 16; ++ks) {
-      const uint32_t xa = ax + ks * 2 * (128 * 16) + h * 64 * 16, wa = aw + ks * 2 * (NP * 16);
-      const uint64_t dxh = desc(xa, 128 * 16, 128), dxl = desc(xa + XLO, 128 * 16, 128);
-      const uint64_t dwh = desc(wa, NP * 16, 128), dwl = desc(wa + WLO, NP * 16, 128);
-      mma_m64k16<NP>(d, dxh, dwh, ks > 0);
-      mma_m64k16<NP>(d, dxl, dwh, 1);
-      mma_m64k16<NP>(d, dxh, dwl, 1);
-      mma_m64k16<NP>(d, dxl, dwl, 1);
-    }
-    commit();
-    wait_all();
-    // fragment (i, j): row 16 * warp + lane / 4 (+8 for j >= 2), column 8 * i + 2 * (lane % 4) + (j & 1)
-    const int r0 = h * 64 + 16 * warp + (lane >> 2), c0 = 2 * (lane & 3);
-#pragma unroll
-    for (int i = 0; i < NP / 8; ++i) {
-      *reinterpret_cast<float2*>(ys + r0 * S::kYStride + 8 * i + c0) = make_float2(d[4 * i], d[4 * i + 1]);
-      *reinterpret_cast<float2*>(ys + (r0 + 8) * S::kYStride + 8 * i + c0) = make_float2(d[4 * i + 2], d[4 * i + 3]);
-    }
-  }
+  const BOperand w{smem_u32(whi), (uint32_t)(NP * KP * 2), NP * 16, 128, 2 * NP * 16};
+  layer_mma<KP, NP, 0, false>(smem_u32(xhi), 128 * KP * 2, w, ys, S::kYStride, 4);
   __syncthreads();
-  // row t, 16-byte aligned (kYStride is a multiple of 4)
+  read_row<NO>(ys, S::kYStride, 4, y);
+}
+
+// The same GEMM with the weights from a resident split image (W [NPF][KPF] K-major, as rowgemm stages it).  TRANS = false:
+// y = W x (the forward); TRANS = true: y = W^T x (dx), the image read MN-major through the transpose bit.  smem is the
+// warpgroup's kResidentStepBytes.
+template <int NPF, int KPF, bool TRANS, int R, int NO>
+__device__ __forceinline__ void resident_rowgemm(uint8_t* smem, const uint8_t* img, const float (&x)[R], float (&y)[NO]) {
+  constexpr int KP = pad16(R), NP = padn(NO);
+  static_assert(TRANS ? (KP <= NPF && NP <= KPF) : (KP == KPF && NP == NPF), "layer outside the resident image");
+  static_assert(2 * 128 * KP * 2 <= kResidentStepBytes && NP * 128 * 4 <= kResidentStepBytes, "resident step plan");
+  uint8_t* xhi = smem;
+  uint8_t* xlo = smem + 128 * KP * 2;
+  float* ys = reinterpret_cast<float*>(smem);
+  const int t = tid();
+  sync();  // the previous step's readers are done with the tile
 #pragma unroll
-  for (int n = 0; n < NO / 4 * 4; n += 4) {
-    const float4 v = *reinterpret_cast<const float4*>(ys + t * S::kYStride + n);
-    y[n] = v.x;
-    y[n + 1] = v.y;
-    y[n + 2] = v.z;
-    y[n + 3] = v.w;
-  }
-#pragma unroll
-  for (int n = NO / 4 * 4; n < NO; ++n) y[n] = ys[t * S::kYStride + n];
+  for (int kc = 0; kc < KP / 8; ++kc) split_store_chunk(xhi, xlo, kc * (128 * 16) + t * 16, x, kc);
+  fence_proxy_async();
+  sync();
+  const uint32_t iw = smem_u32(img), lo = NPF * KPF * 2;
+  const BOperand w = TRANS ? BOperand{iw, lo, 128, NPF * 16, 2 * 128} : BOperand{iw, lo, NPF * 16, 128, 2 * NPF * 16};
+  layer_mma<KP, NP, TRANS ? 1 : 0, true>(smem_u32(xhi), 128 * KP * 2, w, ys, 4, kRowsGroupStride);
+  sync();
+  read_row<NO>(ys, 4, kRowsGroupStride, y);
 }
 
 // y[N] = W x + b (optionally ReLU), W in torch layout [N][K].
@@ -229,9 +293,9 @@ struct DwSmem {
   static constexpr int kBytes = kA + kB + 128 * YS * 4;
 };
 
-// Weight gradient of the CTA's 128-point tile, gW[N][K] += dY^T X and gb[N] += column sums of dY, both operands read
-// K-major over the points (the reduction dimension); accumulated in warpgroup registers and added to the global gradient once
-// per tile.  Every thread of the CTA must call it.
+// Weight gradient of the warpgroup's 128-point tile, gW[N][K] += dY^T X and gb[N] += column sums of dY, both operands
+// read K-major over the points (the reduction dimension); accumulated in warpgroup registers and added to the global
+// gradient once per tile.  Every thread of the CTA (one warpgroup) must call it.
 template <int K, int N>
 __device__ __forceinline__ void weight_grad(uint8_t* smem, const float (&x)[K], const float (&dy)[N], float* __restrict__ gW,
                                             float* __restrict__ gb) {
@@ -242,7 +306,7 @@ __device__ __forceinline__ void weight_grad(uint8_t* smem, const float (&x)[K], 
   uint8_t* bhi = smem + S::kA;
   uint8_t* blo = bhi + KP * 128 * 2;
   float* ys = reinterpret_cast<float*>(smem + S::kA + S::kB);
-  const int t = threadIdx.x;
+  const int t = tid();
   __syncthreads();
   // point t is reduction index t: element (row, t) at (t / 8) * (ROWS * 16) + row * 16 + (t % 8) * 2
   const int pt = (t >> 3) * 16, pl = (t & 7) * 2;
@@ -295,6 +359,167 @@ __device__ __forceinline__ void weight_grad(uint8_t* smem, const float (&x)[K], 
     if (sum != 0.f) atomicAdd(gb + n, sum);
   }
   FNR_PHASE(kPhDwFlush);
+}
+
+// ------------------------------------------------------------------------------------------
+// On-chip weight gradients (ResidentLayers): dW / db of every tile are added to fp32 accumulators in shared memory,
+// which the CTA adds to the global gradient once, at its end.
+// ------------------------------------------------------------------------------------------
+
+// Reduce-scatter over the warp of P values per lane (P a power of two <= 32): returns, in lane l, the sum over the 32
+// lanes of v[l >> (5 - log2 P)].  P - 1 + (5 - log2 P) shuffles; v is clobbered.
+template <int P, int S = 16>
+__device__ __forceinline__ float warp_reduce_scatter(float* v, int lane) {
+  if constexpr (S == 0) {
+    return v[0];
+  } else if constexpr (P == 1) {
+    v[0] += __shfl_xor_sync(0xffffffffu, v[0], S);
+    return warp_reduce_scatter<1, S / 2>(v, lane);
+  } else {
+    const bool up = (lane & S) != 0;
+#pragma unroll
+    for (int i = 0; i < P / 2; ++i) {
+      const float send = up ? v[i] : v[i + P / 2], keep = up ? v[i + P / 2] : v[i];
+      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, S);
+    }
+    return warp_reduce_scatter<P / 2, S / 2>(v, lane);
+  }
+}
+
+constexpr int pow2_at_least(int n) { return n <= 1 ? 1 : 2 * pow2_at_least((n + 1) / 2); }
+constexpr int log2_exact(int n) { return n <= 1 ? 0 : 1 + log2_exact(n / 2); }
+
+// out[i] = sum over the warp's 32 lanes of v(i), i < M, in fp32 (32-value reduce-scatters; no serial loops).
+template <int M, class V>
+__device__ __forceinline__ void warp_column_sums(V v, float* out, int lane) {
+#pragma unroll
+  for (int c = 0; c < M; c += 32) {
+    constexpr int kLeft = M % 32 == 0 ? 32 : M % 32;
+    constexpr int P = pow2_at_least(M >= 32 ? 32 : kLeft);
+    constexpr int SH = 5 - log2_exact(P);
+    float u[P];
+#pragma unroll
+    for (int j = 0; j < P; ++j) u[j] = c + j < M ? v(c + j < M ? c + j : 0) : 0.f;
+    const float s = warp_reduce_scatter<P>(u, lane);
+    const int i = c + (lane >> SH);
+    if ((lane & ((1 << SH) - 1)) == 0 && i < M) out[i] = s;
+  }
+}
+
+// A warpgroup's exclusive use of one accumulator: thread 0 takes the lock, the warpgroup's barrier passes it on.
+__device__ __forceinline__ void acquire(int* lock) {
+  if (tid() == 0) {
+    while (atomicCAS(lock, 0, 1) != 0) __nanosleep(32);
+    __threadfence_block();
+  }
+  sync();
+}
+__device__ __forceinline__ void release(int* lock) {
+  __threadfence_block();
+  sync();
+  if (tid() == 0) {
+    __threadfence_block();
+    atomicExch(lock, 0);
+  }
+}
+
+// Floats of per-warp partial sums a warpgroup needs (kWarpPartial per warp), and of a layer's accumulator: dW in
+// fragment order (the rows of warps that hold outputs n < N, KP / 2 floats per thread) followed by db[N].
+constexpr int kWarpPartial = 256;
+template <int K, int N>
+struct DwAcc {
+  static constexpr int KP = padn(K), kWarps = (N + 15) / 16;
+  static constexpr int kW = kWarps * 32 * (KP / 2), kFloats = kW + N;
+  // output n and input k of accumulator element e < kW
+  static __device__ __forceinline__ void at(int e, int& n, int& k) {
+    const int j = e & 3, f = e >> 2, lane = f & 31, wq = f >> 5, warp = wq / (KP / 8), q = wq % (KP / 8);
+    n = 16 * warp + (lane >> 2) + (j >= 2 ? 8 : 0);
+    k = 8 * q + 2 * (lane & 3) + (j & 1);
+  }
+};
+
+// Weight gradient of the warpgroup's 128-point tile added to the layer's accumulator acc (DwAcc<K, N>): dW = dY^T X
+// with both operands MN-major over the points (16-byte split stores of 8 outputs / inputs of one point), in two 64-point
+// halves (the operands of all 128 points would take 64 KiB).  Each half's fragments are added on their own, so that no
+// accumulator registers are live while the next half is staged (that kept the kernel's spills below the staged
+// kernel's); db from warp reduce-scatters of dY.  smem: the warpgroup's kResidentStepBytes; part: its 4 x kWarpPartial
+// floats.  Every thread of the warpgroup must call it.
+template <int K, int N>
+__device__ __forceinline__ void weight_grad_acc(uint8_t* smem, float* part, const float (&x)[K], const float (&dy)[N],
+                                                float* acc, int* lock) {
+  using A = DwAcc<K, N>;
+  constexpr int KP = A::KP, MC = (N + 7) / 8;  // MMA width; 8-output chunks of dY that are stored
+  static_assert(N <= 64 && N <= kWarpPartial, "one M tile of outputs");
+  constexpr uint32_t ALO = 64 * 64 * 2, BLO = KP * 64 * 2;
+  static_assert(2 * ALO + 2 * BLO <= kResidentStepBytes, "resident step plan");
+  uint8_t* ahi = smem;
+  uint8_t* bhi = smem + 2 * ALO;
+  const int t = tid(), warp = t >> 5, lane = t & 31;
+  warp_column_sums<N>([&](int n) { return dy[n]; }, part + warp * kWarpPartial, lane);
+#pragma unroll 1
+  for (int half = 0; half < 2; ++half) {
+    sync();  // the previous readers of the tile are done
+    if ((t >> 6) == half) {
+      // element (row, point p) at (row / 8) * 1024 + p * 16 + (row % 8) * 2; rows of dY past N are never accumulated
+      const int p = (t & 63) * 16;
+#pragma unroll
+      for (int c = 0; c < MC; ++c) split_store_chunk(ahi, ahi + ALO, c * 1024 + p, dy, c);
+#pragma unroll
+      for (int c = 0; c < KP / 8; ++c) split_store_chunk(bhi, bhi + BLO, c * 1024 + p, x, c);
+    }
+    fence_proxy_async();
+    sync();
+    const uint32_t aa = smem_u32(ahi), ab = smem_u32(bhi);
+    float d[KP / 2];
+#pragma unroll
+    for (int i = 0; i < KP / 2; ++i) d[i] = 0.f;
+    fence_operands();
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {
+      const uint64_t dah = desc(aa + ks * 256, 128, 1024), dal = desc(aa + ALO + ks * 256, 128, 1024);
+      const uint64_t dbh = desc(ab + ks * 256, 128, 1024), dbl = desc(ab + BLO + ks * 256, 128, 1024);
+      mma_m64k16<KP, 1, 1>(d, dah, dbh, ks > 0);
+      mma_m64k16<KP, 1, 1>(d, dal, dbh, 1);
+      mma_m64k16<KP, 1, 1>(d, dah, dbl, 1);
+      mma_m64k16<KP, 1, 1>(d, dal, dbl, 1);
+    }
+    commit();
+    wait_all();
+    FNR_PHASE(kPhDw);
+    acquire(lock);
+    if (warp < A::kWarps) {
+      float4* a4 = reinterpret_cast<float4*>(acc) + warp * (KP / 8) * 32 + lane;
+#pragma unroll
+      for (int q = 0; q < KP / 8; ++q) {
+        float4 v = a4[q * 32];
+        v.x += d[4 * q];
+        v.y += d[4 * q + 1];
+        v.z += d[4 * q + 2];
+        v.w += d[4 * q + 3];
+        a4[q * 32] = v;
+      }
+    }
+    if (half == 1 && t < N) acc[A::kW + t] += part[t] + part[kWarpPartial + t] + part[2 * kWarpPartial + t] + part[3 * kWarpPartial + t];
+    release(lock);
+    FNR_PHASE(kPhDwFlush);
+  }
+}
+
+// Weight gradient of a narrow fp32 head (N = 1, 3 outputs) over the warpgroup's tile, exact fp32 on the CUDA cores: warp
+// reduce-scatters of dy[n] x[k] and dy[n] into per-warp partials, then the warps' sums are added to acc ([N][K] then
+// [N]).  Every thread of the warpgroup must call it.
+template <int K, int N>
+__device__ __forceinline__ void head_weight_grad_acc(float* part, const float (&x)[K], const float (&dy)[N], float* acc, int* lock) {
+  static_assert(K % 32 == 0 && N * K + N <= kWarpPartial, "head partials");
+  const int t = tid(), warp = t >> 5, lane = t & 31;
+  float* pw = part + warp * kWarpPartial;
+#pragma unroll
+  for (int n = 0; n < N; ++n) warp_column_sums<K>([&](int k) { return dy[n] * x[k]; }, pw + n * K, lane);
+  warp_column_sums<N>([&](int n) { return dy[n]; }, pw + N * K, lane);
+  acquire(lock);  // its barrier also orders the partial stores before the reads below
+  for (int e = t; e < N * K + N; e += 128)
+    acc[e] += part[e] + part[kWarpPartial + e] + part[2 * kWarpPartial + e] + part[3 * kWarpPartial + e];
+  release(lock);
 }
 
 }  // namespace wg

@@ -7,8 +7,9 @@ Each timed call is the autograd backward of `ops.render` (zeroing of the flat gr
 events around it, the L2 flushed before every call as bench.py does.  `--phases` builds the library with
 -DFNR_BWD_PHASE_TIMERS into --build-dir (a temporary directory by default, never the package's own library), and
 prints the clock64() cycles per 128-point tile of every phase of the field backward kernel: stash / upstream loads,
-forward recompute, dx, dW, the dW flush to the global gradient, and the hash-table scatter.  The phase marks
-synchronise the CTA, so the timer build is a little slower than the normal one; its split is what it is for.
+forward recompute, dx, dW, the dW flush to the global gradient (or to the CTA's accumulators, plus the CTA's one flush,
+amortised), and the hash-table scatter.  The phase marks synchronise the warpgroup, so the timer build is a little slower
+than the normal one; its split is what it is for.
 """
 from __future__ import annotations
 
@@ -107,8 +108,8 @@ def main():
         per_tile = {p: buf[i] / tiles for i, p in enumerate(PHASES)}
         res["phase_cycles_per_tile"] = {p: round(v) for p, v in per_tile.items()}
         res["phase_cycles_per_tile_total"] = round(sum(per_tile.values()))
-        res["note"] = ("phase timer build (CTA barrier at every mark): cycles of thread 0 of each CTA per 128-point tile, "
-                       "CTAs sharing an SM overlap")
+        res["note"] = ("phase timer build (warpgroup barrier at every mark): cycles of thread 0 of each warpgroup per "
+                       "128-point tile, warpgroups sharing an SM overlap; dw_flush includes the per-CTA flush, amortised")
     line = json.dumps(res)
     print(line)
     if args.json:
