@@ -222,6 +222,10 @@ EXPORTED_SYMBOLS = (
     "fnr_compose_frame",
     "fnr_pixel_batch_lens",
     "fnr_camera_rays_lens",
+    "fnr_tsdf_integrate",
+    "fnr_marching_cubes_scratch_bytes",
+    "fnr_marching_cubes_count",
+    "fnr_marching_cubes_emit",
 )
 
 _lib = None
@@ -320,6 +324,14 @@ def load() -> C.CDLL:
     lib.fnr_pixel_batch_lens.argtypes = [vp, vp, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]
     lib.fnr_camera_rays_lens.restype = C.c_int
     lib.fnr_camera_rays_lens.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i64, i32, vp, vp, vp]
+    lib.fnr_tsdf_integrate.restype = C.c_int
+    lib.fnr_tsdf_integrate.argtypes = [vp, vp, vp, vp, i64, i64, i64, _f32p, _f32p, f32, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, vp]
+    lib.fnr_marching_cubes_scratch_bytes.restype = C.c_int
+    lib.fnr_marching_cubes_scratch_bytes.argtypes = [i64, i64, i64, C.POINTER(C.c_size_t)]
+    lib.fnr_marching_cubes_count.restype = C.c_int
+    lib.fnr_marching_cubes_count.argtypes = [vp, i64, i64, i64, vp, sz, vp, vp]
+    lib.fnr_marching_cubes_emit.restype = C.c_int
+    lib.fnr_marching_cubes_emit.argtypes = [vp, vp, vp, i64, i64, i64, _f32p, _f32p, vp, sz, i64, i64, vp, vp, vp, vp, vp, vp]
     if lib.fnr_version() != ABI_VERSION:
         raise FruitNerfNativeError(f"ABI version mismatch: library reports {lib.fnr_version()}")
     _lib = lib

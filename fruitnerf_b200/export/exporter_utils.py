@@ -303,3 +303,202 @@ def read_line_set_points(path) -> np.ndarray:
     if vertex is None or not {"x", "y", "z"} <= set(vertex):
         raise ValueError(f"{path}: no vertex x/y/z")
     return np.stack([vertex["x"], vertex["y"], vertex["z"]], axis=1).astype(np.float64)
+
+
+# ---- the `tsdf` mesh export (nerfstudio 0.3.2 exporter_utils / tsdf_utils.export_tsdf_mesh) ------------------------------
+def tsdf_cameras(cameras, downscale_factor: float = 2):
+    """The training cameras as distortion-free perspective render cameras (``render.CameraSet``), rescaled by
+    1 / ``downscale_factor``: upstream renders them with ``disable_distortion=True``.  Fisheye and equirectangular cameras
+    are refused: a TSDF projects grid points through a pinhole."""
+    from ..render import CameraSet
+
+    if cameras.camera_type != "perspective":
+        raise ValueError(f"the tsdf export needs perspective cameras; these are {cameras.camera_type!r}")
+    if downscale_factor < 1:
+        raise ValueError(f"downscale_factor must be >= 1, got {downscale_factor}")
+    return CameraSet.from_cameras(cameras).rescale_output_resolution(1.0 / downscale_factor)
+
+
+@torch.no_grad()
+def _fuse(model, cams, tsdf, batch_size: int, depth_output_name: str, rgb_output_name: str) -> None:
+    """Render every camera (rays from fnr_camera_rays, the model's forward chunk by chunk into device frame buffers) and fuse
+    ``batch_size`` frames at a time.  Nothing goes to the host."""
+    from ..compat import RayBundle
+
+    dev = tsdf.device
+    cams = cams.to(dev)
+    H, W = cams.height, cams.width
+    P = H * W
+    chunk = min(int(model.config.eval_num_rays_per_chunk), P)
+    o_buf = torch.empty((chunk, 3), dtype=torch.float32, device=dev)
+    d_buf = torch.empty((chunk, 3), dtype=torch.float32, device=dev)
+    F = len(cams)
+    for f0 in range(0, F, batch_size):
+        n = min(batch_size, F - f0)
+        depth = torch.empty((n, P), dtype=torch.float32, device=dev)
+        rgb = torch.empty((n, P, 3), dtype=torch.float32, device=dev)
+        fruit = torch.empty((n, P), dtype=torch.float32, device=dev)
+        for b in range(n):
+            cam_idx = torch.full((chunk, 1), f0 + b, dtype=torch.long, device=dev)
+            for p0 in range(0, P, chunk):
+                m = min(chunk, P - p0)
+                o, d = ops.camera_rays(cams.camera_to_worlds, cams.fx, cams.fy, cams.cx, cams.cy, "perspective", H, W, f0 + b, p0, m,
+                                       out=(o_buf, d_buf))
+                out = model(RayBundle(origins=o, directions=d, camera_indices=cam_idx[:m]))
+                for name in (depth_output_name, rgb_output_name, "semantics"):
+                    if name not in out:
+                        raise KeyError(f"the model has no output {name!r}")
+                depth[b, p0:p0 + m] = out[depth_output_name].reshape(m)
+                rgb[b, p0:p0 + m] = out[rgb_output_name].reshape(m, 3)
+                fruit[b, p0:p0 + m] = torch.sigmoid(out["semantics"].reshape(m))
+        sl = slice(f0, f0 + n)
+        tsdf.integrate(cams.camera_to_worlds[sl], cams.fx[sl].float(), cams.fy[sl].float(), cams.cx[sl].float(), cams.cy[sl].float(),
+                       depth.view(n, H, W), rgb.view(n, H, W, 3), fruit.view(n, H, W))
+
+
+def export_tsdf_mesh(pipeline, output_dir, downscale_factor: int = 2, depth_output_name: str = "depth", rgb_output_name: str = "rgb",
+                     resolution=128, batch_size: int = 10, use_bounding_box: bool = True, bounding_box_min=(-1.0, -1.0, -1.0),
+                     bounding_box_max=(1.0, 1.0, 1.0), refine_mesh_using_initial_aabb_estimate: bool = False,
+                     refinement_epsilon: float = 1e-2) -> Dict:
+    """nerfstudio export_tsdf_mesh on the GPU: render the training cameras at 1 / ``downscale_factor`` resolution, fuse
+    them ``batch_size`` frames at a time into a ``resolution``^3 TSDF (one value or three) spanning the bounding box (or
+    the scene box), and extract the level-0 mesh.  With ``refine_mesh_using_initial_aabb_estimate`` the fusion runs again
+    in the first mesh's vertex box widened by ``refinement_epsilon``.  The projection uses the rescaled intrinsics, those
+    of the rendered images.
+
+    Writes ``tsdf_mesh.ply`` (every face, vertex colours) and ``fruit_mesh.ply`` (the faces whose three vertices have a
+    fused fruit probability >= 0.5, vertices compacted in order; possibly empty) in the dataparser frame.  An empty mesh
+    raises RuntimeError and writes nothing.  Returns {'mesh', 'fruit_mesh': dicts of numpy arrays, 'aabb' [2,3] of the
+    final grid, 'paths'}."""
+    from .. import mesh as M
+
+    model = pipeline.model
+    dev = next(model.parameters()).device
+    if dev.type != "cuda":
+        raise RuntimeError("export_tsdf_mesh needs the model on a CUDA device: the fusion and marching cubes are CUDA kernels")
+    res = [int(r) for r in (resolution if isinstance(resolution, (list, tuple)) else [resolution])]
+    if len(res) not in (1, 3) or min(res) < 2:
+        raise ValueError(f"resolution must be one or three integers >= 2, got {resolution}")
+    res = res * 3 if len(res) == 1 else res
+    if batch_size < 1:
+        raise ValueError(f"batch_size must be >= 1, got {batch_size}")
+    if use_bounding_box:
+        if not all(lo < hi for lo, hi in zip(bounding_box_min, bounding_box_max)):
+            raise ValueError("Bounding box min must be smaller than max")
+        aabb = torch.tensor([list(bounding_box_min), list(bounding_box_max)], dtype=torch.float32)
+    else:
+        aabb = pipeline.datamanager.train_dataset.scene_box.aabb.detach().float().cpu()
+    cams = tsdf_cameras(pipeline.datamanager.train_dataset.cameras, downscale_factor)
+
+    def run(box):
+        tsdf = M.TSDF.from_aabb(box, res, device=dev)
+        _fuse(model, cams, tsdf, batch_size, depth_output_name, rgb_output_name)
+        out = {k: (None if v is None else v.cpu().numpy()) for k, v in tsdf.get_mesh().items()}
+        if out["faces"].shape[0] == 0:
+            raise RuntimeError(f"the TSDF in the box {box.tolist()} gave an empty mesh: check the bounding box and the trained model")
+        return out
+
+    mesh = run(aabb)
+    if refine_mesh_using_initial_aabb_estimate:
+        v = torch.from_numpy(mesh["vertices"])
+        aabb = torch.stack([v.min(dim=0).values - refinement_epsilon, v.max(dim=0).values + refinement_epsilon]).float()
+        mesh = run(aabb)
+    fv, fn, fc, ff, fidx = M.fruit_submesh(mesh["vertices"], mesh["normals"], mesh["colors"], mesh["fruit"], mesh["faces"])
+    fruit_mesh = {"vertices": fv, "normals": fn, "colors": fc, "fruit": ff, "faces": fidx}
+    out_dir = pathlib.Path(output_dir)
+    paths = {"mesh": str(out_dir / "tsdf_mesh.ply"), "fruit_mesh": str(out_dir / "fruit_mesh.ply")}
+    write_mesh_ply(paths["mesh"], mesh["vertices"], mesh["normals"], mesh["colors"], mesh["faces"])
+    write_mesh_ply(paths["fruit_mesh"], fv, fn, fc, fidx)
+    return {"mesh": mesh, "fruit_mesh": fruit_mesh, "aabb": aabb.numpy(), "paths": paths}
+
+
+_FACE_DTYPE = np.dtype([("n", "u1"), ("v", "<i4", (3,))])  # packed: 13 bytes per face
+
+
+def write_mesh_ply(path, vertices: np.ndarray, normals: np.ndarray, colors: Optional[np.ndarray], faces: np.ndarray) -> None:
+    """Binary little-endian triangle mesh: vertex double x/y/z, double nx/ny/nz, uchar red/green/blue (``write_ply``'s
+    colour conversion; black without ``colors``), then ``face`` rows of ``list uchar int vertex_indices``."""
+    v = np.asarray(vertices, dtype="<f8").reshape(-1, 3)
+    n = v.shape[0]
+    f = np.asarray(faces, dtype=np.int64).reshape(-1, 3)
+    if f.size and (f.min() < 0 or f.max() >= n or n > 0x7FFFFFFF):
+        raise ValueError(f"face indices must lie in [0, {n}) and fit an int")
+    col = np.zeros((n, 3), np.uint8) if colors is None else np.clip(np.asarray(colors, dtype=np.float64).reshape(-1, 3) * 255.0, 0, 255).astype(np.uint8)
+    nrm = np.asarray(normals, dtype="<f8").reshape(-1, 3)
+    header = (
+        "ply\nformat binary_little_endian 1.0\ncomment fruitnerf_b200 export\n"
+        f"element vertex {n}\nproperty double x\nproperty double y\nproperty double z\n"
+        "property double nx\nproperty double ny\nproperty double nz\n"
+        "property uchar red\nproperty uchar green\nproperty uchar blue\n"
+        f"element face {f.shape[0]}\nproperty list uchar int vertex_indices\nend_header\n"
+    )
+    rec = np.empty(n, dtype=[("p", "<f8", (3,)), ("n", "<f8", (3,)), ("c", "u1", (3,))])
+    rec["p"], rec["n"], rec["c"] = v, nrm, col
+    frec = np.empty(f.shape[0], dtype=_FACE_DTYPE)
+    frec["n"], frec["v"] = 3, f
+    pathlib.Path(path).parent.mkdir(parents=True, exist_ok=True)
+    with open(path, "wb") as fh:
+        fh.write(header.encode("ascii"))
+        fh.write(rec.tobytes())
+        fh.write(frec.tobytes())
+
+
+def read_mesh_ply(path):
+    """A binary little-endian triangle mesh as ``write_mesh_ply`` writes it -> (vertices [N,3], normals [N,3] or None,
+    colors [N,3] in [0,1] or None, faces [F,3] int64).  Scalar vertex properties of any type are read by name; the face
+    element must hold one ``list uchar int`` (or ``uint``) property of triangles."""
+    with open(path, "rb") as f:
+        if f.readline().strip() != b"ply":
+            raise ValueError(f"{path}: not a PLY file")
+        fmt, elements = None, []
+        while True:
+            line = f.readline()
+            if not line:
+                raise ValueError(f"{path}: PLY header has no end_header")
+            tok = line.decode("ascii", "replace").split()
+            if not tok or tok[0] in ("comment", "obj_info"):
+                continue
+            if tok[0] == "end_header":
+                break
+            if tok[0] == "format":
+                fmt = tok[1]
+            elif tok[0] == "element":
+                elements.append((tok[1], int(tok[2]), []))
+            elif tok[0] == "property":
+                if not elements:
+                    raise ValueError(f"{path}: property before any element")
+                if tok[1] == "list":
+                    if tok[2] not in ("uchar", "uint8") or tok[3] not in ("int", "int32", "uint", "uint32"):
+                        raise ValueError(f"{path}: unsupported list property {' '.join(tok[1:])}")
+                    elements[-1][2].append((tok[4], "list", _PLY_TYPES[tok[3]]))
+                elif tok[1] in _PLY_TYPES:
+                    elements[-1][2].append((tok[2], _PLY_TYPES[tok[1]], None))
+                else:
+                    raise ValueError(f"{path}: unknown PLY type '{tok[1]}'")
+        if fmt != "binary_little_endian":
+            raise ValueError(f"{path}: only binary_little_endian PLY is supported, got {fmt}")
+        vertex, faces = None, np.zeros((0, 3), np.int64)
+        for name, count, props in elements:
+            lists = [p for p in props if p[1] == "list"]
+            if lists:
+                if name != "face" or len(props) != 1:
+                    raise ValueError(f"{path}: list properties are only read as the face element's single vertex list")
+                dt = np.dtype([("n", "u1"), ("v", lists[0][2], (3,))])
+                rec = np.frombuffer(f.read(count * dt.itemsize), dtype=dt, count=count)
+                if count and (rec["n"] != 3).any():
+                    raise ValueError(f"{path}: only triangle faces are supported")
+                faces = rec["v"].astype(np.int64)
+                continue
+            dt = np.dtype([(p[0], p[1]) for p in props])
+            rec = np.frombuffer(f.read(count * dt.itemsize), dtype=dt, count=count)
+            if name == "vertex":
+                vertex = rec
+            elif count:
+                raise ValueError(f"{path}: unexpected element '{name}' with {count} rows")
+    if vertex is None or not {"x", "y", "z"} <= set(vertex.dtype.names):
+        raise ValueError(f"{path}: no vertex x/y/z")
+    names = set(vertex.dtype.names)
+    stack = lambda keys: np.stack([vertex[k] for k in keys], axis=1).astype(np.float64)  # noqa: E731
+    normals = stack(("nx", "ny", "nz")) if {"nx", "ny", "nz"} <= names else None
+    colors = stack(("red", "green", "blue")) / 255.0 if {"red", "green", "blue"} <= names else None
+    return stack(("x", "y", "z")), normals, colors, faces

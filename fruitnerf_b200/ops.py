@@ -929,3 +929,76 @@ def compose_frame(images: Sequence[FrameImage], accumulation: Optional[Tensor], 
         raise ValueError(f"out must be contiguous uint8 [{height}, {width * k}, 3]")
     L.check(L.load().fnr_compose_frame(arr, k, _ptr(acc), int(height), int(width), _ptr(turbo), _ptr(scratch), _ptr(out), _stream(dev)))
     return out
+
+
+# ======================================================================================================
+# Surface meshes (fnr_mesh.cu; nerfstudio ns-export tsdf)
+# ======================================================================================================
+def _host3(v, what: str):
+    """HOST float[3] of a per-axis value (a scalar, three values or a tensor)."""
+    a = [float(x) for x in (v.detach().cpu().reshape(-1).tolist() if torch.is_tensor(v) else np.asarray(v, dtype=np.float64).reshape(-1))]
+    if len(a) == 1:
+        a = a * 3
+    if len(a) != 3:
+        raise ValueError(f"{what} must be one or three values, got {len(a)}")
+    return (C.c_float * 3)(*a)
+
+
+def _grid_dims(values: Tensor) -> Tuple[int, int, int]:
+    if values.dim() != 3 or values.dtype != torch.float32 or not values.is_contiguous():
+        raise ValueError(f"grid values must be a contiguous fp32 [X,Y,Z] tensor, got {values.dtype} {tuple(values.shape)}")
+    return tuple(int(d) for d in values.shape)
+
+
+def tsdf_integrate(values: Tensor, weights: Tensor, colors: Tensor, fruit_state: Optional[Tensor], origin, voxel_size, truncation: float,
+                   c2w: Tensor, fx, fy, cx, cy, depth: Tensor, rgb: Tensor, fruit: Optional[Tensor] = None) -> None:
+    """Fuse B frames into a TSDF grid in place (fnr_tsdf_integrate): state ``values`` / ``weights`` / ``fruit_state`` [X,Y,Z]
+    and ``colors`` [X,Y,Z,3], contiguous fp32 CUDA tensors; frames c2w [B,3,4], fx / fy / cx / cy [B] (or scalars),
+    depth [B,H,W] (ray distance), rgb [B,H,W,3], fruit [B,H,W] or None."""
+    dev = _require_cuda(values, weights, colors, fruit_state, c2w, depth, rgb, fruit)
+    X, Y, Z = _grid_dims(values)
+    for name, t, shape in (("weights", weights, (X, Y, Z)), ("colors", colors, (X, Y, Z, 3)), ("fruit_state", fruit_state, (X, Y, Z))):
+        if t is not None and (tuple(t.shape) != shape or t.dtype != torch.float32 or not t.is_contiguous()):
+            raise ValueError(f"{name} must be a contiguous fp32 {list(shape)} tensor")
+    if fruit is not None and fruit_state is None:
+        raise ValueError("frame fruit probabilities need a fruit_state grid")
+    B = int(c2w.shape[0])
+    c2w = _f32c(c2w.detach().reshape(B, 3, 4))
+    depth = _f32c(depth.detach())
+    H, W = int(depth.shape[1]), int(depth.shape[2])
+    depth = depth.reshape(B, H, W)
+    rgb = _f32c(rgb.detach().reshape(B, H, W, 3))
+    fruit = None if fruit is None else _f32c(fruit.detach().reshape(B, H, W))
+    fx, fy, cx, cy = (_f32c(torch.as_tensor(t, dtype=torch.float32, device=dev).reshape(-1).expand(B)) for t in (fx, fy, cx, cy))
+    L.check(L.load().fnr_tsdf_integrate(_ptr(values), _ptr(weights), _ptr(colors), _ptr(fruit_state) if fruit is not None else None, X, Y, Z,
+                                        _host3(origin, "origin"), _host3(voxel_size, "voxel_size"), float(truncation), _ptr(c2w), _ptr(fx),
+                                        _ptr(fy), _ptr(cx), _ptr(cy), _ptr(depth), _ptr(rgb), _ptr(fruit), B, H, W, _stream(dev)))
+
+
+def marching_cubes(values: Tensor, origin, voxel_size, colors: Optional[Tensor] = None, fruit: Optional[Tensor] = None) -> dict:
+    """Level-0 isosurface of a CUDA fp32 grid [X,Y,Z] (fnr_marching_cubes_count / _emit): {'vertices' [V,3], 'normals' [V,3],
+    'colors' [V,3] or None, 'fruit' [V] or None (fp32), 'faces' [F,3] int64}, all on the device.  One host read (the
+    vertex and face counts) between the passes."""
+    dev = _require_cuda(values, colors, fruit)
+    values = _f32c(values.detach())
+    X, Y, Z = _grid_dims(values)
+    colors = None if colors is None else _f32c(colors.detach().reshape(X, Y, Z, 3))
+    fruit = None if fruit is None else _f32c(fruit.detach().reshape(X, Y, Z))
+    lib = L.load()
+    nbytes = C.c_size_t(0)
+    L.check(lib.fnr_marching_cubes_scratch_bytes(X, Y, Z, C.byref(nbytes)))
+    scratch = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+    totals = torch.zeros(2, dtype=torch.int64, device=dev)
+    L.check(lib.fnr_marching_cubes_count(_ptr(values), X, Y, Z, _ptr(scratch), nbytes.value, _ptr(totals), _stream(dev)))
+    V, F = (int(v) for v in totals.cpu().tolist())
+    if V > 0x7FFFFFFF:  # the library refuses it before touching any output
+        L.check(lib.fnr_marching_cubes_emit(_ptr(values), None, None, X, Y, Z, _host3(origin, "origin"), _host3(voxel_size, "voxel_size"),
+                                            _ptr(scratch), nbytes.value, V, F, None, None, None, None, None, _stream(dev)))
+    f32 = dict(dtype=torch.float32, device=dev)
+    out = {"vertices": torch.empty((V, 3), **f32), "normals": torch.empty((V, 3), **f32),
+           "colors": None if colors is None else torch.empty((V, 3), **f32), "fruit": None if fruit is None else torch.empty(V, **f32),
+           "faces": torch.empty((F, 3), dtype=torch.int64, device=dev)}
+    L.check(lib.fnr_marching_cubes_emit(_ptr(values), _ptr(colors), _ptr(fruit), X, Y, Z, _host3(origin, "origin"), _host3(voxel_size, "voxel_size"),
+                                        _ptr(scratch), nbytes.value, V, F, _ptr(out["vertices"]), _ptr(out["normals"]), _ptr(out["colors"]),
+                                        _ptr(out["fruit"]), _ptr(out["faces"]), _stream(dev)))
+    return out

@@ -17,7 +17,7 @@ from typing import Optional, Tuple
 
 import torch
 
-from ..export.exporter_utils import generate_point_cloud, sample_volume, write_ply
+from ..export.exporter_utils import export_tsdf_mesh, generate_point_cloud, sample_volume, write_ply
 
 
 def eval_setup(config_path, eval_num_rays_per_chunk: Optional[int] = None, test_mode: str = "test", device: Optional[str] = None):
@@ -139,6 +139,56 @@ class ExportPointCloud(Exporter):
         return pcd
 
 
+@dataclass
+class ExportTSDFMesh(Exporter):
+    """nerfstudio 0.3.2 ExportTSDFMesh: a surface mesh of the scene by TSDF fusion of rendered depth maps, plus the mesh of
+    the fruit surfaces (faces whose vertices have a fused fruit probability >= 0.5).  Single GPU.  Only vertex colours
+    (``texture_method="tsdf"``) are implemented: NeRF texturing needs an xatlas UV unwrap."""
+
+    downscale_factor: int = 2
+    depth_output_name: str = "depth"
+    rgb_output_name: str = "rgb"
+    resolution: Tuple[int, ...] = (128,)
+    batch_size: int = 10
+    use_bounding_box: bool = True
+    bounding_box_min: Tuple[float, float, float] = (-1, -1, -1)
+    bounding_box_max: Tuple[float, float, float] = (1, 1, 1)
+    texture_method: str = "tsdf"
+    refine_mesh_using_initial_aabb_estimate: bool = False
+    refinement_epsilon: float = 1e-2
+
+    def validate(self) -> None:
+        """Refuse what cannot run, before anything is loaded."""
+        if self.texture_method == "nerf":
+            raise ValueError("texture_method 'nerf' needs an xatlas UV unwrap, which is not available; use 'tsdf' (vertex colours)")
+        if self.texture_method != "tsdf":
+            raise ValueError(f"texture_method must be 'tsdf' or 'nerf', got {self.texture_method!r}")
+        res = tuple(self.resolution) if isinstance(self.resolution, (list, tuple)) else (self.resolution,)
+        if len(res) not in (1, 3) or min(int(r) for r in res) < 2:
+            raise ValueError(f"resolution must be one or three integers >= 2, got {list(res)}")
+        if self.downscale_factor < 1:
+            raise ValueError(f"downscale_factor must be >= 1, got {self.downscale_factor}")
+        if self.batch_size < 1:
+            raise ValueError(f"batch_size must be >= 1, got {self.batch_size}")
+        if self.use_bounding_box and not all(lo < hi for lo, hi in zip(self.bounding_box_min, self.bounding_box_max)):
+            raise ValueError("Bounding box min must be smaller than max")
+
+    def main(self, pipeline=None) -> dict:
+        """Writes ``output_dir/tsdf_mesh.ply`` and ``output_dir/fruit_mesh.ply``; returns export_tsdf_mesh's dict."""
+        self.validate()
+        if pipeline is None:
+            if self.load_config is None:
+                raise ValueError("pass load_config (a run folder's config.yml) or an already built pipeline")
+            _, pipeline, _, _ = eval_setup(self.load_config)
+        res = list(self.resolution) if isinstance(self.resolution, (list, tuple)) else [self.resolution]
+        return export_tsdf_mesh(pipeline, Path(self.output_dir), downscale_factor=self.downscale_factor, depth_output_name=self.depth_output_name,
+                                rgb_output_name=self.rgb_output_name, resolution=res, batch_size=self.batch_size,
+                                use_bounding_box=self.use_bounding_box, bounding_box_min=self.bounding_box_min,
+                                bounding_box_max=self.bounding_box_max,
+                                refine_mesh_using_initial_aabb_estimate=self.refine_mesh_using_initial_aabb_estimate,
+                                refinement_epsilon=self.refinement_epsilon)
+
+
 def _require_normal_output(pipeline, normal_output_name: str) -> None:
     """nerfstudio validate_pipeline: render one ray and exit(1) if ``normal_output_name`` is not among the outputs."""
     from ..compat import RayBundle
@@ -183,13 +233,45 @@ def add_pointcloud_parser(sub) -> argparse.ArgumentParser:
     return p
 
 
+def add_tsdf_parser(sub) -> argparse.ArgumentParser:
+    """The ``tsdf`` subcommand: ExportTSDFMesh's fields as nerfstudio's option names, same defaults (texture method
+    ``tsdf``, the only one implemented)."""
+    d = ExportTSDFMesh(load_config=None, output_dir=Path("."))
+    p = sub.add_parser("tsdf", help="surface meshes of the scene and of the fruit by TSDF fusion of rendered depth")
+    p.add_argument("--load-config", type=Path, required=True)
+    p.add_argument("--output-dir", type=Path, required=True)
+    p.add_argument("--downscale-factor", type=int, default=d.downscale_factor)
+    p.add_argument("--depth-output-name", default=d.depth_output_name)
+    p.add_argument("--rgb-output-name", default=d.rgb_output_name)
+    p.add_argument("--resolution", type=int, nargs="+", default=list(d.resolution))
+    p.add_argument("--batch-size", type=int, default=d.batch_size)
+    p.add_argument("--use-bounding-box", type=_flag, default=d.use_bounding_box)
+    p.add_argument("--bounding-box-min", type=float, nargs=3, default=d.bounding_box_min)
+    p.add_argument("--bounding-box-max", type=float, nargs=3, default=d.bounding_box_max)
+    p.add_argument("--texture-method", choices=("tsdf", "nerf"), default=d.texture_method)
+    p.add_argument("--refine-mesh-using-initial-aabb-estimate", type=_flag, default=d.refine_mesh_using_initial_aabb_estimate)
+    p.add_argument("--refinement-epsilon", type=float, default=d.refinement_epsilon)
+    return p
+
+
+def tsdf_exporter_from_args(a) -> ExportTSDFMesh:
+    return ExportTSDFMesh(load_config=a.load_config, output_dir=a.output_dir, downscale_factor=a.downscale_factor,
+                          depth_output_name=a.depth_output_name, rgb_output_name=a.rgb_output_name, resolution=tuple(a.resolution),
+                          batch_size=a.batch_size, use_bounding_box=a.use_bounding_box, bounding_box_min=tuple(a.bounding_box_min),
+                          bounding_box_max=tuple(a.bounding_box_max), texture_method=a.texture_method,
+                          refine_mesh_using_initial_aabb_estimate=a.refine_mesh_using_initial_aabb_estimate,
+                          refinement_epsilon=a.refinement_epsilon)
+
+
 def entrypoint(argv=None):
     """``ns-export-semantics semantic-pointcloud --load-config RUN/config.yml --output-dir OUT [...]`` (exporter.py:124-144;
     upstream parses the same dataclass with tyro, which is not available offline -- argparse with the same option names)
-    and ``ns-export-semantics pointcloud ...`` (nerfstudio ExportPointCloud)."""
+    , ``ns-export-semantics pointcloud ...`` (nerfstudio ExportPointCloud) and ``ns-export-semantics tsdf ...`` (nerfstudio
+    ExportTSDFMesh)."""
     ap = argparse.ArgumentParser(prog="ns-export-semantics")
     sub = ap.add_subparsers(dest="command", required=True)
     add_pointcloud_parser(sub)
+    tsdf_parser = add_tsdf_parser(sub)
     p = sub.add_parser("semantic-pointcloud", help="uniform-volume export of the fruit point clouds")
     p.add_argument("--load-config", type=Path, required=True)
     p.add_argument("--output-dir", type=Path, required=True)
@@ -200,6 +282,23 @@ def entrypoint(argv=None):
     p.add_argument("--num-points-per-side", type=int, default=1000)
     p.add_argument("--stratified-jitter", type=lambda s: s.lower() in ("1", "true", "yes"), default=True)
     a = ap.parse_args(argv)
+    if a.command == "tsdf":
+        exp = tsdf_exporter_from_args(a)
+        try:
+            exp.validate()
+        except ValueError as e:
+            tsdf_parser.error(str(e))
+        try:
+            res = exp.main()
+        except RuntimeError as e:
+            if "empty mesh" not in str(e):
+                raise
+            print(f"error: {e}", file=sys.stderr)
+            sys.exit(1)
+        for key in ("mesh", "fruit_mesh"):
+            m = res[key]
+            print(f"{key}: {m['vertices'].shape[0]} vertices, {m['faces'].shape[0]} faces -> {res['paths'][key]}")
+        return res
     if a.command == "pointcloud":
         exp = ExportPointCloud(load_config=a.load_config, output_dir=a.output_dir, num_points=a.num_points, remove_outliers=a.remove_outliers,
                                reorient_normals=a.reorient_normals, normal_method=a.normal_method, normal_output_name=a.normal_output_name,

@@ -53,6 +53,9 @@
  *   fnr_pixel_batch_lens, fnr_camera_rays_lens
  *                        training and evaluation rays of captured data sets (fruit_nerf/data/fruitnerf_dataparser.py
  *                        cameras): per-frame intrinsics, OpenCV lens distortion, fisheye and equirectangular models
+ *   fnr_tsdf_integrate, fnr_marching_cubes_scratch_bytes, fnr_marching_cubes_count, fnr_marching_cubes_emit
+ *                        the `tsdf` mesh export (nerfstudio ns-export tsdf: TSDF.integrate_tsdf, skimage
+ *                        marching_cubes): fusion of rendered depth maps and the scene / fruit surface meshes
  */
 #ifndef FRUITNERF_B200_H
 #define FRUITNERF_B200_H
@@ -528,6 +531,41 @@ typedef struct fnr_frame_output {
  * float[FNR_COMPOSE_SCRATCH_FLOATS] (NULL when no output uses auto_range).  Exact: min / max do not depend on order. */
 int fnr_compose_frame(const fnr_frame_output* outputs, int32_t num_outputs, const float* accumulation, int32_t height, int32_t width,
                       const float* turbo, float* scratch, uint8_t* image, void* stream);
+
+/* ---- Surface meshes (`ns-export-semantics tsdf`, nerfstudio ns-export tsdf; fnr_mesh.cu) ----
+ * Grids are DEVICE fp32 in C order [nx, ny, nz] (z fastest); grid point (i,j,k) lies at origin + (i,j,k) * voxel_size per
+ * axis (origin, voxel_size: HOST float[3]).  Every voxel, vertex and face count and index is int64.
+ *
+ * fnr_tsdf_integrate fuses num_frames rendered frames into the grid in place, frame after frame (no atomics: the result
+ * does not depend on the launch).  State: values [N] (start at -1), weights [N] (start at 0; a plain count), colors
+ * [N,3], fruit [N] (may be NULL when frame_fruit is).  Frames: c2w [B,3,4] (OpenGL axes), fx, fy, cx, cy [B], depth
+ * [B,H,W] (the ray distance the model renders), rgb [B,H,W,3], frame_fruit [B,H,W] probabilities or NULL.  Per grid
+ * point x and frame: p = R^T (x - t), z_c = -p.z (skip if <= 0); u = cx + fx p.x / z_c, v = cy - fy p.y / z_c; pixel
+ * (floor u, floor v) (skip if off the image); the pixel's ray distance t becomes the depth
+ * z = t / sqrt(((x + 0.5 - cx) / fx)^2 + ((y + 0.5 - cy) / fy)^2 + 1) of its centre ray; sdf = z - z_c (skip if t <= 0
+ * or sdf <= -truncation); value, colour and fruit become (old * w + new) / (w + 1) with tsdf = clamp(sdf / truncation,
+ * -1, 1), and w += 1.  FNR_ERR_INVALID_ARGUMENT: NULL state or inputs, a dim < 2, non-finite or non-positive voxel size
+ * or truncation, H or W <= 0, num_frames < 0.  num_frames = 0 does nothing. */
+int fnr_tsdf_integrate(float* values, float* weights, float* colors, float* fruit, int64_t nx, int64_t ny, int64_t nz, const float* origin,
+                       const float* voxel_size, float truncation, const float* c2w, const float* fx, const float* fy, const float* cx,
+                       const float* cy, const float* depth, const float* rgb, const float* frame_fruit, int32_t num_frames, int32_t height,
+                       int32_t width, void* stream);
+
+/* Marching cubes of values at level 0 (a corner is inside iff its value is < 0), in two passes around a host read of the
+ * counts: fnr_marching_cubes_count fills DEVICE scratch (fnr_marching_cubes_scratch_bytes) and writes DEVICE
+ * totals[2] = {vertices, faces}; fnr_marching_cubes_emit then writes vertices [V,3], unit normals [V,3] (the interpolated
+ * central-difference gradient: toward increasing value; where it vanishes, the edge direction toward its outside end),
+ * vertex_colors [V,3] / vertex_fruit [V] (the nearest grid
+ * point's, round half to even; NULL exactly when colors / fruit is) and faces [F,3] int64.  Each grid edge with one
+ * inside endpoint carries one vertex, ids in (point linear index, axis) order; faces run in cell order, then in the
+ * order of the crack-free, orientable triangle table of fnr_mesh_table.h.  More than 2^31 - 1 vertices return
+ * FNR_ERR_UNSUPPORTED (a PLY face list holds int indices). */
+int fnr_marching_cubes_scratch_bytes(int64_t nx, int64_t ny, int64_t nz, size_t* bytes);
+int fnr_marching_cubes_count(const float* values, int64_t nx, int64_t ny, int64_t nz, void* scratch, size_t scratch_bytes, int64_t* totals,
+                             void* stream);
+int fnr_marching_cubes_emit(const float* values, const float* colors, const float* fruit, int64_t nx, int64_t ny, int64_t nz, const float* origin,
+                            const float* voxel_size, const void* scratch, size_t scratch_bytes, int64_t num_vertices, int64_t num_faces,
+                            float* vertices, float* normals, float* vertex_colors, float* vertex_fruit, int64_t* faces, void* stream);
 
 /* Hash-grid row indices (exact-integer parity hook): rows[N,L,8] in nerfstudio corner order for
  * the masked [0,1]^3 positions of the given samples; also writes positions[N,3] if non-NULL. */
