@@ -226,6 +226,11 @@ EXPORTED_SYMBOLS = (
     "fnr_marching_cubes_scratch_bytes",
     "fnr_marching_cubes_count",
     "fnr_marching_cubes_emit",
+    "fnr_poisson_scratch_bytes",
+    "fnr_poisson_splat",
+    "fnr_poisson_apply",
+    "fnr_poisson_solve",
+    "fnr_poisson_sample",
 )
 
 _lib = None
@@ -332,6 +337,16 @@ def load() -> C.CDLL:
     lib.fnr_marching_cubes_count.argtypes = [vp, i64, i64, i64, vp, sz, vp, vp]
     lib.fnr_marching_cubes_emit.restype = C.c_int
     lib.fnr_marching_cubes_emit.argtypes = [vp, vp, vp, i64, i64, i64, _f32p, _f32p, vp, sz, i64, i64, vp, vp, vp, vp, vp, vp]
+    lib.fnr_poisson_scratch_bytes.restype = C.c_int
+    lib.fnr_poisson_scratch_bytes.argtypes = [i64, i32, C.POINTER(C.c_size_t)]
+    lib.fnr_poisson_splat.restype = C.c_int
+    lib.fnr_poisson_splat.argtypes = [vp, vp, vp, vp, i64, i32, f64p, f64, vp, sz, vp, vp, vp, vp, vp, vp]
+    lib.fnr_poisson_apply.restype = C.c_int
+    lib.fnr_poisson_apply.argtypes = [i64, i32, f32, vp, sz, vp, vp, vp]
+    lib.fnr_poisson_solve.restype = C.c_int
+    lib.fnr_poisson_solve.argtypes = [vp, vp, vp, vp, i64, i32, f64p, f64, f32, i32, f32, vp, sz, vp, vp, vp, vp, _i64p, f64p, vp]
+    lib.fnr_poisson_sample.restype = C.c_int
+    lib.fnr_poisson_sample.argtypes = [vp, i64, i32, f64p, f64, vp, vp, vp]
     if lib.fnr_version() != ABI_VERSION:
         raise FruitNerfNativeError(f"ABI version mismatch: library reports {lib.fnr_version()}")
     _lib = lib

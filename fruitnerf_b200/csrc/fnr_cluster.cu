@@ -27,53 +27,17 @@
 #include <climits>
 #include <cmath>
 #include "fnr_common.cuh"
+#include "fnr_grid.cuh"
 #include "fnr_kernels.h"
 
 namespace fnr {
 
 namespace {
 
-constexpr int kThreads = 256;
-constexpr int kAxisBits = 21;
-constexpr long long kAxisCells = 1LL << kAxisBits;
-constexpr uint64_t kAxisMask = (uint64_t)kAxisCells - 1;
+constexpr int kThreads = kGridThreads;
 constexpr int kNone = 0x7fffffff;  // "no core point" / "no root": above every int32 point index
 constexpr double kCellShrink = 15.0 / 16.0;
 constexpr double kMaxCoordOverCell = 1099511627776.0;  // 2^40: beyond it a key's rounding error nears the 1/16 margin
-
-__device__ __forceinline__ uint64_t pack_key(long long x, long long y, long long z) {
-  return ((uint64_t)x << (2 * kAxisBits)) | ((uint64_t)y << kAxisBits) | (uint64_t)z;
-}
-
-// floor((p - origin) / h), clamped into the key range: the per-axis voxel key of clustering.voxel_down_sample
-__device__ __forceinline__ long long axis_cell(double p, double origin, double h) {
-  const double c = floor(__ddiv_rn(__dsub_rn(p, origin), h));
-  return c < 0.0 ? 0 : (c > (double)(kAxisCells - 1) ? kAxisCells - 1 : (long long)c);
-}
-
-// The grid as the query kernels see it: sorted positions j = 0..n-1, cells c = 0..*ncells-1.
-struct Grid {
-  int n;
-  const uint64_t* keys;   // [n] cell key of sorted position j
-  const int* perm;        // [n] input index of sorted position j
-  const double* x;        // [n] sorted coordinates
-  const double* y;
-  const double* z;
-  const int* cell_of;     // [n] cell of sorted position j
-  const uint64_t* ukeys;  // [ncells] sorted unique keys
-  const int* cstart;      // [ncells + 1] first sorted position of each cell
-  const int* ncells;      // device scalar
-};
-
-__device__ __forceinline__ int lower_bound(const uint64_t* __restrict__ a, int n, uint64_t k) {
-  int lo = 0, hi = n;
-  while (lo < hi) {
-    const int mid = (lo + hi) >> 1;
-    if (a[mid] < k) lo = mid + 1;
-    else hi = mid;
-  }
-  return lo;
-}
 
 // Calls f(cell, ring) for every occupied cell within +-reach cells of `key` on each axis, ring = Chebyshev distance in
 // cells (0 = the cell itself).  f returns false to stop the walk.  The single-radius kernels walk +-2; the multi-radius
@@ -97,46 +61,6 @@ __device__ __forceinline__ void for_each_near_cell(const Grid& g, int nc, uint64
         if (!f(c, ring)) return;
       }
     }
-  }
-}
-
-// ---- grid construction ----------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kThreads) cell_key_kernel(const double* __restrict__ pts, int n, double ox, double oy, double oz,
-                                                            double h, uint64_t* __restrict__ keys, int* __restrict__ idx) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const double* p = pts + 3 * (size_t)i;
-  keys[i] = pack_key(axis_cell(p[0], ox, h), axis_cell(p[1], oy, h), axis_cell(p[2], oz, h));
-  idx[i] = i;
-}
-
-// sorted coordinates + "first of its cell" flags (inclusive-scanned into cell_of afterwards)
-__global__ void __launch_bounds__(kThreads) gather_kernel(const double* __restrict__ pts, int n, const uint64_t* __restrict__ keys,
-                                                          const int* __restrict__ perm, double* __restrict__ x, double* __restrict__ y,
-                                                          double* __restrict__ z, int* __restrict__ first) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= n) return;
-  const double* p = pts + 3 * (size_t)perm[j];
-  x[j] = p[0];
-  y[j] = p[1];
-  z[j] = p[2];
-  first[j] = j == 0 || keys[j] != keys[j - 1];
-}
-
-// cell_of holds the inclusive scan of the flags on entry and the 0-based cell of each sorted position on exit
-__global__ void __launch_bounds__(kThreads) cells_kernel(int n, const uint64_t* __restrict__ keys, int* __restrict__ cell_of,
-                                                         uint64_t* __restrict__ ukeys, int* __restrict__ cstart, int* __restrict__ ncells) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= n) return;
-  const int c = cell_of[j] - 1;
-  cell_of[j] = c;
-  if (j == 0 || keys[j] != keys[j - 1]) {
-    ukeys[c] = keys[j];
-    cstart[c] = j;
-  }
-  if (j == n - 1) {
-    *ncells = c + 1;
-    cstart[c + 1] = n;
   }
 }
 
@@ -763,26 +687,12 @@ __global__ void __launch_bounds__(kSelectThreads) backproject_select_kernel(
 }
 
 // ---- host side ------------------------------------------------------------------------------------------------------
-// Caller-owned device scratch, carved in a fixed order (base == nullptr: sizes only).
-struct Scratch {
-  uint64_t* keys_in;
-  uint64_t* keys;
-  int* idx_in;
-  int* perm;
-  double* x;
-  double* y;
-  double* z;
-  int* cell_of;
-  uint64_t* ukeys;
-  int* cstart;  // [n + 1]
-  int* ncells;
+// Caller-owned device scratch, carved in a fixed order (base == nullptr: sizes only): the grid's buffers, then DBSCAN's.
+struct Scratch : GridBuffers {
   int* core;
   int* cmin;
   int* parent;
-  int* flag;
   int* cid;
-  void* cub;
-  size_t cub_bytes;
 };
 
 int cub_bytes(int n, size_t* bytes) {
@@ -877,24 +787,6 @@ int check_extent(const char* what, const char* what_len, double len, double h, c
       return FNR_ERR_UNSUPPORTED;
     }
   }
-  return FNR_OK;
-}
-
-// Sorted cell keys, sorted coordinates, cells and their first positions for cell side h and origin lo.
-int build_grid(const double* pts, int n, const double* lo, double h, const Scratch& s, cudaStream_t st, Grid* g) {
-  cell_key_kernel<<<grid_for(n, kThreads, INT_MAX), kThreads, 0, st>>>(pts, n, lo[0], lo[1], lo[2], h, s.keys_in, s.idx_in);
-  if (int rc = check_launch("cell_key_kernel")) return rc;
-  size_t tb = s.cub_bytes;
-  if (int rc = check_cuda(cub::DeviceRadixSort::SortPairs(s.cub, tb, s.keys_in, s.keys, s.idx_in, s.perm, n, 0, 3 * kAxisBits, st),
-                          "cub SortPairs (cell keys)"))
-    return rc;
-  gather_kernel<<<grid_for(n, kThreads, INT_MAX), kThreads, 0, st>>>(pts, n, s.keys, s.perm, s.x, s.y, s.z, s.flag);
-  if (int rc = check_launch("gather_kernel")) return rc;
-  tb = s.cub_bytes;
-  if (int rc = check_cuda(cub::DeviceScan::InclusiveSum(s.cub, tb, s.flag, s.cell_of, n, st), "cub InclusiveSum (cells)")) return rc;
-  cells_kernel<<<grid_for(n, kThreads, INT_MAX), kThreads, 0, st>>>(n, s.keys, s.cell_of, s.ukeys, s.cstart, s.ncells);
-  if (int rc = check_launch("cells_kernel")) return rc;
-  *g = Grid{n, s.keys, s.perm, s.x, s.y, s.z, s.cell_of, s.ukeys, s.cstart, s.ncells};
   return FNR_OK;
 }
 

@@ -112,12 +112,15 @@ MAX_EMPTY_BATCHES = 100  # consecutive batches without a kept ray after which ge
 def generate_point_cloud(pipeline, num_points: int = 1000000, remove_outliers: bool = True, reorient_normals: bool = True,
                          estimate_normals: bool = False, rgb_output_name: str = "rgb", depth_output_name: str = "depth",
                          normal_output_name: Optional[str] = None, use_bounding_box: bool = True,
-                         bounding_box_min=(-1.0, -1.0, -1.0), bounding_box_max=(1.0, 1.0, 1.0), std_ratio: float = 10.0) -> Dict:
+                         bounding_box_min=(-1.0, -1.0, -1.0), bounding_box_max=(1.0, 1.0, 1.0), std_ratio: float = 10.0,
+                         fruit: bool = False) -> Dict:
     """nerfstudio exporter_utils.generate_point_cloud (0.3.2) on the GPU.  Renders training-ray batches until at least
     ``num_points`` rays are kept (the last batch whole), back-projects each ray's median depth, keeps rays with
     accumulation > 0.5 (and, with the box, points strictly inside it), then optionally removes statistical outliers
     (20 neighbours, ``std_ratio``), estimates normals (30 neighbours) and flips them against the view direction.
-    Returns {'points' [N,3], 'colors' [N,3], 'normals' [N,3] or None}, float64 numpy, in the dataparser frame.
+    Returns {'points' [N,3], 'colors' [N,3], 'normals' [N,3] or None}, float64 numpy, in the dataparser frame.  With
+    ``fruit``, also 'fruit' [N] fp32: each kept ray's sigmoid(semantics), in the same order (the Poisson export's per-point
+    fruit probability).
 
     Unlike the reference, which loops forever when no ray survives, this raises RuntimeError after
     ``MAX_EMPTY_BATCHES`` consecutive batches that keep nothing."""
@@ -130,6 +133,7 @@ def generate_point_cloud(pipeline, num_points: int = 1000000, remove_outliers: b
     model, dm = pipeline.model, pipeline.datamanager
     dev = next(model.parameters()).device
     buffers = ops.PointBuffers(max(0, num_points) + dm.config.train_num_rays_per_batch, dev)
+    fbuf = ops.PointBuffers(buffers.capacity, dev) if fruit else None  # same selection, sigmoid(semantics) as its colour
     box = (bounding_box_min, bounding_box_max) if use_bounding_box else None
     count = empty = 0
     with torch.no_grad():
@@ -139,6 +143,9 @@ def generate_point_cloud(pipeline, num_points: int = 1000000, remove_outliers: b
             rgba = model.get_rgba_image(outputs, rgb_output_name)
             ops.backproject_select(ray_bundle.origins, ray_bundle.directions, outputs[depth_output_name], rgba[..., :3], rgba[..., 3],
                                    buffers, box)
+            if fbuf is not None:
+                prob = torch.sigmoid(outputs["semantics"].detach().float().reshape(-1, 1)).expand(-1, 3)
+                ops.backproject_select(ray_bundle.origins, ray_bundle.directions, outputs[depth_output_name], prob, rgba[..., 3], fbuf, box)
             kept = int(buffers.count.item())  # the one host read per batch
             if kept > buffers.capacity:
                 raise RuntimeError(f"point buffer of {buffers.capacity} rows overflowed ({kept}): the ray batch size changed")
@@ -150,16 +157,21 @@ def generate_point_cloud(pipeline, num_points: int = 1000000, remove_outliers: b
         points = buffers.points[:count].double()
         colors = buffers.colors[:count]
         view_dirs = buffers.view_dirs[:count]
+        fruit_prob = fbuf.colors[:count, 0] if fbuf is not None else None
         if remove_outliers:
             points, ind = pointcloud.remove_statistical_outliers(points, 20, std_ratio, return_index=True)
             colors, view_dirs = colors[ind], view_dirs[ind]
+            fruit_prob = fruit_prob[ind] if fruit_prob is not None else None
         normals = None
         if estimate_normals:
             normals = pointcloud.estimate_normals(points, 30, view_dirs if reorient_normals else None)
             if reorient_normals:
                 normals = normals.float().double()  # the reference reorients fp32 normals and stores them back
-    return {"points": points.cpu().numpy(), "colors": colors.double().cpu().numpy(),
-            "normals": None if normals is None else normals.cpu().numpy()}
+    out = {"points": points.cpu().numpy(), "colors": colors.double().cpu().numpy(),
+           "normals": None if normals is None else normals.cpu().numpy()}
+    if fruit_prob is not None:
+        out["fruit"] = fruit_prob.cpu().numpy()
+    return out
 
 
 def write_ply(path,points: np.ndarray, colors: np.ndarray, normals: Optional[np.ndarray] = None) -> None:
@@ -410,6 +422,50 @@ def export_tsdf_mesh(pipeline, output_dir, downscale_factor: int = 2, depth_outp
     write_mesh_ply(paths["mesh"], mesh["vertices"], mesh["normals"], mesh["colors"], mesh["faces"])
     write_mesh_ply(paths["fruit_mesh"], fv, fn, fc, fidx)
     return {"mesh": mesh, "fruit_mesh": fruit_mesh, "aabb": aabb.numpy(), "paths": paths}
+
+
+def export_poisson_mesh(pipeline, output_dir, num_points: int = 1000000, remove_outliers: bool = True, reorient_normals: bool = True,
+                        depth_output_name: str = "depth", rgb_output_name: str = "rgb", save_point_cloud: bool = False,
+                        use_bounding_box: bool = True, bounding_box_min=(-1.0, -1.0, -1.0), bounding_box_max=(1.0, 1.0, 1.0),
+                        std_ratio: float = 10.0, depth: int = 9) -> Dict:
+    """nerfstudio ExportPoissonMesh on the GPU: the surface cloud of ``generate_point_cloud`` with estimated normals and
+    per-point fruit probabilities, a screened Poisson reconstruction at ``depth`` (poisson.reconstruct: dense grid, open3d's
+    scale 1.1 and point weight 2), and the trim of the vertices below the 0.1 quantile of density.
+
+    Writes ``poisson_mesh.ply`` (vertex colours) and ``fruit_poisson_mesh.ply`` (the faces whose three vertices have a fruit
+    probability >= 0.5; possibly empty) in the dataparser frame, and with ``save_point_cloud`` also ``point_cloud.ply``.
+    An empty mesh raises RuntimeError and writes nothing.  Returns {'mesh', 'fruit_mesh': dicts of numpy arrays,
+    'point_cloud', 'iterations', 'residual', 'paths'}."""
+    from .. import mesh as M
+    from .. import poisson
+
+    poisson.check_depth(depth)
+    dev = next(pipeline.model.parameters()).device
+    if dev.type != "cuda":
+        raise RuntimeError("export_poisson_mesh needs the model on a CUDA device: the reconstruction runs as CUDA kernels")
+    pcd = generate_point_cloud(pipeline, num_points=num_points, remove_outliers=remove_outliers, reorient_normals=reorient_normals,
+                               estimate_normals=True, rgb_output_name=rgb_output_name, depth_output_name=depth_output_name,
+                               use_bounding_box=use_bounding_box, bounding_box_min=bounding_box_min, bounding_box_max=bounding_box_max,
+                               std_ratio=std_ratio, fruit=True)
+    if len(pcd["points"]) == 0:
+        raise RuntimeError("the surface cloud is empty: the Poisson reconstruction gave an empty mesh")
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)  # noqa: E731
+    r = poisson.reconstruct(t(pcd["points"]), t(pcd["normals"]).float(), t(pcd["colors"]).float(), t(pcd["fruit"]).float(), depth=depth)
+    mesh = r["mesh"]
+    if mesh["faces"].shape[0] == 0:
+        raise RuntimeError(f"the Poisson reconstruction of {len(pcd['points'])} points gave an empty mesh")
+    fv, fn, fc, ff, fidx = M.fruit_submesh(mesh["vertices"], mesh["normals"], mesh["colors"], mesh["fruit"], mesh["faces"])
+    fruit_mesh = {"vertices": fv, "normals": fn, "colors": fc, "fruit": ff, "faces": fidx}
+    out_dir = pathlib.Path(output_dir)
+    out_dir.mkdir(parents=True, exist_ok=True)
+    paths = {"mesh": str(out_dir / "poisson_mesh.ply"), "fruit_mesh": str(out_dir / "fruit_poisson_mesh.ply")}
+    if save_point_cloud:
+        paths["point_cloud"] = str(out_dir / "point_cloud.ply")
+        write_ply(paths["point_cloud"], pcd["points"], pcd["colors"], normals=pcd["normals"])
+    write_mesh_ply(paths["mesh"], mesh["vertices"], mesh["normals"], mesh["colors"], mesh["faces"])
+    write_mesh_ply(paths["fruit_mesh"], fv, fn, fc, fidx)
+    return {"mesh": mesh, "fruit_mesh": fruit_mesh, "point_cloud": pcd, "iterations": r["iterations"], "residual": r["residual"],
+            "paths": paths}
 
 
 _FACE_DTYPE = np.dtype([("n", "u1"), ("v", "<i4", (3,))])  # packed: 13 bytes per face

@@ -1002,3 +1002,94 @@ def marching_cubes(values: Tensor, origin, voxel_size, colors: Optional[Tensor] 
                                         _ptr(scratch), nbytes.value, V, F, _ptr(out["vertices"]), _ptr(out["normals"]), _ptr(out["colors"]),
                                         _ptr(out["fruit"]), _ptr(out["faces"]), _stream(dev)))
     return out
+
+
+# ======================================================================================================
+# Screened Poisson reconstruction (fnr_poisson.cu; nerfstudio ns-export poisson)
+# ======================================================================================================
+def _poisson_inputs(points: Tensor, normals: Tensor, colors: Optional[Tensor], fruit: Optional[Tensor]):
+    dev = _require_cuda(points, normals, colors, fruit)
+    pts = points.detach().to(torch.float64).reshape(-1, 3).contiguous()
+    n = int(pts.shape[0])
+    if n < 1:
+        raise ValueError("the Poisson reconstruction needs at least one point")
+    nrm = _f32c(normals.detach().reshape(n, 3))
+    col = None if colors is None else _f32c(colors.detach().reshape(n, 3))
+    fr = None if fruit is None else _f32c(fruit.detach().reshape(n))
+    return dev, pts, n, nrm, col, fr
+
+
+def _cube(origin, side: float):
+    o = (C.c_double * 3)(*[float(v) for v in np.asarray(origin, np.float64).reshape(3)])
+    return o, float(side)
+
+
+def _poisson_scratch(n: int, depth: int, dev) -> Tuple[Tensor, int]:
+    nbytes = C.c_size_t(0)
+    L.check(L.load().fnr_poisson_scratch_bytes(n, int(depth), C.byref(nbytes)))
+    return torch.empty(nbytes.value, dtype=torch.uint8, device=dev), nbytes.value
+
+
+def poisson_splat(points: Tensor, normals: Tensor, depth: int, origin, side: float, colors: Optional[Tensor] = None,
+                  fruit: Optional[Tensor] = None, scratch: Optional[Tuple[Tensor, int]] = None) -> dict:
+    """The node sums and right-hand side of the screened Poisson system (fnr_poisson_splat) on the cube ``origin`` / ``side``
+    at ``depth``: {'density' [M], 'normal_field' [M,3], 'colors' [M,3] or None, 'fruit' [M] or None, 'rhs' [M]} fp32 with
+    M = (2^depth + 1)^3 in C order, and 'scratch' (the sorted points, which ``poisson_apply`` reads)."""
+    dev, pts, n, nrm, col, fr = _poisson_inputs(points, normals, colors, fruit)
+    M = (2 ** int(depth) + 1) ** 3
+    buf, nbytes = scratch if scratch is not None else _poisson_scratch(n, depth, dev)
+    f32 = dict(dtype=torch.float32, device=dev)
+    out = {"density": torch.empty(M, **f32), "normal_field": torch.empty((M, 3), **f32),
+           "colors": None if col is None else torch.empty((M, 3), **f32), "fruit": None if fr is None else torch.empty(M, **f32),
+           "rhs": torch.empty(M, **f32)}
+    o, s = _cube(origin, side)
+    L.check(L.load().fnr_poisson_splat(_ptr(pts), _ptr(nrm), _ptr(col), _ptr(fr), n, int(depth), o, s, _ptr(buf), nbytes, _ptr(out["density"]),
+                                       _ptr(out["normal_field"]), _ptr(out["colors"]), _ptr(out["fruit"]), _ptr(out["rhs"]), _stream(dev)))
+    out["scratch"] = (buf, nbytes)
+    return out
+
+
+def poisson_apply(x: Tensor, num_points: int, depth: int, scratch: Tuple[Tensor, int], alpha: float = 2.0) -> Tensor:
+    """y = (K + alpha a S^T S) x (fnr_poisson_apply) for the points ``poisson_splat`` left in ``scratch``."""
+    dev = _require_cuda(x)
+    M = (2 ** int(depth) + 1) ** 3
+    x = _f32c(x.detach().reshape(-1))
+    if x.numel() != M:
+        raise ValueError(f"x must have (2^depth + 1)^3 = {M} entries, got {x.numel()}")
+    y = torch.empty_like(x)
+    buf, nbytes = scratch
+    L.check(L.load().fnr_poisson_apply(int(num_points), int(depth), float(alpha), _ptr(buf), nbytes, _ptr(x), _ptr(y), _stream(dev)))
+    return y
+
+
+def poisson_solve(points: Tensor, normals: Tensor, depth: int, origin, side: float, colors: Optional[Tensor] = None,
+                  fruit: Optional[Tensor] = None, alpha: float = 2.0, max_iters: int = 2000, tolerance: float = 1e-5) -> dict:
+    """Coarse-to-fine solve of the screened Poisson system (fnr_poisson_solve): {'chi' [M], 'density' [M], 'colors' [M,3]
+    or None, 'fruit' [M] or None, 'iterations' (finest level), 'total_iterations', 'residual' (|r| / |b|)}."""
+    dev, pts, n, nrm, col, fr = _poisson_inputs(points, normals, colors, fruit)
+    M = (2 ** int(depth) + 1) ** 3
+    buf, nbytes = _poisson_scratch(n, depth, dev)
+    f32 = dict(dtype=torch.float32, device=dev)
+    out = {"chi": torch.empty(M, **f32), "density": torch.empty(M, **f32), "colors": None if col is None else torch.empty((M, 3), **f32),
+           "fruit": None if fr is None else torch.empty(M, **f32)}
+    iters = (C.c_int64 * 2)()
+    res = C.c_double(0.0)
+    o, s = _cube(origin, side)
+    L.check(L.load().fnr_poisson_solve(_ptr(pts), _ptr(nrm), _ptr(col), _ptr(fr), n, int(depth), o, s, float(alpha), int(max_iters),
+                                       float(tolerance), _ptr(buf), nbytes, _ptr(out["chi"]), _ptr(out["density"]), _ptr(out["colors"]),
+                                       _ptr(out["fruit"]), iters, C.byref(res), _stream(dev)))
+    out.update(iterations=int(iters[0]), total_iterations=int(iters[1]), residual=float(res.value))
+    return out
+
+
+def poisson_sample(points: Tensor, grid: Tensor, depth: int, origin, side: float) -> Tensor:
+    """Trilinear samples [n] fp32 of a node grid [M] at the points (fnr_poisson_sample)."""
+    dev = _require_cuda(points, grid)
+    pts = points.detach().to(torch.float64).reshape(-1, 3).contiguous()
+    grid = _f32c(grid.detach().reshape(-1))
+    if grid.numel() != (2 ** int(depth) + 1) ** 3:
+        raise ValueError("grid must have (2^depth + 1)^3 entries")
+    out = torch.empty(pts.shape[0], dtype=torch.float32, device=dev)
+    o, s = _cube(origin, side)
+    L.check(L.load().fnr_poisson_sample(_ptr(pts), int(pts.shape[0]), int(depth), o, s, _ptr(grid), _ptr(out), _stream(dev)))
+    return out

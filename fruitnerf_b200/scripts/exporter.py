@@ -17,7 +17,7 @@ from typing import Optional, Tuple
 
 import torch
 
-from ..export.exporter_utils import export_tsdf_mesh, generate_point_cloud, sample_volume, write_ply
+from ..export.exporter_utils import export_poisson_mesh, export_tsdf_mesh, generate_point_cloud, sample_volume, write_ply
 
 
 def eval_setup(config_path, eval_num_rays_per_chunk: Optional[int] = None, test_mode: str = "test", device: Optional[str] = None):
@@ -189,6 +189,65 @@ class ExportTSDFMesh(Exporter):
                                 refinement_epsilon=self.refinement_epsilon)
 
 
+@dataclass
+class ExportPoissonMesh(Exporter):
+    """nerfstudio 0.3.2 ExportPoissonMesh: a watertight mesh of the scene by screened Poisson reconstruction of the surface
+    cloud, trimmed at the 0.1 quantile of vertex density, plus the mesh of the fruit surfaces (faces whose vertices have a
+    fruit probability >= 0.5).  Single GPU.  Only vertex colours (``texture_method="point_cloud"``) are implemented: NeRF
+    texturing needs an xatlas UV unwrap.  ``depth`` (open3d's octree depth, here the dense grid's 2^depth cells per
+    axis) is the one option upstream does not have."""
+
+    num_points: int = 1000000
+    remove_outliers: bool = True
+    reorient_normals: bool = True
+    depth_output_name: str = "depth"
+    rgb_output_name: str = "rgb"
+    normal_method: str = "model_output"
+    """"open3d": estimate normals from the cloud; "model_output": take them from the model, which FruitModel cannot."""
+    normal_output_name: str = "normals"
+    save_point_cloud: bool = False
+    use_bounding_box: bool = True
+    bounding_box_min: Tuple[float, float, float] = (-1, -1, -1)
+    bounding_box_max: Tuple[float, float, float] = (1, 1, 1)
+    num_rays_per_batch: int = 32768
+    texture_method: str = "point_cloud"
+    std_ratio: float = 10.0
+    depth: int = 9
+
+    def validate(self) -> None:
+        """Refuse what cannot run, before anything is loaded."""
+        from .. import poisson
+
+        if self.texture_method == "nerf":
+            raise ValueError("texture_method 'nerf' needs an xatlas UV unwrap, which is not available; use 'point_cloud' (vertex colours)")
+        if self.texture_method != "point_cloud":
+            raise ValueError(f"texture_method must be 'point_cloud' or 'nerf', got {self.texture_method!r}")
+        if self.normal_method not in ("open3d", "model_output"):
+            raise ValueError(f"normal_method must be 'open3d' or 'model_output', got {self.normal_method!r}")
+        poisson.check_depth(self.depth)
+        if self.num_points < 1:
+            raise ValueError(f"num_points must be >= 1, got {self.num_points}")
+        if self.use_bounding_box and not all(lo < hi for lo, hi in zip(self.bounding_box_min, self.bounding_box_max)):
+            raise ValueError("Bounding box min must be smaller than max")
+
+    def main(self, pipeline=None) -> dict:
+        """Writes ``output_dir/poisson_mesh.ply`` and ``output_dir/fruit_poisson_mesh.ply``; returns export_poisson_mesh's
+        dict.  Exits with status 1 for ``normal_method="model_output"`` when the model renders no ``normal_output_name``."""
+        self.validate()
+        if pipeline is None:
+            if self.load_config is None:
+                raise ValueError("pass load_config (a run folder's config.yml) or an already built pipeline")
+            _, pipeline, _, _ = eval_setup(self.load_config)
+        if self.normal_method == "model_output":
+            _require_normal_output(pipeline, self.normal_output_name)
+        pipeline.datamanager.config.train_num_rays_per_batch = self.num_rays_per_batch
+        return export_poisson_mesh(pipeline, Path(self.output_dir), num_points=self.num_points, remove_outliers=self.remove_outliers,
+                                   reorient_normals=self.reorient_normals, depth_output_name=self.depth_output_name,
+                                   rgb_output_name=self.rgb_output_name, save_point_cloud=self.save_point_cloud,
+                                   use_bounding_box=self.use_bounding_box, bounding_box_min=self.bounding_box_min,
+                                   bounding_box_max=self.bounding_box_max, std_ratio=self.std_ratio, depth=self.depth)
+
+
 def _require_normal_output(pipeline, normal_output_name: str) -> None:
     """nerfstudio validate_pipeline: render one ray and exit(1) if ``normal_output_name`` is not among the outputs."""
     from ..compat import RayBundle
@@ -254,6 +313,59 @@ def add_tsdf_parser(sub) -> argparse.ArgumentParser:
     return p
 
 
+def add_poisson_parser(sub) -> argparse.ArgumentParser:
+    """The ``poisson`` subcommand: ExportPoissonMesh's fields as nerfstudio's option names, same defaults (texture method
+    ``point_cloud``, the only one implemented), plus ``--depth``."""
+    d = ExportPoissonMesh(load_config=None, output_dir=Path("."))
+    p = sub.add_parser("poisson", help="watertight meshes of the scene and of the fruit by screened Poisson reconstruction")
+    p.add_argument("--load-config", type=Path, required=True)
+    p.add_argument("--output-dir", type=Path, required=True)
+    p.add_argument("--num-points", type=int, default=d.num_points)
+    p.add_argument("--remove-outliers", type=_flag, default=d.remove_outliers)
+    p.add_argument("--reorient-normals", type=_flag, default=d.reorient_normals)
+    p.add_argument("--depth-output-name", default=d.depth_output_name)
+    p.add_argument("--rgb-output-name", default=d.rgb_output_name)
+    p.add_argument("--normal-method", choices=("open3d", "model_output"), default=d.normal_method)
+    p.add_argument("--normal-output-name", default=d.normal_output_name)
+    p.add_argument("--save-point-cloud", type=_flag, default=d.save_point_cloud)
+    p.add_argument("--use-bounding-box", type=_flag, default=d.use_bounding_box)
+    p.add_argument("--bounding-box-min", type=float, nargs=3, default=d.bounding_box_min)
+    p.add_argument("--bounding-box-max", type=float, nargs=3, default=d.bounding_box_max)
+    p.add_argument("--num-rays-per-batch", type=int, default=d.num_rays_per_batch)
+    p.add_argument("--texture-method", choices=("point_cloud", "nerf"), default=d.texture_method)
+    p.add_argument("--std-ratio", type=float, default=d.std_ratio)
+    p.add_argument("--depth", type=int, default=d.depth)
+    return p
+
+
+def poisson_exporter_from_args(a) -> ExportPoissonMesh:
+    return ExportPoissonMesh(load_config=a.load_config, output_dir=a.output_dir, num_points=a.num_points, remove_outliers=a.remove_outliers,
+                             reorient_normals=a.reorient_normals, depth_output_name=a.depth_output_name, rgb_output_name=a.rgb_output_name,
+                             normal_method=a.normal_method, normal_output_name=a.normal_output_name, save_point_cloud=a.save_point_cloud,
+                             use_bounding_box=a.use_bounding_box, bounding_box_min=tuple(a.bounding_box_min),
+                             bounding_box_max=tuple(a.bounding_box_max), num_rays_per_batch=a.num_rays_per_batch,
+                             texture_method=a.texture_method, std_ratio=a.std_ratio, depth=a.depth)
+
+
+def _run_mesh_export(exp, parser):
+    """validate (argparse error, status 2), run, exit 1 on an empty mesh, print the two meshes."""
+    try:
+        exp.validate()
+    except ValueError as e:
+        parser.error(str(e))
+    try:
+        res = exp.main()
+    except RuntimeError as e:
+        if "empty mesh" not in str(e):
+            raise
+        print(f"error: {e}", file=sys.stderr)
+        sys.exit(1)
+    for key in ("mesh", "fruit_mesh"):
+        m = res[key]
+        print(f"{key}: {m['vertices'].shape[0]} vertices, {m['faces'].shape[0]} faces -> {res['paths'][key]}")
+    return res
+
+
 def tsdf_exporter_from_args(a) -> ExportTSDFMesh:
     return ExportTSDFMesh(load_config=a.load_config, output_dir=a.output_dir, downscale_factor=a.downscale_factor,
                           depth_output_name=a.depth_output_name, rgb_output_name=a.rgb_output_name, resolution=tuple(a.resolution),
@@ -266,12 +378,13 @@ def tsdf_exporter_from_args(a) -> ExportTSDFMesh:
 def entrypoint(argv=None):
     """``ns-export-semantics semantic-pointcloud --load-config RUN/config.yml --output-dir OUT [...]`` (exporter.py:124-144;
     upstream parses the same dataclass with tyro, which is not available offline -- argparse with the same option names)
-    , ``ns-export-semantics pointcloud ...`` (nerfstudio ExportPointCloud) and ``ns-export-semantics tsdf ...`` (nerfstudio
-    ExportTSDFMesh)."""
+    , ``ns-export-semantics pointcloud ...`` (nerfstudio ExportPointCloud), ``ns-export-semantics tsdf ...`` (nerfstudio
+    ExportTSDFMesh) and ``ns-export-semantics poisson ...`` (nerfstudio ExportPoissonMesh)."""
     ap = argparse.ArgumentParser(prog="ns-export-semantics")
     sub = ap.add_subparsers(dest="command", required=True)
     add_pointcloud_parser(sub)
     tsdf_parser = add_tsdf_parser(sub)
+    poisson_parser = add_poisson_parser(sub)
     p = sub.add_parser("semantic-pointcloud", help="uniform-volume export of the fruit point clouds")
     p.add_argument("--load-config", type=Path, required=True)
     p.add_argument("--output-dir", type=Path, required=True)
@@ -282,23 +395,10 @@ def entrypoint(argv=None):
     p.add_argument("--num-points-per-side", type=int, default=1000)
     p.add_argument("--stratified-jitter", type=lambda s: s.lower() in ("1", "true", "yes"), default=True)
     a = ap.parse_args(argv)
+    if a.command == "poisson":
+        return _run_mesh_export(poisson_exporter_from_args(a), poisson_parser)
     if a.command == "tsdf":
-        exp = tsdf_exporter_from_args(a)
-        try:
-            exp.validate()
-        except ValueError as e:
-            tsdf_parser.error(str(e))
-        try:
-            res = exp.main()
-        except RuntimeError as e:
-            if "empty mesh" not in str(e):
-                raise
-            print(f"error: {e}", file=sys.stderr)
-            sys.exit(1)
-        for key in ("mesh", "fruit_mesh"):
-            m = res[key]
-            print(f"{key}: {m['vertices'].shape[0]} vertices, {m['faces'].shape[0]} faces -> {res['paths'][key]}")
-        return res
+        return _run_mesh_export(tsdf_exporter_from_args(a), tsdf_parser)
     if a.command == "pointcloud":
         exp = ExportPointCloud(load_config=a.load_config, output_dir=a.output_dir, num_points=a.num_points, remove_outliers=a.remove_outliers,
                                reorient_normals=a.reorient_normals, normal_method=a.normal_method, normal_output_name=a.normal_output_name,

@@ -56,6 +56,9 @@
  *   fnr_tsdf_integrate, fnr_marching_cubes_scratch_bytes, fnr_marching_cubes_count, fnr_marching_cubes_emit
  *                        the `tsdf` mesh export (nerfstudio ns-export tsdf: TSDF.integrate_tsdf, skimage
  *                        marching_cubes): fusion of rendered depth maps and the scene / fruit surface meshes
+ *   fnr_poisson_scratch_bytes, fnr_poisson_splat, fnr_poisson_apply, fnr_poisson_solve, fnr_poisson_sample
+ *                        the `poisson` mesh export (nerfstudio ns-export poisson: open3d
+ *                        create_from_point_cloud_poisson): screened Poisson reconstruction of the surface cloud
  */
 #ifndef FRUITNERF_B200_H
 #define FRUITNERF_B200_H
@@ -566,6 +569,38 @@ int fnr_marching_cubes_count(const float* values, int64_t nx, int64_t ny, int64_
 int fnr_marching_cubes_emit(const float* values, const float* colors, const float* fruit, int64_t nx, int64_t ny, int64_t nz, const float* origin,
                             const float* voxel_size, const void* scratch, size_t scratch_bytes, int64_t num_vertices, int64_t num_faces,
                             float* vertices, float* normals, float* vertex_colors, float* vertex_fruit, int64_t* faces, void* stream);
+
+/* ---- Screened Poisson reconstruction (`ns-export-semantics poisson`, nerfstudio ns-export poisson; fnr_poisson.cu) ----
+ * points: DEVICE [n,3] fp64, 1 <= n <= 2^31 - 1; normals [n,3], colors [n,3] (or NULL), fruit [n] (or NULL): DEVICE fp32.
+ * The cube (origin: HOST double[3], side) carries R = 2^depth cells per axis, 2 <= depth <= 10, and (R+1)^3 nodes in C
+ * order; node (i,j,k) lies at origin + (i,j,k) * side / R.  Every point must be finite and lie in a cell,
+ * 0 <= floor((p - origin) / (side / R)) < R per axis (FNR_ERR_INVALID_ARGUMENT otherwise: one host read).  Node sums
+ * gather over the points of the node's 8 adjacent cells, in cell order and then input order, in fp64 rounded to fp32
+ * once (no atomics: repeated calls give identical bits).  DEVICE scratch: fnr_poisson_scratch_bytes(n, depth).
+ *
+ * fnr_poisson_splat writes density [M] = sum phi, normal_field [M,3] = (a / h^3) sum phi n with h = 1/R and
+ * a = h^2 * (occupied cells) / n, node_colors [M,3] / node_fruit [M] = sum phi c / density (0 where density is 0; NULL
+ * exactly when colors / fruit is) and rhs [M] = sum_j (int grad phi_i phi_j) . v_j.  It leaves the sorted points in
+ * scratch, which fnr_poisson_apply reads: y = (K + alpha a S^T S) x for x [M], with K the Q1 stiffness matrix of the
+ * cells inside the cube (Neumann boundaries) and S [n, M] the trilinear point samples.
+ * fnr_poisson_solve splats at every depth from max(depth - 3, 4) to depth (depth alone when depth <= 4) and solves each
+ * level by Jacobi-preconditioned conjugate gradient in fp32 (fp64 block dot products), starting from the previous
+ * level's chi prolonged trilinearly, until |r| <= tolerance |b| or max_iters iterations.  chi [M]; density,
+ * node_colors, node_fruit as fnr_poisson_splat's at the finest depth; HOST iterations[2] = {finest level, all levels};
+ * HOST residual = |r| / |b| at the finest level.
+ * fnr_poisson_sample writes out [n] fp32, the trilinear sample of a node grid [M] at each point (clamped to the border
+ * cells). */
+int fnr_poisson_scratch_bytes(int64_t num_points, int32_t depth, size_t* bytes);
+int fnr_poisson_splat(const double* points, const float* normals, const float* colors, const float* fruit, int64_t num_points, int32_t depth,
+                      const double* origin, double side, void* scratch, size_t scratch_bytes, float* density, float* normal_field,
+                      float* node_colors, float* node_fruit, float* rhs, void* stream);
+int fnr_poisson_apply(int64_t num_points, int32_t depth, float alpha, const void* scratch, size_t scratch_bytes, const float* x, float* y,
+                      void* stream);
+int fnr_poisson_solve(const double* points, const float* normals, const float* colors, const float* fruit, int64_t num_points, int32_t depth,
+                      const double* origin, double side, float alpha, int32_t max_iters, float tolerance, void* scratch, size_t scratch_bytes,
+                      float* chi, float* density, float* node_colors, float* node_fruit, int64_t* iterations, double* residual, void* stream);
+int fnr_poisson_sample(const double* points, int64_t num_points, int32_t depth, const double* origin, double side, const float* grid, float* out,
+                       void* stream);
 
 /* Hash-grid row indices (exact-integer parity hook): rows[N,L,8] in nerfstudio corner order for
  * the masked [0,1]^3 positions of the given samples; also writes positions[N,3] if non-NULL. */
