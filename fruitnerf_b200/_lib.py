@@ -182,6 +182,7 @@ FNR_MAX_FRAME_OUTPUTS = 8
 FNR_COMPOSE_SCRATCH_FLOATS = FNR_MAX_FRAME_OUTPUTS * 256 * 2
 
 FNR_OPT_ADAM, FNR_OPT_RADAM = 0, 1
+FNR_MESH_ASSIGN_SCRATCH_BYTES = 256
 FNR_MAX_ADAM_TENSORS = 48
 
 LIB_PATH = Path(__file__).resolve().parent / "csrc" / "libfruitnerf_b200.so"
@@ -231,6 +232,10 @@ EXPORTED_SYMBOLS = (
     "fnr_poisson_apply",
     "fnr_poisson_solve",
     "fnr_poisson_sample",
+    "fnr_mesh_measure_scratch_bytes",
+    "fnr_mesh_components",
+    "fnr_mesh_assign_centers",
+    "fnr_mesh_measure_groups",
 )
 
 _lib = None
@@ -347,6 +352,14 @@ def load() -> C.CDLL:
     lib.fnr_poisson_solve.argtypes = [vp, vp, vp, vp, i64, i32, f64p, f64, f32, i32, f32, vp, sz, vp, vp, vp, vp, _i64p, f64p, vp]
     lib.fnr_poisson_sample.restype = C.c_int
     lib.fnr_poisson_sample.argtypes = [vp, i64, i32, f64p, f64, vp, vp, vp]
+    lib.fnr_mesh_measure_scratch_bytes.restype = C.c_int
+    lib.fnr_mesh_measure_scratch_bytes.argtypes = [i64, i64, C.POINTER(C.c_size_t)]
+    lib.fnr_mesh_components.restype = C.c_int
+    lib.fnr_mesh_components.argtypes = [vp, i64, i64, vp, sz, vp, _i64p, vp]
+    lib.fnr_mesh_assign_centers.restype = C.c_int
+    lib.fnr_mesh_assign_centers.argtypes = [vp, vp, i64, i64, vp, i64, f64, vp, sz, vp, vp]
+    lib.fnr_mesh_measure_groups.restype = C.c_int
+    lib.fnr_mesh_measure_groups.argtypes = [vp, vp, i64, i64, vp, i64, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     if lib.fnr_version() != ABI_VERSION:
         raise FruitNerfNativeError(f"ABI version mismatch: library reports {lib.fnr_version()}")
     _lib = lib

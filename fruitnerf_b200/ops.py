@@ -1093,3 +1093,71 @@ def poisson_sample(points: Tensor, grid: Tensor, depth: int, origin, side: float
     o, s = _cube(origin, side)
     L.check(L.load().fnr_poisson_sample(_ptr(pts), int(pts.shape[0]), int(depth), o, s, _ptr(grid), _ptr(out), _stream(dev)))
     return out
+
+
+# ======================================================================================================
+# Per-fruit measurement of triangle meshes (fnr_measure.cu)
+# ======================================================================================================
+def _mesh_inputs(vertices: Optional[Tensor], faces: Tensor):
+    """(device, vertices [V,3] fp64 or None, faces [F,3] int64), contiguous."""
+    dev = _require_cuda(vertices, faces)
+    v = None if vertices is None else vertices.detach().to(torch.float64).reshape(-1, 3).contiguous()
+    f = faces.detach().to(torch.int64).reshape(-1, 3).contiguous()
+    return dev, v, f
+
+
+def _measure_scratch(num_vertices: int, num_faces: int, dev) -> Tuple[Tensor, int]:
+    nbytes = C.c_size_t(0)
+    L.check(L.load().fnr_mesh_measure_scratch_bytes(int(num_vertices), int(num_faces), C.byref(nbytes)))
+    return torch.empty(nbytes.value, dtype=torch.uint8, device=dev), nbytes.value
+
+
+def mesh_components(faces: Tensor, num_vertices: int) -> Tuple[Tensor, int]:
+    """(int32 [F] labels, number of groups): the connected components of the faces through shared vertex indices
+    (fnr_mesh_components), numbered in the order of their smallest vertex index."""
+    dev, _, f = _mesh_inputs(None, faces)
+    F = int(f.shape[0])
+    labels = torch.empty(F, dtype=torch.int32, device=dev)
+    buf, nbytes = _measure_scratch(num_vertices, F, dev)
+    num = C.c_int64(0)
+    L.check(L.load().fnr_mesh_components(_ptr(f), F, int(num_vertices), _ptr(buf), nbytes, _ptr(labels), C.byref(num), _stream(dev)))
+    return labels, int(num.value)
+
+
+def mesh_assign_centers(vertices: Tensor, faces: Tensor, centers: Tensor, max_distance: float = float("inf")) -> Tensor:
+    """int32 [F]: the index of the centre [K,3] nearest each face centroid, -1 beyond ``max_distance``
+    (fnr_mesh_assign_centers)."""
+    dev, v, f = _mesh_inputs(vertices, faces)
+    _require_cuda(centers)
+    c = centers.detach().to(torch.float64).reshape(-1, 3).contiguous()
+    F = int(f.shape[0])
+    labels = torch.empty(F, dtype=torch.int32, device=dev)
+    flag = torch.empty(L.FNR_MESH_ASSIGN_SCRATCH_BYTES, dtype=torch.uint8, device=dev)
+    L.check(L.load().fnr_mesh_assign_centers(_ptr(v), _ptr(f), F, int(v.shape[0]), _ptr(c), int(c.shape[0]), float(max_distance), _ptr(flag),
+                                             flag.numel(), _ptr(labels), _stream(dev)))
+    return labels
+
+
+def mesh_measure_groups(vertices: Tensor, faces: Tensor, face_group: Tensor, num_groups: int) -> Dict[str, Tensor]:
+    """Per-group measurements of the labels 0..G-1 (fnr_mesh_measure_groups), device tensors: 'faces', 'boundary_edges',
+    'nonmanifold_edges' [G] int64, 'area' [G], 'centroid' [G,3], 'sphere' [G,5] (centre, radius, rms), 'volume' [G],
+    'coverage' [G] fp64, 'fit_ok' [G] int32, and 'unassigned_faces' / 'unassigned_area' [1] for the label -1 faces."""
+    dev, v, f = _mesh_inputs(vertices, faces)
+    _require_cuda(face_group)
+    g = face_group.detach().to(torch.int32).reshape(-1).contiguous()
+    V, F, G = int(v.shape[0]), int(f.shape[0]), int(num_groups)
+    if g.shape[0] != F:
+        raise ValueError(f"{g.shape[0]} face labels for {F} faces")
+    buf, nbytes = _measure_scratch(V, F, dev)
+    i64 = dict(dtype=torch.int64, device=dev)
+    f64 = dict(dtype=torch.float64, device=dev)
+    G0 = max(G, 0)
+    out = {"faces": torch.empty(G0, **i64), "boundary_edges": torch.empty(G0, **i64), "nonmanifold_edges": torch.empty(G0, **i64),
+           "area": torch.empty(G0, **f64), "centroid": torch.empty((G0, 3), **f64), "sphere": torch.empty((G0, 5), **f64),
+           "volume": torch.empty(G0, **f64), "coverage": torch.empty(G0, **f64), "fit_ok": torch.empty(G0, dtype=torch.int32, device=dev),
+           "unassigned_faces": torch.empty(1, **i64), "unassigned_area": torch.empty(1, **f64)}
+    p = lambda k: _ptr(out[k]) if G0 else None  # noqa: E731
+    L.check(L.load().fnr_mesh_measure_groups(_ptr(v), _ptr(f), F, V, _ptr(g), G, _ptr(buf), nbytes, p("faces"), p("boundary_edges"),
+                                             p("nonmanifold_edges"), p("area"), p("centroid"), p("sphere"), p("volume"), p("coverage"),
+                                             p("fit_ok"), _ptr(out["unassigned_faces"]), _ptr(out["unassigned_area"]), _stream(dev)))
+    return out

@@ -189,3 +189,28 @@ def touching_fruit_cloud(seed: int = 0, singles: int = 3, pairs: int = 3, triple
             shells.append(shell(c, fruit_radius, points_per_fruit))
     pts = np.concatenate(shells)
     return pts[rng.permutation(pts.shape[0])], np.array(centres)
+
+
+def sphere_lattice(dev, n=(13, 10, 10), cell=48, seed=0):
+    """Marching cubes (on the device) of spheres in a lattice of cubic cells of `cell` voxels, one per cell, radii 17..22
+    voxels and centres within half a voxel of the cell's centre, so that no sphere reaches its cell's wall:
+    (vertices fp64, faces, centres [K,3] in cell order, radii [K])."""
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    K = n[0] * n[1] * n[2]
+    radii = 17.0 + 5.0 * torch.rand(K, generator=g, dtype=torch.float64)
+    offs = (torch.rand(K, 3, generator=g, dtype=torch.float64) - 0.5)
+    dims = [a * cell for a in n]
+    ax = [torch.arange(d, device=dev, dtype=torch.float32) for d in dims]
+    cid = [(a // cell).long() for a in ax]
+    k = (cid[0][:, None, None] * n[1] + cid[1][None, :, None]) * n[2] + cid[2][None, None, :]
+    cen = torch.stack(torch.meshgrid(*(torch.arange(a, dtype=torch.float64) for a in n), indexing="ij"), -1).reshape(-1, 3) * cell + cell / 2 + offs
+    cd, rd = cen.to(dev).float(), radii.to(dev).float()
+    X, Y, Z = ax[0][:, None, None], ax[1][None, :, None], ax[2][None, None, :]
+    values = torch.sqrt((X - cd[k, 0]) ** 2 + (Y - cd[k, 1]) ** 2 + (Z - cd[k, 2]) ** 2) - rd[k]
+    del k
+    from .mesh import marching_cubes
+
+    m = marching_cubes(values.contiguous(), (0.0, 0.0, 0.0), 1.0)
+    del values
+    torch.cuda.empty_cache()
+    return m["vertices"].double(), m["faces"], cen, radii

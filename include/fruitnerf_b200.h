@@ -59,6 +59,9 @@
  *   fnr_poisson_scratch_bytes, fnr_poisson_splat, fnr_poisson_apply, fnr_poisson_solve, fnr_poisson_sample
  *                        the `poisson` mesh export (nerfstudio ns-export poisson: open3d
  *                        create_from_point_cloud_poisson): screened Poisson reconstruction of the surface cloud
+ *   fnr_mesh_measure_scratch_bytes, fnr_mesh_components, fnr_mesh_assign_centers, fnr_mesh_measure_groups
+ *                        per-fruit measurement of the fruit meshes (no reference counterpart): grouping by connected
+ *                        components or nearest count centre, area, sphere fit, volume, solid-angle coverage, edges
  */
 #ifndef FRUITNERF_B200_H
 #define FRUITNERF_B200_H
@@ -601,6 +604,41 @@ int fnr_poisson_solve(const double* points, const float* normals, const float* c
                       float* chi, float* density, float* node_colors, float* node_fruit, int64_t* iterations, double* residual, void* stream);
 int fnr_poisson_sample(const double* points, int64_t num_points, int32_t depth, const double* origin, double side, const float* grid, float* out,
                        void* stream);
+
+/* ---- Per-fruit measurement of triangle meshes (fnr_measure.cu; DESIGN section 4.3n) ----
+ * vertices: DEVICE [V,3] fp64; faces: DEVICE [F,3] int64, every index in [0, V) (FNR_ERR_INVALID_ARGUMENT otherwise: a
+ * device check and one host read); face_group: DEVICE [F] int32, a group id or -1 (unassigned).  V <= 2^31 - 1 and
+ * F <= (2^31 - 1) / 3, else FNR_ERR_UNSUPPORTED; negative counts and NULL inputs return FNR_ERR_INVALID_ARGUMENT.
+ * DEVICE scratch of fnr_mesh_components and fnr_mesh_measure_groups: fnr_mesh_measure_scratch_bytes(V, F).
+ *
+ * fnr_mesh_components labels each face with its connected component (faces connected when they share a vertex index;
+ * vertices no face uses are ignored), components numbered in the order of their smallest vertex index, and writes the
+ * count to HOST *num_groups (one host read).
+ * fnr_mesh_assign_centers labels each face with the index of the centre (DEVICE [K,3] fp64, all finite) nearest its
+ * centroid (v0 + v1 + v2) / 3 in fp64 squared distance ((dx^2 + dy^2) + dz^2, no FMA; ties to the lower index), or -1
+ * when that distance exceeds max_distance (> 0; may be infinite).  Its DEVICE scratch is FNR_MESH_ASSIGN_SCRATCH_BYTES
+ * (the flag of the check of the face indices and the centres, one host read).
+ * fnr_mesh_measure_groups measures the groups 0..G-1 (labels outside [-1, G) are refused).  Per group: group_faces,
+ * boundary_edges, nonmanifold_edges [G] int64 (per edge key (min, max) vertex id and group: one half-edge of the group is
+ * a boundary edge, three or more a non-manifold edge); area [G] = sum |e1 x e2| / 2; centroid [G,3] area-weighted (the
+ * plain mean of the face centroids when the area is 0); sphere [G,5] = centre xyz, radius and area-weighted RMS of
+ * |p_f - centre| - radius over the face centroids p_f, from the area-weighted algebraic (Kasa) fit about the centroid;
+ * fit_ok [G] int32 (0: singular system or d + |x|^2 <= 0, centre = centroid, radius = the area-weighted RMS distance of
+ * the face centroids from it); volume [G] = sum det(v0 - c, v1 - c, v2 - c) / 6 and coverage [G] = (sum of the signed
+ * solid angles, Van Oosterom-Strackee) / 4 pi, about c = the sphere centre; both are positive for faces whose right-hand
+ * normal points out of the enclosed volume.  A group with no faces gets 0 counts, area, volume and coverage and NaN
+ * centroid and sphere.  unassigned_faces [1] / unassigned_area [1] (DEVICE, both or neither NULL): the label -1 faces.
+ * Every sum runs in a fixed order: repeated calls give identical bits. */
+int fnr_mesh_measure_scratch_bytes(int64_t num_vertices, int64_t num_faces, size_t* bytes);
+int fnr_mesh_components(const int64_t* faces, int64_t num_faces, int64_t num_vertices, void* scratch, size_t scratch_bytes, int32_t* face_group,
+                        int64_t* num_groups, void* stream);
+#define FNR_MESH_ASSIGN_SCRATCH_BYTES 256
+int fnr_mesh_assign_centers(const double* vertices, const int64_t* faces, int64_t num_faces, int64_t num_vertices, const double* centers,
+                            int64_t num_centers, double max_distance, void* scratch, size_t scratch_bytes, int32_t* face_group, void* stream);
+int fnr_mesh_measure_groups(const double* vertices, const int64_t* faces, int64_t num_faces, int64_t num_vertices, const int32_t* face_group,
+                            int64_t num_groups, void* scratch, size_t scratch_bytes, int64_t* group_faces, int64_t* boundary_edges,
+                            int64_t* nonmanifold_edges, double* area, double* centroid, double* sphere, double* volume, double* coverage,
+                            int32_t* fit_ok, int64_t* unassigned_faces, double* unassigned_area, void* stream);
 
 /* Hash-grid row indices (exact-integer parity hook): rows[N,L,8] in nerfstudio corner order for
  * the masked [0,1]^3 positions of the given samples; also writes positions[N,3] if non-NULL. */
