@@ -13,7 +13,7 @@ CSRC = Path(__file__).resolve().parent / "csrc"
 LIB = CSRC / "libfruitnerf_b200.so"
 STAMP = CSRC / "libfruitnerf_b200.recipe"  # flags and sources LIB was built from
 SOURCES = ["fnr_api.cu", "fnr_simt.cu", "fnr_proposal.cu", "fnr_optim.cu", "fnr_glue.cu", "fnr_nvls.cu", "fnr_cluster.cu",
-           "fnr_fruit_split.cu", "fnr_render.cu", "fnr_mesh.cu", "fnr_poisson.cu", "fnr_measure.cu"]
+           "fnr_fruit_split.cu", "fnr_render.cu", "fnr_mesh.cu", "fnr_poisson.cu", "fnr_measure.cu", "fnr_metrics.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr",

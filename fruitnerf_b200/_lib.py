@@ -184,6 +184,10 @@ FNR_COMPOSE_SCRATCH_FLOATS = FNR_MAX_FRAME_OUTPUTS * 256 * 2
 FNR_OPT_ADAM, FNR_OPT_RADAM = 0, 1
 FNR_MESH_ASSIGN_SCRATCH_BYTES = 256
 FNR_MAX_ADAM_TENSORS = 48
+FNR_IMAGE_RECORD_DOUBLES = 12
+# record slots of fnr_image_stats / fnr_ssim (FNR_REC_* of the header), in order
+IMAGE_RECORD_FIELDS = ("sse", "rgb_min", "rgb_max", "image_min", "image_max", "accumulation_sum", "fruit_tp", "fruit_fp", "fruit_fn",
+                       "fruit_tn", "ssim", "data_range")
 
 LIB_PATH = Path(__file__).resolve().parent / "csrc" / "libfruitnerf_b200.so"
 
@@ -236,6 +240,9 @@ EXPORTED_SYMBOLS = (
     "fnr_mesh_components",
     "fnr_mesh_assign_centers",
     "fnr_mesh_measure_groups",
+    "fnr_image_metrics_scratch_bytes",
+    "fnr_image_stats",
+    "fnr_ssim",
 )
 
 _lib = None
@@ -360,6 +367,12 @@ def load() -> C.CDLL:
     lib.fnr_mesh_assign_centers.argtypes = [vp, vp, i64, i64, vp, i64, f64, vp, sz, vp, vp]
     lib.fnr_mesh_measure_groups.restype = C.c_int
     lib.fnr_mesh_measure_groups.argtypes = [vp, vp, i64, i64, vp, i64, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.fnr_image_metrics_scratch_bytes.restype = C.c_int
+    lib.fnr_image_metrics_scratch_bytes.argtypes = [i32, i32, C.POINTER(C.c_size_t)]
+    lib.fnr_image_stats.restype = C.c_int
+    lib.fnr_image_stats.argtypes = [vp, vp, vp, vp, vp, i32, i32, vp, sz, vp, vp]
+    lib.fnr_ssim.restype = C.c_int
+    lib.fnr_ssim.argtypes = [vp, vp, i32, i32, vp, sz, vp, vp]
     if lib.fnr_version() != ABI_VERSION:
         raise FruitNerfNativeError(f"ABI version mismatch: library reports {lib.fnr_version()}")
     _lib = lib

@@ -14,6 +14,8 @@ The reference takes these from third-party packages that are absent offline; wha
   turbo table; matplotlib is absent here, so the table is rebuilt from the published degree-5 polynomial fit of turbo (close to
   the table in the interior, visibly off at the two ends): these are pictures for a viewer / logger, not parity outputs.
   The `render` command's frame kernel (fnr_compose_frame) is handed this same table.
+* ``restated_image_scores`` -- the record the `eval` command's device kernels (fnr_image_stats, fnr_ssim) write for one
+  view, in fp64: the tests' reference for them.
 * LPIPS needs the pretrained AlexNet weights torchmetrics downloads: not restated; the key is omitted.
 """
 from __future__ import annotations
@@ -131,3 +133,36 @@ def image_metrics_and_images(outputs: Dict[str, Tensor], batch: Dict[str, Tensor
     metrics["fruit_iou"] = float(binary_jaccard((torch.sigmoid(sem) > 0.9)[..., 0], mask[..., 0])) if float(mask.sum()) or bool(
         (torch.sigmoid(sem) > 0.9).any()) else 1.0
     return metrics, images
+
+
+def restated_image_scores(rgb: Tensor, semantics: Tensor, accumulation: Tensor, image: Tensor, fruit_mask: Tensor) -> Dict[str, float]:
+    """What ``ops.image_stats`` and ``ops.image_ssim`` (fnr_metrics.cu) write into their record, restated in fp64 torch
+    on the inputs' device (the tests' reference; keys ``_lib.IMAGE_RECORD_FIELDS``).  ``rgb`` as rendered ([H*W,3] or
+    [H,W,3]), ``semantics`` logits, ``accumulation``, ``image`` [H,W,3] and ``fruit_mask`` [H,W,1], all fp32.
+    The SSIM is torchmetrics' with NO padding: the window runs over the unpadded images and the (H - 10) x (W - 10) map
+    that results is exactly the interior ``ssim`` above keeps after its crop, because a kept pixel's window never
+    reaches the reflect-padded border."""
+    H, W = image.shape[:2]
+    if H < 11 or W < 11:
+        raise ValueError(f"a {W}x{H} image is smaller than the 11x11 SSIM window")
+    x32 = torch.clamp(rgb.float().reshape(H, W, 3), min=0, max=1)
+    y32 = image.float().reshape(H, W, 3)
+    x, y = x32.double(), y32.double()
+    pred = (torch.sigmoid(semantics.float()) > 0.9).reshape(-1)
+    truth = (fruit_mask.float() > 0.5).reshape(-1)
+    out = {"sse": float(((x - y) ** 2).sum()), "rgb_min": float(x32.min()), "rgb_max": float(x32.max()), "image_min": float(y32.min()),
+           "image_max": float(y32.max()), "accumulation_sum": float(accumulation.double().sum()),
+           "fruit_tp": float((pred & truth).sum()), "fruit_fp": float((pred & ~truth).sum()), "fruit_fn": float((~pred & truth).sum()),
+           "fruit_tn": float((~pred & ~truth).sum())}
+    data_range = float(torch.maximum(x32.max() - x32.min(), y32.max() - y32.min()))  # fp32 differences, as torchmetrics
+    c1, c2 = (0.01 * data_range) ** 2, (0.03 * data_range) ** 2
+    g = _gaussian_window(11, 1.5, torch.float64, x.device)  # [1, 11]
+    xc, yc = x.permute(2, 0, 1)[:, None], y.permute(2, 0, 1)[:, None]  # [3,1,H,W]
+    stack = torch.cat((xc, yc, xc * xc, yc * yc, xc * yc))
+    rows = F.conv2d(stack, g[None, None])  # horizontal 11 taps, then vertical
+    mu_x, mu_y, xx, yy, xy = F.conv2d(rows, g.t()[None, None]).split(3)
+    mxx, myy, mxy = mu_x * mu_x, mu_y * mu_y, mu_x * mu_y
+    full = ((2 * mxy + c1) * (2 * (xy - mxy) + c2)) / ((mxx + myy + c1) * ((xx - mxx) + (yy - myy) + c2))
+    out["ssim"] = float(full.sum() / full.numel())
+    out["data_range"] = data_range
+    return out

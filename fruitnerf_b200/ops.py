@@ -1161,3 +1161,72 @@ def mesh_measure_groups(vertices: Tensor, faces: Tensor, face_group: Tensor, num
                                              p("nonmanifold_edges"), p("area"), p("centroid"), p("sphere"), p("volume"), p("coverage"),
                                              p("fit_ok"), _ptr(out["unassigned_faces"]), _ptr(out["unassigned_area"]), _stream(dev)))
     return out
+
+
+# ======================================================================================================
+# Held-out evaluation scores of one rendered view (fnr_metrics.cu; the `eval` command)
+# ======================================================================================================
+def image_metrics_scratch(height: int, width: int, dev) -> Tensor:
+    """The uint8 device scratch ``image_stats`` and ``image_ssim`` share for images of this size."""
+    nbytes = C.c_size_t(0)
+    L.check(L.load().fnr_image_metrics_scratch_bytes(int(height), int(width), C.byref(nbytes)))
+    return torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+
+
+def _metric_input(t: Tensor, numel: int, what: str) -> Tensor:
+    if t.dtype != torch.float32 or not t.is_contiguous() or t.numel() != numel:
+        raise ValueError(f"{what} must be a contiguous fp32 tensor of {numel} values, got {t.dtype} {tuple(t.shape)}"
+                         f"{'' if t.is_contiguous() else ' (not contiguous)'}")
+    return t
+
+
+def _metric_record(record: Optional[Tensor], dev) -> Tensor:
+    if record is None:
+        return torch.zeros(L.FNR_IMAGE_RECORD_DOUBLES, dtype=torch.float64, device=dev)
+    _require_cuda(record)
+    if record.dtype != torch.float64 or not record.is_contiguous() or record.numel() != L.FNR_IMAGE_RECORD_DOUBLES:
+        raise ValueError(f"record must be a contiguous fp64 tensor of {L.FNR_IMAGE_RECORD_DOUBLES} values, got {record.dtype} {tuple(record.shape)}")
+    return record
+
+
+def _image_size(image: Tensor) -> Tuple[int, int]:
+    if image.dim() != 3 or image.shape[2] != 3:
+        raise ValueError(f"image must be [H,W,3], got {tuple(image.shape)}")
+    return int(image.shape[0]), int(image.shape[1])
+
+
+def image_stats(rgb: Tensor, semantics: Tensor, accumulation: Tensor, image: Tensor, fruit_mask: Tensor, record: Optional[Tensor] = None,
+                scratch: Optional[Tensor] = None) -> Tensor:
+    """One pass over a rendered view (fnr_image_stats): ``rgb`` [H*W,3] as rendered, ``semantics`` logits and
+    ``accumulation`` [H*W] or [H*W,1], against ``image`` [H,W,3] and ``fruit_mask`` [H,W,1] or [H,W]; all CUDA fp32 and
+    contiguous.  Fills and returns ``record`` (fp64 [12], slots ``_lib.IMAGE_RECORD_FIELDS``; e.g. one row of an [N,12]
+    tensor): squared error of the clamped rgb, both value ranges, accumulation sum and fruit confusion counts."""
+    dev = _require_cuda(rgb, semantics, accumulation, image, fruit_mask, scratch)
+    H, W = _image_size(image)
+    P = H * W
+    _metric_input(image, 3 * P, "image")
+    _metric_input(rgb, 3 * P, "rgb")
+    _metric_input(semantics, P, "semantics")
+    _metric_input(accumulation, P, "accumulation")
+    _metric_input(fruit_mask, P, "fruit_mask")
+    record = _metric_record(record, dev)
+    if scratch is None:
+        scratch = image_metrics_scratch(H, W, dev)
+    L.check(L.load().fnr_image_stats(_ptr(rgb), _ptr(semantics), _ptr(accumulation), _ptr(image), _ptr(fruit_mask), H, W, _ptr(scratch),
+                                     scratch.numel() * scratch.element_size(), _ptr(record), _stream(dev)))
+    return record
+
+
+def image_ssim(rgb: Tensor, image: Tensor, record: Tensor, scratch: Optional[Tensor] = None) -> Tensor:
+    """torchmetrics' SSIM of the clamped ``rgb`` [H*W,3] against ``image`` [H,W,3] (fnr_ssim) into ``record``, which
+    ``image_stats`` of the same pair has filled on this stream (the data range comes from its min / max slots).  Images
+    with H or W < 11 are refused."""
+    dev = _require_cuda(rgb, image, record, scratch)
+    H, W = _image_size(image)
+    _metric_input(image, 3 * H * W, "image")
+    _metric_input(rgb, 3 * H * W, "rgb")
+    record = _metric_record(record, dev)
+    if scratch is None:
+        scratch = image_metrics_scratch(H, W, dev)
+    L.check(L.load().fnr_ssim(_ptr(rgb), _ptr(image), H, W, _ptr(scratch), scratch.numel() * scratch.element_size(), _ptr(record), _stream(dev)))
+    return record

@@ -298,6 +298,30 @@ def probe_outputs(model) -> List[str]:
 
 
 @torch.no_grad()
+def render_into_buffers(model, chunk_rays: Callable[[int, int], RayBundle], num_rays: int, chunk: int, names: Sequence[str],
+                        bufs: Dict[str, Tensor], stage: Callable[[str], None]) -> Dict[str, Tensor]:
+    """One image through the model, chunk by chunk, with nothing leaving the device: ``chunk_rays(p0, n)`` gives the rays
+    of pixels [p0, p0 + n) and the outputs ``names`` land in rows p0 .. p0 + n of ``bufs[name]`` ([num_rays, C] fp32,
+    allocated on first use and reused for the next image).  ``stage`` is told "rays" and "field" as each chunk's ray
+    generation and forward start.  Shared by ``render_frames`` and ``evaluate.evaluate_split``."""
+    dev = model.device
+    for p0 in range(0, num_rays, chunk):
+        n = min(chunk, num_rays - p0)
+        stage("rays")
+        bundle = chunk_rays(p0, n)
+        stage("field")
+        out = model(bundle)
+        for name in names:
+            if name not in out or not torch.is_tensor(out[name]):
+                raise KeyError(f"the model has no output {name!r}; available: {tensor_output_names(out)}")
+            t = out[name].reshape(n, -1)
+            if name not in bufs:
+                bufs[name] = torch.empty((num_rays, t.shape[1]), dtype=torch.float32, device=dev)
+            bufs[name][p0:p0 + n] = t
+    return bufs
+
+
+@torch.no_grad()
 def render_frames(pipeline, cameras: CameraSet, output_names: Sequence[str], num_rays_per_chunk: Optional[int] = None,
                   depth_near_plane: Optional[float] = None, depth_far_plane: Optional[float] = None,
                   sink: Optional[Callable[[np.ndarray], None]] = None, on_stage: Optional[Callable[[str], None]] = None) -> List[np.ndarray]:
@@ -328,20 +352,13 @@ def render_frames(pipeline, cameras: CameraSet, output_names: Sequence[str], num
     frames, bufs = [], {}
     for f in range(len(cams)):
         cam_idx = torch.full((n_max, 1), f, dtype=torch.long, device=dev)
-        for p0 in range(0, P, chunk):
-            n = min(chunk, P - p0)
-            stage("rays")
+
+        def chunk_rays(p0: int, n: int, f=f, cam_idx=cam_idx) -> RayBundle:
             o, d = ops.camera_rays(cams.camera_to_worlds, cams.fx, cams.fy, cams.cx, cams.cy, cams.camera_type, H, W, f, p0, n,
                                    out=(o_buf, d_buf))
-            stage("field")
-            out = model(RayBundle(origins=o, directions=d, camera_indices=cam_idx[:n]))
-            for name in needed:
-                if name not in out or not torch.is_tensor(out[name]):
-                    raise KeyError(f"the model has no output {name!r}; available: {tensor_output_names(out)}")
-                t = out[name].reshape(n, -1)
-                if name not in bufs:
-                    bufs[name] = torch.empty((P, t.shape[1]), dtype=torch.float32, device=dev)
-                bufs[name][p0:p0 + n] = t
+            return RayBundle(origins=o, directions=d, camera_indices=cam_idx[:n])
+
+        render_into_buffers(model, chunk_rays, P, chunk, needed, bufs, stage)
         stage("compose")
         images = []
         for name in names:

@@ -62,6 +62,9 @@
  *   fnr_mesh_measure_scratch_bytes, fnr_mesh_components, fnr_mesh_assign_centers, fnr_mesh_measure_groups
  *                        per-fruit measurement of the fruit meshes (no reference counterpart): grouping by connected
  *                        components or nearest count centre, area, sphere fit, volume, solid-angle coverage, edges
+ *   fnr_image_metrics_scratch_bytes, fnr_image_stats, fnr_ssim
+ *                        the `eval` command (nerfstudio ns-eval; FruitModel.get_image_metrics_and_images,
+ *                        fruit_nerf/fruit_nerf.py:403-458): PSNR, SSIM and fruit-mask agreement of a rendered view
  */
 #ifndef FRUITNERF_B200_H
 #define FRUITNERF_B200_H
@@ -639,6 +642,44 @@ int fnr_mesh_measure_groups(const double* vertices, const int64_t* faces, int64_
                             int64_t num_groups, void* scratch, size_t scratch_bytes, int64_t* group_faces, int64_t* boundary_edges,
                             int64_t* nonmanifold_edges, double* area, double* centroid, double* sphere, double* volume, double* coverage,
                             int32_t* fit_ok, int64_t* unassigned_faces, double* unassigned_area, void* stream);
+
+/* ---- Held-out evaluation scores of one rendered view (the `eval` command, nerfstudio ns-eval; fnr_metrics.cu; DESIGN
+ * section 4.3o) ----
+ * rgb: DEVICE [H*W,3] fp32 as rendered (clamped to [0,1] here, as FruitModel.get_image_metrics_and_images does; NaN stays
+ * NaN); semantics [H*W] logits, accumulation [H*W], image [H,W,3] and fruit_mask [H*W] ({0,1}): DEVICE fp32.
+ * 1 <= H*W <= (2^31 - 1) / 3.  record: DEVICE double[FNR_IMAGE_RECORD_DOUBLES], slots FNR_REC_*; the counts are whole
+ * numbers held exactly in fp64.  DEVICE scratch: fnr_image_metrics_scratch_bytes(H, W), shared by the two calls of one
+ * image.  Sums are fp64 block sums in a fixed tree, finished in index order over a grid that depends on H and W alone:
+ * no floating-point atomics, and repeated calls give identical bits.
+ *
+ * fnr_image_stats writes slots SSE .. FRUIT_TN: the sum over the 3 H W values of (clamp(rgb) - image)^2 (PSNR is
+ * 10 log10(3 H W / SSE)); min / max of clamp(rgb) and of image (NaN ignored); the sum of accumulation; the confusion
+ * counts of fp32 sigmoid(semantics) > 0.9 (the thresholding of FruitModel.get_outputs) against fruit_mask > 0.5.
+ * fnr_ssim reads the four min / max slots, so it follows fnr_image_stats of the same image on the stream, and writes
+ * slots SSIM and DATA_RANGE: torchmetrics structural_similarity_index_measure with its defaults (11x11 gaussian window,
+ * sigma 1.5, k1 0.01, k2 0.03, data_range = the larger fp32 value range of the two images, the map cropped by 5 pixels
+ * per side and averaged over pixels and channels), window sums and formula in fp64.  The crop keeps only windows that
+ * lie inside the image, so torchmetrics' reflect padding never reaches a kept pixel and none is applied.  H or W < 11
+ * (an empty cropped map) returns FNR_ERR_UNSUPPORTED. */
+#define FNR_IMAGE_RECORD_DOUBLES 12
+#define FNR_IMAGE_STATS_PARTIALS 256
+#define FNR_REC_SSE 0
+#define FNR_REC_RGB_MIN 1
+#define FNR_REC_RGB_MAX 2
+#define FNR_REC_IMAGE_MIN 3
+#define FNR_REC_IMAGE_MAX 4
+#define FNR_REC_ACCUMULATION_SUM 5
+#define FNR_REC_FRUIT_TP 6
+#define FNR_REC_FRUIT_FP 7
+#define FNR_REC_FRUIT_FN 8
+#define FNR_REC_FRUIT_TN 9
+#define FNR_REC_SSIM 10
+#define FNR_REC_DATA_RANGE 11
+int fnr_image_metrics_scratch_bytes(int32_t height, int32_t width, size_t* bytes);
+int fnr_image_stats(const float* rgb, const float* semantics, const float* accumulation, const float* image, const float* fruit_mask,
+                    int32_t height, int32_t width, void* scratch, size_t scratch_bytes, double* record, void* stream);
+int fnr_ssim(const float* rgb, const float* image, int32_t height, int32_t width, void* scratch, size_t scratch_bytes, double* record,
+             void* stream);
 
 /* Hash-grid row indices (exact-integer parity hook): rows[N,L,8] in nerfstudio corner order for
  * the masked [0,1]^3 positions of the given samples; also writes positions[N,3] if non-NULL. */
