@@ -75,6 +75,7 @@ struct KCompositeBwd {
 struct KFieldBwd {
   const float* point_grads;     // [N,5]
   const float* stash_encoding;  // [N,32] or NULL (recompute)
+  float2* denc;                 // [L][N] encoding gradients, level-major (small family's tensor-core backward; else NULL)
 };
 
 struct KExport {
@@ -225,7 +226,8 @@ inline int grid_for(long long work, int per_block, int max_blocks) {
 }
 
 // Field kernels of fnr_simt.cu for a shipped family: tc selects the tensor-core (wgmma, sm_90a) instantiation, otherwise
-// the exact-fp32 simt one.
+// the exact-fp32 simt one.  The small family's tensor-core backward is two launches: the field backward stores the encoding
+// gradients to B.denc, and level_scatter_kernel adds them to the table gradient one level at a time.
 int launch_field_forward(Family fam, bool tc, const KField& F, const KParams& P, const KRays& Rr, const KFieldOut& O, cudaStream_t st);
 int launch_field_backward(Family fam, bool tc, const KField& F, const KParams& P, const KParams& G, const KRays& Rr, const KFieldBwd& B,
                           cudaStream_t st);

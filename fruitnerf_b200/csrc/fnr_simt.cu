@@ -874,8 +874,16 @@ __global__ void __launch_bounds__(backward_threads<C, TC>()) simt_field_backward
       Lin::template dx<kBase0, C::ENC, C::BASE_H>(P.base_w[0], dh1, denc);
       Lin::template dw<kBase0, C::ENC, C::BASE_H>(sX, sY, enc, dh1, G.base_w[0], G.base_b[0]);
     }
-    // ---- hash-table scatter -----------------------------------------------------------------
-    if (valid) {
+    // ---- hash-table gradient -----------------------------------------------------------------
+    if constexpr (kResident) {
+      // level_scatter_kernel adds these to the table; streaming stores (one 256 B segment per warp and level) that do
+      // not evict the table gradient from L2.  The big family's staged kernel keeps the inline scatter: moving it out
+      // made its step slower (DESIGN.md section 4.3).
+      if (valid) {
+#pragma unroll
+        for (int l = 0; l < C::L; ++l) __stcs(B.denc + (size_t)l * N + p, make_float2(denc[2 * l], denc[2 * l + 1]));
+      }
+    } else if (valid) {
       float2* gt = reinterpret_cast<float2*>(G.hash_table);
 #pragma unroll 1
       for (int l = 0; l < C::L; ++l) {
@@ -913,6 +921,38 @@ extern "C" int fnr_bwd_phase_cycles(unsigned long long* out) {
   return e == cudaSuccess ? 0 : (int)e;
 }
 #endif
+
+// ------------------------------------------------------------------------------------------
+// K5: level-major hash-table scatter of the small family's tensor-core backward.  The work is the flat index over
+// (level, point), level outermost, grid-strided by persistent CTAs: the whole grid adds level 0 of every point, then
+// level 1, and so on.
+// Positions are recomputed with the backward's field_position from the same ray inputs, so the corner rows are the ones
+// the simt backward's inline scatter hits.  DESIGN.md section 4.3 has the measured choices (one level per work item,
+// no level left inline in the field backward).
+// ------------------------------------------------------------------------------------------
+constexpr int kScatterThreads = 256;
+
+__global__ void __launch_bounds__(kScatterThreads) level_scatter_kernel(KField F, KRays Rr, const float2* __restrict__ denc,
+                                                                       float2* __restrict__ table_grad) {
+  const long long N = (long long)Rr.R * Rr.S;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  const long long first = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  int l = (int)(first / N);
+  for (long long p = first - (long long)l * N; l < F.L; p += stride) {
+    while (p >= N) {  // the stride may exceed N
+      p -= N;
+      ++l;
+    }
+    if (l >= F.L) break;
+    const float2 g = __ldcs(denc + (size_t)l * N + p);
+    if (g.x == 0.f && g.y == 0.f) continue;
+    const int r = (int)(p / Rr.S);
+    bool sel;
+    const Vec3 pos = field_position(Rr.origins + 3 * (size_t)r, Rr.directions + 3 * (size_t)r, Rr.starts[p], Rr.ends[p],
+                                    F.position_mode, F.aabb, sel);
+    level_scatter(table_grad, pos, F.scalings[l], l, F.log2T, g.x, g.y);
+  }
+}
 
 // ------------------------------------------------------------------------------------------
 // Export kernel: uniform bins, field in AABB / mean-appearance mode, thresholds + compaction
@@ -1092,7 +1132,7 @@ int launch_field_forward(Family fam, bool tc, const KField& F, const KParams& P,
 
 int launch_field_backward(Family fam, bool tc, const KField& F, const KParams& P, const KParams& G, const KRays& Rr, const KFieldBwd& B,
                           cudaStream_t st) {
-  return with_layers(fam, tc, [&](auto c, auto t) {
+  const int rc = with_layers(fam, tc, [&](auto c, auto t) {
     using C = decltype(c);
     constexpr bool TC = decltype(t)::value;
     if constexpr (resident_backward<C, TC>()) {
@@ -1109,6 +1149,18 @@ int launch_field_backward(Family fam, bool tc, const KField& F, const KParams& P
     return launch_field_kernel(simt_field_backward_kernel<C, TC>, Layers<C, TC>::kBwdSmemBytes, (long long)Rr.R * Rr.S,
                                TC ? "simt_field_backward_kernel<wgmma>" : "simt_field_backward_kernel", st, F, P, G, Rr, B);
   });
+  const long long N = (long long)Rr.R * Rr.S;
+  if (rc || !(tc && fam == kFamilySmall) || N == 0) return rc;
+  // persistent CTAs, as many as are resident at once
+  static int per_sm = 0;
+  if (!per_sm) {
+    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, level_scatter_kernel, kScatterThreads, 0);
+    if (e != cudaSuccess) return check_cuda(e, "cudaOccupancyMaxActiveBlocksPerMultiprocessor");
+    if (per_sm < 1) per_sm = 1;
+  }
+  level_scatter_kernel<<<grid_for(N * F.L, kScatterThreads, sm_count() * per_sm), kScatterThreads, 0, st>>>(
+      F, Rr, B.denc, reinterpret_cast<float2*>(G.hash_table));
+  return check_launch("level_scatter_kernel");
 }
 
 int launch_export(Family fam, bool tc, const KField& F, const KParams& P, const KExport& E, cudaStream_t st) {

@@ -345,7 +345,10 @@ int fnr_render_backward(const fnr_field_desc* desc, const fnr_field_params* para
                         const fnr_render_saved* saved, const fnr_render_grads* upstream,
                         const fnr_field_params* grads, void* scratch, size_t scratch_bytes, void* stream);
 
-/* Bytes of caller-allocated device scratch fnr_render_backward needs for this shape. */
+/* Bytes of caller-allocated device scratch fnr_render_backward needs for this shape and desc: the per-sample upstream
+ * gradients (R*S*5 floats) for every impl, plus, for the fruit_nerf shape on the tensor-core impls, the level-major
+ * encoding gradients (R*S*L*F floats, about 96 MiB at 4096 x 192) that its table scatter reads.  fnr_render_backward
+ * refuses smaller scratch before any device work. */
 int fnr_render_backward_scratch_bytes(const fnr_field_desc* desc, int32_t num_rays, int32_t num_samples, size_t* bytes);
 
 /* Uniform-volume export of one ray batch: rays are `origins[b] + t * normal` (normal = 3 HOST

@@ -1,14 +1,17 @@
 """Device time of the render backward (`fnr_render_backward`: compositing backward + field backward) alone, at the
 bench.py shape (4096 rays x 192 samples, the bench.py field and batch), and optionally its split into phases.
 
-    python tools/bench_backward.py [--variant small|big] [--steps 20] [--phases] [--build-dir DIR] [--json FILE]
+    python tools/bench_backward.py [--variant small|big] [--steps 20] [--kernels] [--phases] [--build-dir DIR] [--json FILE]
 
 Each timed call is the autograd backward of `ops.render` (zeroing of the flat gradient buffer + the library call), CUDA
-events around it, the L2 flushed before every call as bench.py does.  `--phases` builds the library with
--DFNR_BWD_PHASE_TIMERS into --build-dir (a temporary directory by default, never the package's own library), and
+events around it, the L2 flushed before every call as bench.py does.  `--kernels` then runs the same calls again under
+torch.profiler, in a run of their own after the timed one, and adds the device time of each kernel of the backward per
+call (the field backward and fruit_nerf's tensor-core level-major table scatter separately).  `--phases` builds the
+library with -DFNR_BWD_PHASE_TIMERS into --build-dir (a temporary directory by default, never the package's own library), and
 prints the clock64() cycles per 128-point tile of every phase of the field backward kernel: stash / upstream loads,
 forward recompute, dx, dW, the dW flush to the global gradient (or to the CTA's accumulators, plus the CTA's one flush,
-amortised), and the hash-table scatter.  The phase marks synchronise the warpgroup, so the timer build is a little slower
+amortised), and the hash-table scatter (for fruit_nerf's tensor-core backward: the store of the encoding gradients for
+the scatter kernel).  The phase marks synchronise the warpgroup, so the timer build is a little slower
 than the normal one; its split is what it is for.
 """
 from __future__ import annotations
@@ -47,6 +50,7 @@ def main():
     ap.add_argument("--kernel", default="auto", choices=["auto", "simt", "tcgen05"])
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--kernels", action="store_true", help="device time per kernel from a torch.profiler run after the timed one")
     ap.add_argument("--phases", action="store_true", help="per-phase cycles from a -DFNR_BWD_PHASE_TIMERS build")
     ap.add_argument("--build-dir", default=None, help="where --phases builds its library (default: a temporary directory)")
     ap.add_argument("--json", default=None)
@@ -100,6 +104,16 @@ def main():
     res = {"variant": args.variant, "kernel": args.kernel, "rays": bench.R_RAYS, "samples": bench.S_SAMPLES,
            "render_backward_ms_median": statistics.median(ms), "render_backward_ms_min": min(ms),
            "render_backward_ms_max": max(ms), "steps": args.steps, "card": card()}
+    if args.kernels:
+        from torch.profiler import ProfilerActivity, profile
+
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for i in range(args.steps):
+                flush.fill_(float(i))
+                backward()
+            torch.cuda.synchronize()
+        per_kernel = {ka.key: ka.self_device_time_total / 1e3 for ka in prof.key_averages() if "fnr::" in ka.key}  # the library's kernels
+        res["kernel_ms_per_call"] = {k: round(v / args.steps, 4) for k, v in sorted(per_kernel.items(), key=lambda kv: -kv[1])}
     if args.phases:
         buf = (ctypes.c_uint64 * len(PHASES))()
         if lib.fnr_bwd_phase_cycles(buf) != 0:
