@@ -202,6 +202,7 @@ EXPORTED_SYMBOLS = (
     "fnr_render_backward_scratch_bytes",
     "fnr_export_forward",
     "fnr_hash_indices",
+    "fnr_level_scatter",
     "fnr_proposal_weights_forward",
     "fnr_proposal_weights_backward",
     "fnr_pdf_sample",
@@ -285,6 +286,8 @@ def load() -> C.CDLL:
     ]
     lib.fnr_hash_indices.restype = C.c_int
     lib.fnr_hash_indices.argtypes = [C.POINTER(FieldDesc), C.POINTER(RayBatch), C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.fnr_level_scatter.restype = C.c_int
+    lib.fnr_level_scatter.argtypes = [C.POINTER(FieldDesc), C.POINTER(RayBatch), C.c_void_p, C.c_void_p, C.c_void_p]
     lib.fnr_proposal_weights_forward.restype = C.c_int
     lib.fnr_proposal_weights_forward.argtypes = [C.POINTER(DensityDesc), C.POINTER(DensityParams), C.POINTER(RayBatch), C.c_void_p, C.c_void_p, C.c_void_p]
     lib.fnr_proposal_weights_backward.restype = C.c_int

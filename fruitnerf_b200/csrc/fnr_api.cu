@@ -350,6 +350,21 @@ int fnr_hash_indices(const fnr_field_desc* desc, const fnr_ray_batch* rays, int3
   return launch_hash_indices(make_field(desc), Rr, rows, positions, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int fnr_level_scatter(const fnr_field_desc* desc, const fnr_ray_batch* rays, const float* denc, float* table_grad, void* stream) {
+  int rc = validate_desc(desc);
+  if (rc) return rc;
+  KRays Rr;
+  fnr_field_desc d2 = *desc;
+  d2.appearance_mode = FNR_APP_ZEROS;
+  if ((rc = make_rays(&d2, rays, &Rr))) return rc;
+  if (desc->features_per_level != 2 || !denc || !aligned16(table_grad)) {
+    set_error("level scatter: features_per_level must be 2, denc non-NULL and table_grad 16-byte aligned");
+    return FNR_ERR_INVALID_ARGUMENT;
+  }
+  return launch_level_scatter(make_field(desc), Rr, reinterpret_cast<const float2*>(denc), reinterpret_cast<float2*>(table_grad),
+                              reinterpret_cast<cudaStream_t>(stream));
+}
+
 static int make_density(const fnr_density_desc* d, const fnr_density_params* p, KDensity* K, const char* what) {
   if (!d || !p) {
     set_error("%s: NULL density desc/params", what);

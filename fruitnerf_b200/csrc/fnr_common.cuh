@@ -16,6 +16,7 @@ namespace fnr {
 
 constexpr uint32_t kPrimeY = 2654435761u;
 constexpr uint32_t kPrimeZ = 805459861u;
+constexpr unsigned kFull = 0xffffffffu;  // every lane of a warp
 
 struct Vec3 {
   float x, y, z;
@@ -143,6 +144,68 @@ __device__ __forceinline__ void level_scatter(float2* __restrict__ table_grad, c
   }
 }
 
+// level_scatter of one level for the 32 points held by the lanes of a warp, with fewer reds.  When the lanes hold
+// consecutive samples of a ray, neighbouring lanes often share a cell and so add to the same rows.  For each corner, lanes
+// with equal rows in a row form a run; a segmented shuffle sum gives the run's total to its last lane, which alone issues
+// the red.  A cell's floor-x and ceil-x corners differ in x only; with an even floor x their rows are r and r ^ 1 (the
+// hash's x prime is 1 and the level base is even), one 16-byte-aligned pair, so where both runs end at the same lane their
+// totals go out as one float4 red.  table_grad must be 16-byte aligned.
+//
+// All 32 lanes call this together from warp-uniform control flow, the same number of times: it shuffles and ballots with
+// the full mask.  A lane with nothing to add passes active = false (its rows become the null key and its values zero).
+__device__ __forceinline__ void warp_level_scatter(float2* __restrict__ table_grad, const LevelCell& c, bool active, int level,
+                                                   uint32_t log2T, float g0, float g1, int lane) {
+  constexpr uint32_t kNull = 0xffffffffu;
+  constexpr int kCeilX[4] = {0, 1, 4, 5}, kFloorX[4] = {3, 2, 7, 6};  // x-neighbour corners in the oracle's order
+  const uint32_t mask = (1u << log2T) - 1u, base = (uint32_t)level << log2T;
+  active = active && (g0 != 0.f || g1 != 0.f);
+  const uint32_t at_or_below = 0xffffffffu >> (31 - lane);
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    uint32_t key[2];
+    float v[2][2];
+    int start[2];
+    bool last[2];
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int k = j ? kFloorX[q] : kCeilX[q];
+      const float w = corner_weight(c, k);
+      const bool on = active && w != 0.f;
+      key[j] = on ? corner_row(c, k, mask, base) : kNull;
+      v[j][0] = on ? w * g0 : 0.f;
+      v[j][1] = on ? w * g1 : 0.f;
+      const uint32_t up = __shfl_up_sync(kFull, key[j], 1);
+      const uint32_t heads = __ballot_sync(kFull, lane == 0 || key[j] != up);
+      start[j] = 31 - __clz(heads & at_or_below);
+      last[j] = lane == 31 || ((heads >> (lane + 1)) & 1u);
+    }
+    // segmented inclusive sums: after the step of distance d, a lane holds the sum over its run's last 2d lanes.  The
+    // loop ends when no lane with a row needs another step (a ballot, so every lane leaves on the same step).
+    for (int d = 1; d < 32; d <<= 1) {
+      const bool need0 = key[0] != kNull && lane - d >= start[0];
+      const bool need1 = key[1] != kNull && lane - d >= start[1];
+      if (!__ballot_sync(kFull, need0 || need1)) break;
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const float t0 = __shfl_up_sync(kFull, v[j][0], d), t1 = __shfl_up_sync(kFull, v[j][1], d);
+        if (j ? need1 : need0) {
+          v[j][0] += t0;
+          v[j][1] += t1;
+        }
+      }
+    }
+    const bool red0 = last[0] && key[0] != kNull, red1 = last[1] && key[1] != kNull;
+    if (red0 && red1 && (key[0] ^ key[1]) == 1u) {
+      const bool lo0 = key[0] < key[1];
+      const float4 v4 = lo0 ? make_float4(v[0][0], v[0][1], v[1][0], v[1][1]) : make_float4(v[1][0], v[1][1], v[0][0], v[0][1]);
+      atomicAdd(reinterpret_cast<float4*>(table_grad + (key[0] & ~1u)), v4);
+    } else {
+      if (red0) atomicAdd(table_grad + key[0], make_float2(v[0][0], v[0][1]));
+      if (red1) atomicAdd(table_grad + key[1], make_float2(v[1][0], v[1][1]));
+    }
+  }
+}
+
 // [NS] components_from_spherical_harmonics(levels=4) on the shifted direction (d+1)/2.
 __device__ __forceinline__ void sh_degree4(float dx, float dy, float dz, float* __restrict__ c) {
   const float x = (dx + 1.0f) * 0.5f, y = (dy + 1.0f) * 0.5f, z = (dz + 1.0f) * 0.5f;
@@ -182,7 +245,6 @@ __device__ __forceinline__ double dist2(double ax, double ay, double az, double 
 // ---- warp-per-ray primitives ----------------------------------------------------------------
 // A ray's samples are walked in chunks of 32, lane i holding sample c0 + i; `run` arguments carry a sum over the
 // earlier chunks.
-constexpr unsigned kFull = 0xffffffffu;
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

@@ -235,5 +235,7 @@ int launch_export(Family fam, bool tc, const KField& F, const KParams& P, const 
 int launch_simt_composite(const KRays& Rr, const KComposite& Cm, cudaStream_t st);
 int launch_simt_composite_backward(const KRays& Rr, const KCompositeBwd& B, cudaStream_t st);
 int launch_hash_indices(const KField& F, const KRays& Rr, int32_t* rows, float* positions, cudaStream_t st);
+// level_scatter_kernel alone: adds the [L][N] encoding gradients denc to the table gradient (16-byte aligned)
+int launch_level_scatter(const KField& F, const KRays& Rr, const float2* denc, float2* table_grad, cudaStream_t st);
 
 }  // namespace fnr

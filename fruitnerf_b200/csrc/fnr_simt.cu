@@ -923,34 +923,38 @@ extern "C" int fnr_bwd_phase_cycles(unsigned long long* out) {
 #endif
 
 // ------------------------------------------------------------------------------------------
-// K5: level-major hash-table scatter of the small family's tensor-core backward.  The work is the flat index over
-// (level, point), level outermost, grid-strided by persistent CTAs: the whole grid adds level 0 of every point, then
-// level 1, and so on.
+// K5: level-major hash-table scatter of the small family's tensor-core backward.  A work item is one level of one
+// 32-point chunk, taken by one warp; the items are ordered level-major and grid-strided over the warps of persistent CTAs,
+// so the whole grid adds level 0 of every point, then level 1, and so on.  A warp's lanes hold consecutive samples of a
+// ray, which at the coarse levels often share a cell: warp_level_scatter merges their reds.
 // Positions are recomputed with the backward's field_position from the same ray inputs, so the corner rows are the ones
-// the simt backward's inline scatter hits.  DESIGN.md section 4.3 has the measured choices (one level per work item,
-// no level left inline in the field backward).
+// the simt backward's inline scatter hits.  DESIGN.md section 4.3 has the measured choices (level-major rather than
+// all levels of a chunk per work item, one float4 red per x-neighbour pair).
 // ------------------------------------------------------------------------------------------
 constexpr int kScatterThreads = 256;
 
 __global__ void __launch_bounds__(kScatterThreads) level_scatter_kernel(KField F, KRays Rr, const float2* __restrict__ denc,
                                                                        float2* __restrict__ table_grad) {
   const long long N = (long long)Rr.R * Rr.S;
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  const long long first = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  int l = (int)(first / N);
-  for (long long p = first - (long long)l * N; l < F.L; p += stride) {
-    while (p >= N) {  // the stride may exceed N
-      p -= N;
-      ++l;
+  const long long chunks = (N + 31) / 32;
+  const long long warps = (long long)gridDim.x * (kScatterThreads / 32);
+  const int lane = threadIdx.x & 31;
+  // w is the same in every lane of a warp: every lane runs every iteration and reaches each shuffle of warp_level_scatter
+  // as often as the others.  No lane leaves the loop or skips an iteration on its own; a lane past N or with a zero
+  // gradient takes part with active = false.
+  for (long long w = ((long long)blockIdx.x * kScatterThreads + threadIdx.x) / 32; w < chunks * F.L; w += warps) {
+    const int l = (int)(w / chunks);
+    const long long p = (w - l * chunks) * 32 + lane;
+    const bool in = p < N;
+    const float2 g = in ? __ldcs(denc + (size_t)l * N + p) : make_float2(0.f, 0.f);
+    Vec3 pos{0.f, 0.f, 0.f};
+    if (in && (g.x != 0.f || g.y != 0.f)) {
+      const int r = (int)(p / Rr.S);
+      bool sel;
+      pos = field_position(Rr.origins + 3 * (size_t)r, Rr.directions + 3 * (size_t)r, Rr.starts[p], Rr.ends[p], F.position_mode,
+                           F.aabb, sel);
     }
-    if (l >= F.L) break;
-    const float2 g = __ldcs(denc + (size_t)l * N + p);
-    if (g.x == 0.f && g.y == 0.f) continue;
-    const int r = (int)(p / Rr.S);
-    bool sel;
-    const Vec3 pos = field_position(Rr.origins + 3 * (size_t)r, Rr.directions + 3 * (size_t)r, Rr.starts[p], Rr.ends[p],
-                                    F.position_mode, F.aabb, sel);
-    level_scatter(table_grad, pos, F.scalings[l], l, F.log2T, g.x, g.y);
+    warp_level_scatter(table_grad, level_cell(pos, F.scalings[l]), in, l, F.log2T, g.x, g.y, lane);
   }
 }
 
@@ -1149,8 +1153,13 @@ int launch_field_backward(Family fam, bool tc, const KField& F, const KParams& P
     return launch_field_kernel(simt_field_backward_kernel<C, TC>, Layers<C, TC>::kBwdSmemBytes, (long long)Rr.R * Rr.S,
                                TC ? "simt_field_backward_kernel<wgmma>" : "simt_field_backward_kernel", st, F, P, G, Rr, B);
   });
+  if (rc || !(tc && fam == kFamilySmall)) return rc;
+  return launch_level_scatter(F, Rr, B.denc, reinterpret_cast<float2*>(G.hash_table), st);
+}
+
+int launch_level_scatter(const KField& F, const KRays& Rr, const float2* denc, float2* table_grad, cudaStream_t st) {
   const long long N = (long long)Rr.R * Rr.S;
-  if (rc || !(tc && fam == kFamilySmall) || N == 0) return rc;
+  if (N == 0) return FNR_OK;
   // persistent CTAs, as many as are resident at once
   static int per_sm = 0;
   if (!per_sm) {
@@ -1158,8 +1167,8 @@ int launch_field_backward(Family fam, bool tc, const KField& F, const KParams& P
     if (e != cudaSuccess) return check_cuda(e, "cudaOccupancyMaxActiveBlocksPerMultiprocessor");
     if (per_sm < 1) per_sm = 1;
   }
-  level_scatter_kernel<<<grid_for(N * F.L, kScatterThreads, sm_count() * per_sm), kScatterThreads, 0, st>>>(
-      F, Rr, B.denc, reinterpret_cast<float2*>(G.hash_table));
+  level_scatter_kernel<<<grid_for((N + 31) / 32 * F.L, kScatterThreads / 32, sm_count() * per_sm), kScatterThreads, 0, st>>>(
+      F, Rr, denc, table_grad);
   return check_launch("level_scatter_kernel");
 }
 

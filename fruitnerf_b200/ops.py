@@ -268,6 +268,22 @@ def hash_indices(shape: FieldShape, origins, directions, starts, ends, position_
     return rows, pos
 
 
+def level_scatter(shape: FieldShape, origins, directions, starts, ends, position_mode: int, denc: Tensor, table_grad: Tensor):
+    """Adds the encoding gradients denc [L, R*S, 2] (level-major) to table_grad [L * 2**T, 2] in place, as the tensor-core
+    backward's table scatter does (test hook for that kernel alone)."""
+    dev = _require_cuda(origins, directions, starts, ends, denc, table_grad)
+    lib = L.load()
+    R, S = starts.shape
+    origins, directions, starts, ends, denc = map(_f32c, (origins, directions, starts, ends, denc))
+    if denc.shape != (shape.num_levels, R * S, 2):
+        raise ValueError(f"denc must be [{shape.num_levels}, {R * S}, 2], got {list(denc.shape)}")
+    if table_grad.dtype != torch.float32 or not table_grad.is_contiguous() or table_grad.numel() != shape.num_levels * 2 * (1 << shape.log2_hashmap_size):
+        raise ValueError("table_grad must be a contiguous fp32 [L * 2**T, 2] tensor")
+    desc = shape.desc(position_mode, L.FNR_APP_ZEROS)
+    rays = L.RayBatch(R, S, _ptr(origins), _ptr(directions), _ptr(starts), _ptr(ends), None)
+    L.check(lib.fnr_level_scatter(C.byref(desc), C.byref(rays), denc.data_ptr(), table_grad.data_ptr(), _stream(dev)))
+
+
 class ExportBuffers:
     """Device-side compaction buffers of the volume export (three point sets, see include/)."""
 

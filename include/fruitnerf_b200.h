@@ -689,6 +689,13 @@ int fnr_ssim(const float* rgb, const float* image, int32_t height, int32_t width
 int fnr_hash_indices(const fnr_field_desc* desc, const fnr_ray_batch* rays, int32_t* rows, float* positions,
                      void* stream);
 
+/* The tensor-core backward's table-gradient scatter on its own (test hook): for every level l and sample p, adds
+ * denc[l][p] (float2, level-major [L][N], N = num_rays * num_samples) times each corner's trilinear weight to the
+ * corner's row of table_grad [L * 2^log2T, 2] (16-byte aligned), at the masked positions of the given samples.
+ * features_per_level must be 2. */
+int fnr_level_scatter(const fnr_field_desc* desc, const fnr_ray_batch* rays, const float* denc, float* table_grad,
+                      void* stream);
+
 #ifdef __cplusplus
 }
 #endif
