@@ -150,7 +150,8 @@ enum Slot { kBase0, kBase1, kSem0, kSem1, kCol0, kCol1, kHead, kCol2, kSem2 };
 // How the field kernels evaluate a Linear layer W [N][K] (SLOT: which one): forward y = act(W x + b), input gradient
 // dx = W^T dy and weight gradient dW = dY^T X over the tile.  TC = false: per thread in fp32 on the CUDA cores (the exact
 // device reference).  TC = true: warpgroup-wide on the tensor cores with the weight tile staged from global memory at
-// every step (fnr_wgmma.cuh; every thread of the 128-thread CTA must take part).
+// every step (fnr_wgmma.cuh; every thread of the 128-thread CTA must take part): the big family's tensor-core path.  The
+// small family's runs on ResidentLayers below.
 template <class C, bool TC>
 struct Layers {
   // the 1- and 3-wide output heads (64 MACs per point) stay in exact fp32 on the CUDA cores on both paths
@@ -191,11 +192,11 @@ struct Layers {
   }
 };
 
-// The small family's tensor-core backward: CTAs of two warpgroups, each taking its own 128-point tiles.  Per CTA, the six
-// tensor-core layers are split once into a resident bf16 hi / lo image (the K-major tiles rowgemm stages, so the recompute
-// runs the forward's bytes and MMA sequence; dx reads the same image MN-major), and the weight gradients of all eight
-// layers are accumulated in fp32 in shared memory and added to the global gradient once, when the CTA ends.
-// Dynamic shared memory: weight image | accumulators | locks | per-warpgroup step tiles | per-warpgroup warp partials.
+// The small family's tensor-core kernels (forward, export, backward) run persistent CTAs of G warpgroups, each warpgroup
+// taking its own 128-point tiles.  Per CTA, the six tensor-core layers are split once into a resident bf16 hi / lo image
+// (the K-major tiles rowgemm stages, so every layer runs the staged path's bytes and MMA sequence; dx reads the same image
+// MN-major).  The backward also accumulates the weight gradients of all eight layers in fp32 in shared memory and adds
+// them to the global gradient once, when the CTA ends.
 // The resident plan of the small family: shape of every slot, offsets of its weight image (six tensor-core layers) and of
 // its fp32 gradient accumulator (all eight; wg::DwAcc layout for the tensor-core layers, [N][K] then [N] for the heads).
 namespace resident {
@@ -214,40 +215,63 @@ constexpr int N(int s) {
 constexpr bool tensor(int n) { return n >= 8; }
 constexpr int img_bytes(int s) { return 2 * wg::padn(N(s)) * wg::pad16(K(s)) * 2; }
 constexpr int img_off(int s) { return s == 0 ? 0 : img_off(s - 1) + img_bytes(s - 1); }
+constexpr int kImageBytes = img_off(kImageSlots);
+static_assert(kImageBytes == 64 * 1024, "16384 split weights");
 constexpr int acc_floats(int s) { return tensor(N(s)) ? (N(s) + 15) / 16 * 32 * (wg::padn(K(s)) / 2) + N(s) : N(s) * K(s) + N(s); }
 constexpr int acc_off(int s) { return s == 0 ? 0 : acc_off(s - 1) + (acc_floats(s - 1) + 3) / 4 * 4; }  // float4-aligned
 constexpr int align128(int b) { return (b + 127) / 128 * 128; }
 }  // namespace resident
 
+// Warpgroups per CTA of the resident forward and export.  Two fit the kernels' registers as compiled (CTA of 256
+// threads, 128 KiB of dynamic shared memory); three need <= 168 registers and 160 KiB (DESIGN.md section 4.3 has the
+// measured choice).
+#ifndef FNR_FWD_GROUPS
+#define FNR_FWD_GROUPS 2
+#endif
+
+// Dynamic shared memory of the resident forward and export CTA: weight image | per-warpgroup step tiles.
+struct ForwardPlan {
+  static constexpr int kGroups = FNR_FWD_GROUPS;
+  static constexpr int kStepOff = resident::kImageBytes;
+  static constexpr int kBytes = kStepOff + kGroups * wg::kResidentStepBytes;
+};
+// Dynamic shared memory of the resident backward CTA: weight image | accumulators | locks | per-warpgroup step tiles |
+// per-warpgroup warp partials.
+struct BackwardPlan {
+  static constexpr int kGroups = 2;
+  static constexpr int kAccOff = resident::kImageBytes;
+  static constexpr int kLockOff = kAccOff + resident::acc_off(resident::kSlots) * 4;
+  static constexpr int kStepOff = resident::align128(kLockOff + resident::kSlots * 4);
+  static constexpr int kPartOff = kStepOff + kGroups * wg::kResidentStepBytes;
+  static constexpr int kBytes = kPartOff + kGroups * 4 * wg::kWarpPartial * 4;
+};
+
+// The layers of the small family's tensor-core kernels on the resident image (Plan: the kernel's shared-memory plan).
+// fwd is the same code in the forward, the export and the backward's recompute; acc / lock / part, prepare, flush, dx
+// and dw exist in the backward's plan only.
+template <class Plan>
 struct ResidentLayers {
   using C = CfgSmall;
-  static constexpr int kGroups = 2;
+  static constexpr int kGroups = Plan::kGroups;
   static constexpr int kSlots = resident::kSlots;
   static constexpr int K(int s) { return resident::K(s); }
   static constexpr int N(int s) { return resident::N(s); }
   static constexpr bool tensor(int n) { return resident::tensor(n); }
   static constexpr int img_off(int s) { return resident::img_off(s); }
   static constexpr int acc_off(int s) { return resident::acc_off(s); }
-  static constexpr int kImageBytes = resident::img_off(resident::kImageSlots);
-  static constexpr int kAccOff = kImageBytes;
-  static constexpr int kLockOff = kAccOff + resident::acc_off(kSlots) * 4;
-  static constexpr int kStepOff = resident::align128(kLockOff + kSlots * 4);
-  static constexpr int kPartOff = kStepOff + kGroups * wg::kResidentStepBytes;
-  static constexpr int kBytes = kPartOff + kGroups * 4 * wg::kWarpPartial * 4;
-  static_assert(kImageBytes == 64 * 1024, "16384 split weights");
 
   static __device__ __forceinline__ uint8_t* smem() {
     extern __shared__ __align__(128) uint8_t wg_smem[];
     return wg_smem;
   }
-  static __device__ __forceinline__ uint8_t* step() { return smem() + kStepOff + wg::group() * wg::kResidentStepBytes; }
-  static __device__ __forceinline__ float* part() { return reinterpret_cast<float*>(smem() + kPartOff) + wg::group() * 4 * wg::kWarpPartial; }
+  static __device__ __forceinline__ uint8_t* step() { return smem() + Plan::kStepOff + wg::group() * wg::kResidentStepBytes; }
+  static __device__ __forceinline__ float* part() { return reinterpret_cast<float*>(smem() + Plan::kPartOff) + wg::group() * 4 * wg::kWarpPartial; }
   template <int S>
   static __device__ __forceinline__ float* acc() {
     constexpr int off = acc_off(S);
-    return reinterpret_cast<float*>(smem() + kAccOff) + off;
+    return reinterpret_cast<float*>(smem() + Plan::kAccOff) + off;
   }
-  static __device__ __forceinline__ int* lock(int s) { return reinterpret_cast<int*>(smem() + kLockOff) + s; }
+  static __device__ __forceinline__ int* lock(int s) { return reinterpret_cast<int*>(smem() + Plan::kLockOff) + s; }
   static __device__ __forceinline__ const float* weight(const KParams& P, int s) {
     return s == kBase0 ? P.base_w[0] : s == kBase1 ? P.base_w[1] : s == kSem0 ? P.sem_w[0] : s == kSem1 ? P.sem_w[1]
          : s == kCol0 ? P.col_w[0] : s == kCol1 ? P.col_w[1] : s == kHead ? P.head_w : P.col_w[2];
@@ -271,14 +295,23 @@ struct ResidentLayers {
       wg::split_store8(hi, hi + NP * KP * 2, kc * (NP * 16) + n * 16, v);
     }
   }
-  // Once per CTA, before the first tile: the weight image, zero accumulators and free locks.
-  static __device__ __forceinline__ void prepare(const KParams& P) {
+  static __device__ __forceinline__ void split_all(const KParams& P) {
     split_image<kBase0>(P);
     split_image<kBase1>(P);
     split_image<kSem0>(P);
     split_image<kSem1>(P);
     split_image<kCol0>(P);
     split_image<kCol1>(P);
+  }
+  // Once per CTA, before the first tile: the weight image (forward and export).
+  static __device__ __forceinline__ void build_image(const KParams& P) {
+    split_all(P);
+    wg::fence_proxy_async();
+    __syncthreads();
+  }
+  // Once per CTA, before the first tile: the weight image, zero accumulators and free locks (backward).
+  static __device__ __forceinline__ void prepare(const KParams& P) {
+    split_all(P);
     constexpr int kAccFloats = acc_off(kSlots);
     float* a = acc<0>();
     for (int i = threadIdx.x; i < kAccFloats; i += blockDim.x) a[i] = 0.f;
@@ -347,6 +380,8 @@ struct ResidentLayers {
     FNR_PHASE(kPhDw);
   }
 };
+using ResidentForward = ResidentLayers<ForwardPlan>;
+using ResidentBackward = ResidentLayers<BackwardPlan>;
 
 template <class C>
 struct Acts {
@@ -364,7 +399,7 @@ struct Acts {
 // The field's branch forwards.  field_mlps and the backward's recompute both run these, so the recompute gives the
 // forward's pre-activations bit for bit and its ReLU masks agree with the forward that ran.
 //
-// Lin: how the layers are evaluated (Layers<C, TC> or ResidentLayers).
+// Lin: how the layers are evaluated (Layers<C, TC> or ResidentLayers<Plan>).
 //
 // base MLP: enc -> [h0, geo...]; geo = out[1:]
 template <class C, class Lin>
@@ -404,10 +439,9 @@ __device__ __forceinline__ void colour_fwd(const KParams& P, const float* __rest
   Lin::template fwd<kCol2, C::COL_H, 3, false>(P.col_w[2], P.col_b[2], c2, o3);
 }
 
-template <class C, bool TC>
+template <class C, class Lin>
 __device__ __forceinline__ void field_mlps(const KParams& P, const float (&enc)[C::ENC], const float* __restrict__ dir,
                                            const float (&app)[C::APP], Acts<C>& a) {
-  using Lin = Layers<C, TC>;
   float geo[C::GEO];
   base_fwd<C, Lin>(P, enc, a.h1, a.out, geo);
   semantic_fwd<C, Lin>(P, geo, a.z1, a.z2, a.zo);
@@ -445,16 +479,38 @@ __device__ __forceinline__ void block_mean_embedding(const KParams& P, int num_i
 // ------------------------------------------------------------------------------------------
 // K1: per-point field forward.
 // ------------------------------------------------------------------------------------------
-// The loop runs whole 128-point tiles per CTA (threads past N compute a clamped point and store nothing), so that the
-// block-wide tensor-core layers see every thread.
+// The small family's tensor-core forward and export run on the resident weight image (ResidentForward); the other
+// instantiations stage the weights at every layer step (Layers<C, TC>) in CTAs of one warpgroup.
 template <class C, bool TC>
-__global__ void __launch_bounds__(kThreads) simt_field_forward_kernel(KField F, KParams P, KRays Rr, KFieldOut O) {
+constexpr bool on_resident_image() { return TC && std::is_same<C, CfgSmall>::value; }
+template <class C, bool TC>
+constexpr int forward_threads() { return on_resident_image<C, TC>() ? ForwardPlan::kGroups * kThreads : kThreads; }
+template <class C, bool TC>
+using ForwardLayers = std::conditional_t<on_resident_image<C, TC>(), ResidentForward, Layers<C, TC>>;
+// The warpgroup of this thread in a CTA of G warpgroups, and the thread's index in it (G = 1: the CTA's own indices, so
+// that the one-warpgroup kernels compile as they did before there were several)
+template <int G>
+__device__ __forceinline__ int group_of() { return G == 1 ? 0 : wg::group(); }
+template <int G>
+__device__ __forceinline__ unsigned thread_of() { return G == 1 ? threadIdx.x : (unsigned)wg::tid(); }
+
+// Every warpgroup takes whole 128-point tiles, tile g of CTA b then every (gridDim.x * warpgroups)-th one after it; threads
+// past N compute a clamped point and store nothing, so that the warpgroup-wide tensor-core layers see every thread.  A
+// warpgroup syncs on its own barrier only (wg::sync): the tile loop has no CTA-wide barrier, and a warpgroup without
+// tiles leaves at once.
+template <class C, bool TC>
+__global__ void __launch_bounds__(forward_threads<C, TC>()) simt_field_forward_kernel(KField F, KParams P, KRays Rr, KFieldOut O) {
+  constexpr int kGroups = forward_threads<C, TC>() / kThreads;
+  using Lin = ForwardLayers<C, TC>;
   __shared__ float s_app[C::APP];
   block_mean_embedding(P, F.num_images, C::APP, F.appearance_mode, s_app);
+  if constexpr (on_resident_image<C, TC>()) ResidentForward::build_image(P);
   const long long N = (long long)Rr.R * Rr.S;
-  for (long long p0 = (long long)blockIdx.x * blockDim.x; p0 < N; p0 += (long long)gridDim.x * blockDim.x) {
-    const bool valid = p0 + threadIdx.x < N;
-    const long long p = valid ? p0 + threadIdx.x : N - 1;
+  const int g = group_of<kGroups>();
+  const unsigned t = thread_of<kGroups>();
+  for (long long p0 = (long long)blockIdx.x * blockDim.x + g * kThreads; p0 < N; p0 += (long long)gridDim.x * blockDim.x) {
+    const bool valid = p0 + t < N;
+    const long long p = valid ? p0 + t : N - 1;
     const int r = (int)(p / Rr.S);
     const float* o = Rr.origins + 3 * (size_t)r;
     const float* d = Rr.directions + 3 * (size_t)r;
@@ -475,7 +531,7 @@ __global__ void __launch_bounds__(kThreads) simt_field_forward_kernel(KField F, 
 #pragma unroll
     for (int i = 0; i < C::APP; ++i) appv[i] = (F.appearance_mode == FNR_APP_PER_CAMERA) ? __ldg(app + i) : app[i];
     Acts<C> a;
-    field_mlps<C, TC>(P, enc, d, appv, a);
+    field_mlps<C, Lin>(P, enc, d, appv, a);
     if (!valid) continue;
     const float density = sel ? expf(a.out[0]) : 0.f;
     if (O.sample_density) O.sample_density[p] = density;
@@ -655,7 +711,7 @@ __global__ void __launch_bounds__(kThreads) simt_composite_backward_kernel(KRays
 // layer the tile's inputs X[128,K] and output grads dY[128,N] go to shared memory.  simt: each thread
 // reduces a 4x4 block of dW = dY^T X over the tile, then adds it to the global gradient.  Tensor cores:
 // the tile's dW is one MMA, added to the global gradient per tile (Layers<C, true>) or to accumulators in
-// shared memory that the CTA flushes once (ResidentLayers, small family).
+// shared memory that the CTA flushes once (ResidentBackward, small family).
 // ------------------------------------------------------------------------------------------
 template <int K, int N>
 __device__ __forceinline__ void tile_weight_grad(float* __restrict__ sX, float* __restrict__ sY, const float (&x)[K],
@@ -707,23 +763,21 @@ __device__ unsigned long long g_bwd_phase_cycles[kBwdPhases];
 #endif
 
 template <class C, bool TC>
-constexpr bool resident_backward() { return TC && std::is_same<C, CfgSmall>::value; }
-template <class C, bool TC>
-constexpr int backward_threads() { return resident_backward<C, TC>() ? ResidentLayers::kGroups * kThreads : kThreads; }
+constexpr int backward_threads() { return on_resident_image<C, TC>() ? ResidentBackward::kGroups * kThreads : kThreads; }
 
 template <class C, bool TC>
 __global__ void __launch_bounds__(backward_threads<C, TC>()) simt_field_backward_kernel(KField F, KParams P, KParams G, KRays Rr,
                                                                                        KFieldBwd B) {
-  constexpr bool kResident = resident_backward<C, TC>();
+  constexpr bool kResident = on_resident_image<C, TC>();
   constexpr int kGroups = backward_threads<C, TC>() / kThreads;  // warpgroups (tiles in flight) per CTA
-  using Lin = std::conditional_t<kResident, ResidentLayers, Layers<C, TC>>;
+  using Lin = std::conditional_t<kResident, ResidentBackward, Layers<C, TC>>;
   extern __shared__ __align__(16) float smem[];
   constexpr int TP = ((C::MAXW + 3) & ~3) + 4;
   float* sX = smem;
   float* sY = smem + kThreads * TP;
   __shared__ float s_app[C::APP];
   block_mean_embedding(P, F.num_images, C::APP, F.appearance_mode, s_app);
-  if constexpr (kResident) ResidentLayers::prepare(P);
+  if constexpr (kResident) ResidentBackward::prepare(P);
 #ifdef FNR_BWD_PHASE_TIMERS
   if (threadIdx.x < 2 * kBwdPhases) phase::cycles[threadIdx.x / kBwdPhases][threadIdx.x % kBwdPhases] = 0;
   if (wg::tid() == 0) phase::last[wg::group()] = clock64();
@@ -900,7 +954,7 @@ __global__ void __launch_bounds__(backward_threads<C, TC>()) simt_field_backward
 #ifdef FNR_BWD_PHASE_TIMERS
     const long long f0 = clock64();
 #endif
-    ResidentLayers::flush_all(G);
+    ResidentBackward::flush_all(G);
 #ifdef FNR_BWD_PHASE_TIMERS
     __syncthreads();
     if (threadIdx.x == 0) phase::cycles[0][kPhDwFlush] += (unsigned long long)(clock64() - f0);
@@ -975,14 +1029,19 @@ __device__ __forceinline__ int warp_claim(int* counter, bool pred, int lane, int
 }
 
 template <class C, bool TC>
-__global__ void __launch_bounds__(kThreads) simt_export_kernel(KField F, KParams P, KExport E) {
+__global__ void __launch_bounds__(forward_threads<C, TC>()) simt_export_kernel(KField F, KParams P, KExport E) {
+  constexpr int kGroups = forward_threads<C, TC>() / kThreads;
+  using Lin = ForwardLayers<C, TC>;
   __shared__ float s_app[C::APP];
   block_mean_embedding(P, F.num_images, C::APP, FNR_APP_MEAN, s_app);
+  if constexpr (on_resident_image<C, TC>()) ResidentForward::build_image(P);
   const int lane = threadIdx.x & 31;
   const long long N = (long long)E.B * E.S;
-  // whole 128-point tiles per CTA (see simt_field_forward_kernel): warp-converged row claims, block-wide MLP layers
-  for (long long p0 = (long long)blockIdx.x * blockDim.x; p0 < N; p0 += (long long)gridDim.x * blockDim.x) {
-    const long long p = p0 + threadIdx.x;
+  const int g = group_of<kGroups>();
+  const unsigned t = thread_of<kGroups>();
+  // whole 128-point tiles per warpgroup (see simt_field_forward_kernel): warp-converged row claims, warpgroup-wide MLP layers
+  for (long long p0 = (long long)blockIdx.x * blockDim.x + g * kThreads; p0 < N; p0 += (long long)gridDim.x * blockDim.x) {
+    const long long p = p0 + t;
     const bool valid = p < N;
     const long long pc = valid ? p : N - 1;
     const int r = (int)(pc / E.S), s = (int)(pc % E.S);
@@ -1001,7 +1060,7 @@ __global__ void __launch_bounds__(kThreads) simt_export_kernel(KField F, KParams
     float appv[C::APP];
     load_appearance(P, FNR_APP_MEAN, 0, s_app, appv);
     Acts<C> a;
-    field_mlps<C, TC>(P, enc, E.normal, appv, a);
+    field_mlps<C, Lin>(P, enc, E.normal, appv, a);
     const float density = sel ? expf(a.out[0]) : 0.f;
     const float sg = sigmoidf_(a.logit);
     // heaviside(sigmoid(logit) - thr, 0): 1 iff sigmoid - thr > 0
@@ -1118,6 +1177,17 @@ static int launch_field_kernel(Kernel kernel, int smem, long long N, const char*
   return check_launch(name);
 }
 
+// One launch of a resident kernel (the small family's tensor-core forward, export and backward): one CTA of `threads`
+// per SM (its shared memory is most of the SM's), no more CTAs than the points need.
+template <class Kernel, class... Args>
+static int launch_resident(Kernel kernel, int threads, int smem, long long N, const char* name, cudaStream_t st, const Args&... args) {
+  if (N == 0) return FNR_OK;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute");
+  kernel<<<grid_for(N, threads, sm_count()), threads, smem, st>>>(args...);
+  return check_launch(name);
+}
+
 // Calls launch(C{}, std::bool_constant<TC>{}) with the family's config C and the implementation TC as types.
 template <class Launch>
 static int with_layers(Family fam, bool tc, Launch launch) {
@@ -1129,6 +1199,9 @@ int launch_field_forward(Family fam, bool tc, const KField& F, const KParams& P,
   return with_layers(fam, tc, [&](auto c, auto t) {
     using C = decltype(c);
     constexpr bool TC = decltype(t)::value;
+    if constexpr (on_resident_image<C, TC>())
+      return launch_resident(simt_field_forward_kernel<C, TC>, forward_threads<C, TC>(), ForwardPlan::kBytes, (long long)Rr.R * Rr.S,
+                             "simt_field_forward_kernel<wgmma>", st, F, P, Rr, O);
     return launch_field_kernel(simt_field_forward_kernel<C, TC>, Layers<C, TC>::kFwdSmemBytes, (long long)Rr.R * Rr.S,
                                TC ? "simt_field_forward_kernel<wgmma>" : "simt_field_forward_kernel", st, F, P, Rr, O);
   });
@@ -1139,17 +1212,9 @@ int launch_field_backward(Family fam, bool tc, const KField& F, const KParams& P
   const int rc = with_layers(fam, tc, [&](auto c, auto t) {
     using C = decltype(c);
     constexpr bool TC = decltype(t)::value;
-    if constexpr (resident_backward<C, TC>()) {
-      // one CTA of two warpgroups per SM (its shared memory is most of the SM's), as many warpgroups as there are tiles
-      const long long N = (long long)Rr.R * Rr.S;
-      if (N == 0) return FNR_OK;
-      auto kernel = simt_field_backward_kernel<C, TC>;
-      constexpr int threads = backward_threads<C, TC>();
-      cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ResidentLayers::kBytes);
-      if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute");
-      kernel<<<grid_for(N, threads, sm_count()), threads, ResidentLayers::kBytes, st>>>(F, P, G, Rr, B);
-      return check_launch("simt_field_backward_kernel<wgmma>");
-    }
+    if constexpr (on_resident_image<C, TC>())
+      return launch_resident(simt_field_backward_kernel<C, TC>, backward_threads<C, TC>(), BackwardPlan::kBytes, (long long)Rr.R * Rr.S,
+                             "simt_field_backward_kernel<wgmma>", st, F, P, G, Rr, B);
     return launch_field_kernel(simt_field_backward_kernel<C, TC>, Layers<C, TC>::kBwdSmemBytes, (long long)Rr.R * Rr.S,
                                TC ? "simt_field_backward_kernel<wgmma>" : "simt_field_backward_kernel", st, F, P, G, Rr, B);
   });
@@ -1176,6 +1241,9 @@ int launch_export(Family fam, bool tc, const KField& F, const KParams& P, const 
   return with_layers(fam, tc, [&](auto c, auto t) {
     using C = decltype(c);
     constexpr bool TC = decltype(t)::value;
+    if constexpr (on_resident_image<C, TC>())
+      return launch_resident(simt_export_kernel<C, TC>, forward_threads<C, TC>(), ForwardPlan::kBytes, (long long)E.B * E.S,
+                             "simt_export_kernel<wgmma>", st, F, P, E);
     return launch_field_kernel(simt_export_kernel<C, TC>, Layers<C, TC>::kFwdSmemBytes, (long long)E.B * E.S,
                                TC ? "simt_export_kernel<wgmma>" : "simt_export_kernel", st, F, P, E);
   });

@@ -6,9 +6,10 @@
 // (x ~= hi + lo, 16 mantissa bits), the weights W[N][K] are split the same way, and the warpgroup runs
 // D[128, N] = Xhi Whi^T + Xlo Whi^T + Xhi Wlo^T + Xlo Wlo^T with fp32 accumulation (wgmma m64nNk16, two M halves);
 // the accumulator fragments go back to shared memory in fp32 and every thread reads its row.  Relative error of a
-// product ~2^-17 (the rounding of the lo halves), fp32-class for the parity bar of the tests.  The forward and export
-// kernels (one warpgroup per CTA) stage the weight tile from global memory at every step; the small family's backward
-// (two warpgroups per CTA) splits its weights once per CTA into a resident image and accumulates dW / db in shared memory.
+// product ~2^-17 (the rounding of the lo halves), fp32-class for the parity bar of the tests.  The small family's forward,
+// export and backward (CTAs of several warpgroups) split their weights once per CTA into a resident image, and the backward
+// accumulates dW / db in shared memory; the big family's kernels (one warpgroup per CTA) stage the weight tile from global
+// memory at every step.
 //
 // Operand layout (no swizzle, core matrices of 8 rows x 16 bytes).  K-major: element (row, k) of a ROWS x KP tile is at
 //     (k / 8) * (ROWS * 16) + row * 16 + (k % 8) * 2
