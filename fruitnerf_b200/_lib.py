@@ -185,6 +185,8 @@ FNR_OPT_ADAM, FNR_OPT_RADAM = 0, 1
 FNR_MESH_ASSIGN_SCRATCH_BYTES = 256
 FNR_MAX_ADAM_TENSORS = 48
 FNR_IMAGE_RECORD_DOUBLES = 12
+FNR_TEXTURE_MAX_SIDE = 16384
+FNR_MEAN_EDGE_DOUBLES = 1 + 256
 # record slots of fnr_image_stats / fnr_ssim (FNR_REC_* of the header), in order
 IMAGE_RECORD_FIELDS = ("sse", "rgb_min", "rgb_max", "image_min", "image_max", "accumulation_sum", "fruit_tp", "fruit_fp", "fruit_fn",
                        "fruit_tn", "ssim", "data_range")
@@ -244,6 +246,9 @@ EXPORTED_SYMBOLS = (
     "fnr_image_metrics_scratch_bytes",
     "fnr_image_stats",
     "fnr_ssim",
+    "fnr_texture_atlas_size",
+    "fnr_texel_rays",
+    "fnr_mesh_mean_edge",
 )
 
 _lib = None
@@ -376,6 +381,12 @@ def load() -> C.CDLL:
     lib.fnr_image_stats.argtypes = [vp, vp, vp, vp, vp, i32, i32, vp, sz, vp, vp]
     lib.fnr_ssim.restype = C.c_int
     lib.fnr_ssim.argtypes = [vp, vp, i32, i32, vp, sz, vp, vp]
+    lib.fnr_texture_atlas_size.restype = C.c_int
+    lib.fnr_texture_atlas_size.argtypes = [i64, i32, _i64p, _i64p]
+    lib.fnr_texel_rays.restype = C.c_int
+    lib.fnr_texel_rays.argtypes = [vp, vp, vp, i64, i32, i32, i32, f32, i64, i32, vp, vp, vp]
+    lib.fnr_mesh_mean_edge.restype = C.c_int
+    lib.fnr_mesh_mean_edge.argtypes = [vp, vp, i64, vp, vp]
     if lib.fnr_version() != ABI_VERSION:
         raise FruitNerfNativeError(f"ABI version mismatch: library reports {lib.fnr_version()}")
     _lib = lib

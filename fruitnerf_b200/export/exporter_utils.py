@@ -468,6 +468,74 @@ def export_poisson_mesh(pipeline, output_dir, num_points: int = 1000000, remove_
             "paths": paths}
 
 
+@torch.no_grad()
+def export_textured_mesh(pipeline, mesh: Dict, output_dir, prefix: str = "", px_per_uv_triangle: int = 4) -> Dict:
+    """nerfstudio texture_utils.export_textured_mesh with ``unwrap_method="custom"`` on the GPU, for one mesh dict of
+    ``export_tsdf_mesh`` / ``export_poisson_mesh`` ('vertices', 'normals', 'faces').  Every face gets its own triangle of
+    the atlas (texture.py), and every texel one ray from 0.5 raylen outside the surface along the inverted normal, near 0,
+    far raylen, camera 0, with raylen = 2 * the mean first-edge length (fnr_mesh_mean_edge).  The rays (fnr_texel_rays)
+    go through the model chunk by chunk on the device, the ``rgb`` output is quantised by fnr_compose_frame, and one
+    device-to-host copy gives the image.
+
+    Writes ``{prefix}mesh.obj``, ``{prefix}material_0.mtl`` and ``{prefix}material_0.png`` under ``output_dir``.  Returns
+    {'obj', 'mtl', 'png': paths, 'width', 'height', 'raylen'}.  An atlas side over texture.MAX_SIDE raises
+    texture.AtlasTooLargeError before anything is rendered or written."""
+    from PIL import Image
+
+    from .. import texture
+    from ..compat import RayBundle
+    from ..render import _turbo_table, render_into_buffers
+
+    model = pipeline.model
+    dev = next(model.parameters()).device
+    if dev.type != "cuda":
+        raise RuntimeError("export_textured_mesh needs the model on a CUDA device: the texel rays are a CUDA kernel")
+    p = texture.check_px_per_uv_triangle(px_per_uv_triangle)
+    faces = np.asarray(mesh["faces"], np.int64).reshape(-1, 3)
+    W, H = texture.atlas_size(len(faces), p)
+    t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a, dt)).to(dev)  # noqa: E731
+    verts, nrms, fdev = t(mesh["vertices"], np.float32).reshape(-1, 3), t(mesh["normals"], np.float32).reshape(-1, 3), t(faces, np.int64)
+    raylen = float(np.float32(2.0 * float(ops.mesh_mean_edge(verts, fdev))))
+    P = W * H
+    chunk = min(int(model.config.eval_num_rays_per_chunk), P)
+    o_buf = torch.empty((chunk, 3), dtype=torch.float32, device=dev)
+    d_buf = torch.empty((chunk, 3), dtype=torch.float32, device=dev)
+    cam_idx = torch.zeros((chunk, 1), dtype=torch.long, device=dev)
+    nears = torch.zeros((chunk, 1), dtype=torch.float32, device=dev)
+    fars = torch.full((chunk, 1), raylen, dtype=torch.float32, device=dev)
+
+    def chunk_rays(t0: int, n: int) -> RayBundle:
+        o, d = ops.texel_rays(verts, nrms, fdev, p, W, H, raylen, t0, n, out=(o_buf, d_buf))
+        return RayBundle(origins=o, directions=d, camera_indices=cam_idx[:n], nears=nears[:n], fars=fars[:n])
+
+    bufs = render_into_buffers(model, chunk_rays, P, chunk, ["rgb"], {}, lambda _stage: None)
+    image = ops.compose_frame([ops.FrameImage(bufs["rgb"], "color")], None, H, W, _turbo_table(dev)).cpu().numpy()
+    out_dir = pathlib.Path(output_dir)
+    out_dir.mkdir(parents=True, exist_ok=True)
+    mtl, png = f"{prefix}material_0.mtl", f"{prefix}material_0.png"
+    paths = {"obj": str(out_dir / f"{prefix}mesh.obj"), "mtl": str(out_dir / mtl), "png": str(out_dir / png)}
+    Image.fromarray(image).save(paths["png"])
+    texture.write_textured_obj(paths["obj"], mtl, png, mesh["vertices"], mesh["normals"], faces, texture.uv_coordinates(len(faces), p))
+    return {**paths, "width": W, "height": H, "raylen": raylen}
+
+
+def export_textured_meshes(pipeline, result: Dict, output_dir, px_per_uv_triangle: int = 4) -> Dict[str, str]:
+    """Texture the scene mesh (``mesh.obj`` / ``material_0.{mtl,png}``) and, unless it is empty, the fruit mesh
+    (``fruit_mesh.obj`` / ``fruit_material_0.{mtl,png}``) of an ``export_tsdf_mesh`` / ``export_poisson_mesh`` result.
+    Both atlases are sized first, so an atlas that is too large (texture.AtlasTooLargeError) writes nothing.  Returns the
+    paths, keyed 'mesh_obj', 'mesh_mtl', 'mesh_png' and 'fruit_mesh_obj', ...."""
+    from .. import texture
+
+    jobs = [(key, prefix) for key, prefix in (("mesh", ""), ("fruit_mesh", "fruit_")) if len(result[key]["faces"]) > 0]
+    for key, _ in jobs:
+        texture.atlas_size(len(result[key]["faces"]), px_per_uv_triangle)
+    paths = {}
+    for key, prefix in jobs:
+        r = export_textured_mesh(pipeline, result[key], output_dir, prefix, px_per_uv_triangle)
+        paths.update({f"{key}_{kind}": r[kind] for kind in ("obj", "mtl", "png")})
+    return paths
+
+
 _FACE_DTYPE = np.dtype([("n", "u1"), ("v", "<i4", (3,))])  # packed: 13 bytes per face
 
 

@@ -1246,3 +1246,47 @@ def image_ssim(rgb: Tensor, image: Tensor, record: Tensor, scratch: Optional[Ten
         scratch = image_metrics_scratch(H, W, dev)
     L.check(L.load().fnr_ssim(_ptr(rgb), _ptr(image), H, W, _ptr(scratch), scratch.numel() * scratch.element_size(), _ptr(record), _stream(dev)))
     return record
+
+
+# ======================================================================================================
+# NeRF textures of exported meshes (fnr_texture.cu; nerfstudio texture_utils.export_textured_mesh, unwrap "custom")
+# ======================================================================================================
+def _texture_mesh(vertices: Tensor, faces: Tensor, normals: Optional[Tensor] = None):
+    dev = _require_cuda(vertices, faces, normals)
+    v = _f32c(vertices.detach().reshape(-1, 3))
+    n = None if normals is None else _f32c(normals.detach().reshape(-1, 3))
+    if n is not None and n.shape != v.shape:
+        raise ValueError(f"{v.shape[0]} vertices with {n.shape[0]} normals")
+    f = faces.detach().reshape(-1, 3).to(torch.int64).contiguous()
+    if f.shape[0] < 1:
+        raise ValueError("the mesh has no faces")
+    return dev, v, n, f
+
+
+def texel_rays(vertices: Tensor, normals: Tensor, faces: Tensor, px_per_uv_triangle: int, width: int, height: int, raylen: float,
+               texel_start: int, num_texels: int, out: Optional[Tuple[Tensor, Tensor]] = None) -> Tuple[Tensor, Tensor]:
+    """Origins and unit directions [n,3] of texels [texel_start, texel_start + n) (row-major) of the per-face atlas of a mesh
+    (fnr_texel_rays): vertices / normals [V,3] fp32 and faces [F,3] int64 on the device, (width, height) the atlas size
+    (texture.atlas_size).  ``out``: preallocated (origins, directions) with at least n rows, of which the first n are
+    written and returned."""
+    dev, v, n, f = _texture_mesh(vertices, faces, normals)
+    if out is None:
+        o = torch.empty((num_texels, 3), dtype=torch.float32, device=dev)
+        d = torch.empty((num_texels, 3), dtype=torch.float32, device=dev)
+    else:
+        _require_cuda(*out)
+        o, d = out[0][:num_texels], out[1][:num_texels]
+        if o.shape != (num_texels, 3) or d.shape != (num_texels, 3) or not (o.is_contiguous() and d.is_contiguous()):
+            raise ValueError("out buffers must be contiguous fp32 [>= n, 3]")
+    L.check(L.load().fnr_texel_rays(_ptr(v), _ptr(n), _ptr(f), int(f.shape[0]), int(px_per_uv_triangle), int(width), int(height), float(raylen),
+                                    int(texel_start), int(num_texels), _ptr(o), _ptr(d), _stream(dev)))
+    return o, d
+
+
+def mesh_mean_edge(vertices: Tensor, faces: Tensor) -> Tensor:
+    """The mean over faces of the first edge's length |v1 - v0| (fnr_mesh_mean_edge), a 0-dim fp64 CUDA tensor: fp64
+    sums in a fixed order, so repeated calls give identical bits."""
+    dev, v, _, f = _texture_mesh(vertices, faces)
+    out = torch.empty(L.FNR_MEAN_EDGE_DOUBLES, dtype=torch.float64, device=dev)
+    L.check(L.load().fnr_mesh_mean_edge(_ptr(v), _ptr(f), int(f.shape[0]), _ptr(out), _stream(dev)))
+    return out[0]

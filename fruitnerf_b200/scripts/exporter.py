@@ -17,7 +17,8 @@ from typing import Optional, Tuple
 
 import torch
 
-from ..export.exporter_utils import export_poisson_mesh, export_tsdf_mesh, generate_point_cloud, sample_volume, write_ply
+from ..export.exporter_utils import (export_poisson_mesh, export_textured_meshes, export_tsdf_mesh, generate_point_cloud, sample_volume,
+                                     write_ply)
 
 
 def eval_setup(config_path, eval_num_rays_per_chunk: Optional[int] = None, test_mode: str = "test", device: Optional[str] = None):
@@ -142,8 +143,10 @@ class ExportPointCloud(Exporter):
 @dataclass
 class ExportTSDFMesh(Exporter):
     """nerfstudio 0.3.2 ExportTSDFMesh: a surface mesh of the scene by TSDF fusion of rendered depth maps, plus the mesh of
-    the fruit surfaces (faces whose vertices have a fused fruit probability >= 0.5).  Single GPU.  Only vertex colours
-    (``texture_method="tsdf"``) are implemented: NeRF texturing needs an xatlas UV unwrap."""
+    the fruit surfaces (faces whose vertices have a fused fruit probability >= 0.5).  Single GPU.  The PLYs carry vertex
+    colours.  ``texture_method="nerf"`` with ``unwrap_method="custom"`` also writes both meshes as OBJs textured by the
+    NeRF, ``px_per_uv_triangle`` texels per face (DESIGN section 4.3p); the xatlas unwrap is not available.  Unlike
+    nerfstudio, the full mesh is textured (no ``target_num_faces`` decimation)."""
 
     downscale_factor: int = 2
     depth_output_name: str = "depth"
@@ -156,13 +159,14 @@ class ExportTSDFMesh(Exporter):
     texture_method: str = "tsdf"
     refine_mesh_using_initial_aabb_estimate: bool = False
     refinement_epsilon: float = 1e-2
+    unwrap_method: str = "xatlas"
+    px_per_uv_triangle: int = 4
 
     def validate(self) -> None:
         """Refuse what cannot run, before anything is loaded."""
-        if self.texture_method == "nerf":
-            raise ValueError("texture_method 'nerf' needs an xatlas UV unwrap, which is not available; use 'tsdf' (vertex colours)")
-        if self.texture_method != "tsdf":
+        if self.texture_method not in ("tsdf", "nerf"):
             raise ValueError(f"texture_method must be 'tsdf' or 'nerf', got {self.texture_method!r}")
+        _validate_nerf_texture(self.texture_method, self.unwrap_method, self.px_per_uv_triangle, "tsdf")
         res = tuple(self.resolution) if isinstance(self.resolution, (list, tuple)) else (self.resolution,)
         if len(res) not in (1, 3) or min(int(r) for r in res) < 2:
             raise ValueError(f"resolution must be one or three integers >= 2, got {list(res)}")
@@ -174,28 +178,36 @@ class ExportTSDFMesh(Exporter):
             raise ValueError("Bounding box min must be smaller than max")
 
     def main(self, pipeline=None) -> dict:
-        """Writes ``output_dir/tsdf_mesh.ply`` and ``output_dir/fruit_mesh.ply``; returns export_tsdf_mesh's dict."""
+        """Writes ``output_dir/tsdf_mesh.ply`` and ``output_dir/fruit_mesh.ply``, and with NeRF texturing then
+        ``mesh.obj`` / ``material_0.{mtl,png}`` and ``fruit_mesh.obj`` / ``fruit_material_0.{mtl,png}`` (no fruit OBJ for an
+        empty fruit mesh); returns export_tsdf_mesh's dict, the OBJ, MTL and PNG paths added to its 'paths'.  An atlas
+        over texture.MAX_SIDE a side raises texture.AtlasTooLargeError after the PLYs are written, before any OBJ."""
         self.validate()
         if pipeline is None:
             if self.load_config is None:
                 raise ValueError("pass load_config (a run folder's config.yml) or an already built pipeline")
             _, pipeline, _, _ = eval_setup(self.load_config)
         res = list(self.resolution) if isinstance(self.resolution, (list, tuple)) else [self.resolution]
-        return export_tsdf_mesh(pipeline, Path(self.output_dir), downscale_factor=self.downscale_factor, depth_output_name=self.depth_output_name,
-                                rgb_output_name=self.rgb_output_name, resolution=res, batch_size=self.batch_size,
-                                use_bounding_box=self.use_bounding_box, bounding_box_min=self.bounding_box_min,
-                                bounding_box_max=self.bounding_box_max,
-                                refine_mesh_using_initial_aabb_estimate=self.refine_mesh_using_initial_aabb_estimate,
-                                refinement_epsilon=self.refinement_epsilon)
+        out = export_tsdf_mesh(pipeline, Path(self.output_dir), downscale_factor=self.downscale_factor, depth_output_name=self.depth_output_name,
+                               rgb_output_name=self.rgb_output_name, resolution=res, batch_size=self.batch_size,
+                               use_bounding_box=self.use_bounding_box, bounding_box_min=self.bounding_box_min,
+                               bounding_box_max=self.bounding_box_max,
+                               refine_mesh_using_initial_aabb_estimate=self.refine_mesh_using_initial_aabb_estimate,
+                               refinement_epsilon=self.refinement_epsilon)
+        if self.texture_method == "nerf":
+            out["paths"].update(export_textured_meshes(pipeline, out, Path(self.output_dir), self.px_per_uv_triangle))
+        return out
 
 
 @dataclass
 class ExportPoissonMesh(Exporter):
     """nerfstudio 0.3.2 ExportPoissonMesh: a watertight mesh of the scene by screened Poisson reconstruction of the surface
     cloud, trimmed at the 0.1 quantile of vertex density, plus the mesh of the fruit surfaces (faces whose vertices have a
-    fruit probability >= 0.5).  Single GPU.  Only vertex colours (``texture_method="point_cloud"``) are implemented: NeRF
-    texturing needs an xatlas UV unwrap.  ``depth`` (open3d's octree depth, here the dense grid's 2^depth cells per
-    axis) is the one option upstream does not have."""
+    fruit probability >= 0.5).  Single GPU.  The PLYs carry vertex colours.  ``texture_method="nerf"`` with
+    ``unwrap_method="custom"`` also writes both meshes as OBJs textured by the NeRF, ``px_per_uv_triangle`` texels per
+    face (DESIGN section 4.3p); the xatlas unwrap is not available.  Unlike nerfstudio, the full mesh is textured (no
+    ``target_num_faces`` decimation).  ``depth`` (open3d's octree depth, here the dense grid's 2^depth cells per axis) is
+    the one option upstream does not have."""
 
     num_points: int = 1000000
     remove_outliers: bool = True
@@ -213,15 +225,16 @@ class ExportPoissonMesh(Exporter):
     texture_method: str = "point_cloud"
     std_ratio: float = 10.0
     depth: int = 9
+    unwrap_method: str = "xatlas"
+    px_per_uv_triangle: int = 4
 
     def validate(self) -> None:
         """Refuse what cannot run, before anything is loaded."""
         from .. import poisson
 
-        if self.texture_method == "nerf":
-            raise ValueError("texture_method 'nerf' needs an xatlas UV unwrap, which is not available; use 'point_cloud' (vertex colours)")
-        if self.texture_method != "point_cloud":
+        if self.texture_method not in ("point_cloud", "nerf"):
             raise ValueError(f"texture_method must be 'point_cloud' or 'nerf', got {self.texture_method!r}")
+        _validate_nerf_texture(self.texture_method, self.unwrap_method, self.px_per_uv_triangle, "point_cloud")
         if self.normal_method not in ("open3d", "model_output"):
             raise ValueError(f"normal_method must be 'open3d' or 'model_output', got {self.normal_method!r}")
         poisson.check_depth(self.depth)
@@ -231,8 +244,9 @@ class ExportPoissonMesh(Exporter):
             raise ValueError("Bounding box min must be smaller than max")
 
     def main(self, pipeline=None) -> dict:
-        """Writes ``output_dir/poisson_mesh.ply`` and ``output_dir/fruit_poisson_mesh.ply``; returns export_poisson_mesh's
-        dict.  Exits with status 1 for ``normal_method="model_output"`` when the model renders no ``normal_output_name``."""
+        """Writes ``output_dir/poisson_mesh.ply`` and ``output_dir/fruit_poisson_mesh.ply``, and with NeRF texturing the
+        OBJs as ExportTSDFMesh.main does; returns export_poisson_mesh's dict.  Exits with status 1 for
+        ``normal_method="model_output"`` when the model renders no ``normal_output_name``."""
         self.validate()
         if pipeline is None:
             if self.load_config is None:
@@ -241,11 +255,26 @@ class ExportPoissonMesh(Exporter):
         if self.normal_method == "model_output":
             _require_normal_output(pipeline, self.normal_output_name)
         pipeline.datamanager.config.train_num_rays_per_batch = self.num_rays_per_batch
-        return export_poisson_mesh(pipeline, Path(self.output_dir), num_points=self.num_points, remove_outliers=self.remove_outliers,
-                                   reorient_normals=self.reorient_normals, depth_output_name=self.depth_output_name,
-                                   rgb_output_name=self.rgb_output_name, save_point_cloud=self.save_point_cloud,
-                                   use_bounding_box=self.use_bounding_box, bounding_box_min=self.bounding_box_min,
-                                   bounding_box_max=self.bounding_box_max, std_ratio=self.std_ratio, depth=self.depth)
+        out = export_poisson_mesh(pipeline, Path(self.output_dir), num_points=self.num_points, remove_outliers=self.remove_outliers,
+                                  reorient_normals=self.reorient_normals, depth_output_name=self.depth_output_name,
+                                  rgb_output_name=self.rgb_output_name, save_point_cloud=self.save_point_cloud,
+                                  use_bounding_box=self.use_bounding_box, bounding_box_min=self.bounding_box_min,
+                                  bounding_box_max=self.bounding_box_max, std_ratio=self.std_ratio, depth=self.depth)
+        if self.texture_method == "nerf":
+            out["paths"].update(export_textured_meshes(pipeline, out, Path(self.output_dir), self.px_per_uv_triangle))
+        return out
+
+
+def _validate_nerf_texture(texture_method: str, unwrap_method: str, px_per_uv_triangle: int, vertex_colours: str) -> None:
+    """The options of NeRF texturing: only the per-face ("custom") unwrap is available, at >= 2 texels per triangle."""
+    from ..texture import check_px_per_uv_triangle
+
+    if unwrap_method not in ("xatlas", "custom"):
+        raise ValueError(f"unwrap_method must be 'xatlas' or 'custom', got {unwrap_method!r}")
+    if texture_method == "nerf" and unwrap_method == "xatlas":
+        raise ValueError(f"texture_method 'nerf' with the xatlas UV unwrap needs the xatlas package, which is not available; use "
+                         f"--unwrap-method custom (one atlas triangle per face) or texture_method '{vertex_colours}' (vertex colours)")
+    check_px_per_uv_triangle(px_per_uv_triangle)
 
 
 def _require_normal_output(pipeline, normal_output_name: str) -> None:
@@ -293,8 +322,8 @@ def add_pointcloud_parser(sub) -> argparse.ArgumentParser:
 
 
 def add_tsdf_parser(sub) -> argparse.ArgumentParser:
-    """The ``tsdf`` subcommand: ExportTSDFMesh's fields as nerfstudio's option names, same defaults (texture method
-    ``tsdf``, the only one implemented)."""
+    """The ``tsdf`` subcommand: ExportTSDFMesh's fields as nerfstudio's option names, same defaults except the texture
+    method, which stays ``tsdf``: nerfstudio's default, ``nerf`` with the xatlas unwrap, is not available."""
     d = ExportTSDFMesh(load_config=None, output_dir=Path("."))
     p = sub.add_parser("tsdf", help="surface meshes of the scene and of the fruit by TSDF fusion of rendered depth")
     p.add_argument("--load-config", type=Path, required=True)
@@ -310,12 +339,13 @@ def add_tsdf_parser(sub) -> argparse.ArgumentParser:
     p.add_argument("--texture-method", choices=("tsdf", "nerf"), default=d.texture_method)
     p.add_argument("--refine-mesh-using-initial-aabb-estimate", type=_flag, default=d.refine_mesh_using_initial_aabb_estimate)
     p.add_argument("--refinement-epsilon", type=float, default=d.refinement_epsilon)
+    p.add_argument("--unwrap-method", choices=("xatlas", "custom"), default=d.unwrap_method)
+    p.add_argument("--px-per-uv-triangle", type=int, default=d.px_per_uv_triangle)
     return p
 
 
 def add_poisson_parser(sub) -> argparse.ArgumentParser:
-    """The ``poisson`` subcommand: ExportPoissonMesh's fields as nerfstudio's option names, same defaults (texture method
-    ``point_cloud``, the only one implemented), plus ``--depth``."""
+    """The ``poisson`` subcommand: ExportPoissonMesh's fields as nerfstudio's option names, same defaults, plus ``--depth``."""
     d = ExportPoissonMesh(load_config=None, output_dir=Path("."))
     p = sub.add_parser("poisson", help="watertight meshes of the scene and of the fruit by screened Poisson reconstruction")
     p.add_argument("--load-config", type=Path, required=True)
@@ -335,6 +365,8 @@ def add_poisson_parser(sub) -> argparse.ArgumentParser:
     p.add_argument("--texture-method", choices=("point_cloud", "nerf"), default=d.texture_method)
     p.add_argument("--std-ratio", type=float, default=d.std_ratio)
     p.add_argument("--depth", type=int, default=d.depth)
+    p.add_argument("--unwrap-method", choices=("xatlas", "custom"), default=d.unwrap_method)
+    p.add_argument("--px-per-uv-triangle", type=int, default=d.px_per_uv_triangle)
     return p
 
 
@@ -344,11 +376,15 @@ def poisson_exporter_from_args(a) -> ExportPoissonMesh:
                              normal_method=a.normal_method, normal_output_name=a.normal_output_name, save_point_cloud=a.save_point_cloud,
                              use_bounding_box=a.use_bounding_box, bounding_box_min=tuple(a.bounding_box_min),
                              bounding_box_max=tuple(a.bounding_box_max), num_rays_per_batch=a.num_rays_per_batch,
-                             texture_method=a.texture_method, std_ratio=a.std_ratio, depth=a.depth)
+                             texture_method=a.texture_method, std_ratio=a.std_ratio, depth=a.depth, unwrap_method=a.unwrap_method,
+                             px_per_uv_triangle=a.px_per_uv_triangle)
 
 
 def _run_mesh_export(exp, parser):
-    """validate (argparse error, status 2), run, exit 1 on an empty mesh, print the two meshes."""
+    """validate (argparse error, status 2), run, exit 1 on an empty mesh or an atlas that is too large, print the two
+    meshes (and their textured OBJs)."""
+    from ..texture import AtlasTooLargeError
+
     try:
         exp.validate()
     except ValueError as e:
@@ -356,13 +392,15 @@ def _run_mesh_export(exp, parser):
     try:
         res = exp.main()
     except RuntimeError as e:
-        if "empty mesh" not in str(e):
+        if "empty mesh" not in str(e) and not isinstance(e, AtlasTooLargeError):
             raise
         print(f"error: {e}", file=sys.stderr)
         sys.exit(1)
     for key in ("mesh", "fruit_mesh"):
         m = res[key]
         print(f"{key}: {m['vertices'].shape[0]} vertices, {m['faces'].shape[0]} faces -> {res['paths'][key]}")
+        if f"{key}_obj" in res["paths"]:
+            print(f"{key}: textured -> {res['paths'][f'{key}_obj']} ({res['paths'][f'{key}_png']})")
     return res
 
 
@@ -372,7 +410,8 @@ def tsdf_exporter_from_args(a) -> ExportTSDFMesh:
                           batch_size=a.batch_size, use_bounding_box=a.use_bounding_box, bounding_box_min=tuple(a.bounding_box_min),
                           bounding_box_max=tuple(a.bounding_box_max), texture_method=a.texture_method,
                           refine_mesh_using_initial_aabb_estimate=a.refine_mesh_using_initial_aabb_estimate,
-                          refinement_epsilon=a.refinement_epsilon)
+                          refinement_epsilon=a.refinement_epsilon, unwrap_method=a.unwrap_method,
+                          px_per_uv_triangle=a.px_per_uv_triangle)
 
 
 def entrypoint(argv=None):

@@ -65,6 +65,9 @@
  *   fnr_image_metrics_scratch_bytes, fnr_image_stats, fnr_ssim
  *                        the `eval` command (nerfstudio ns-eval; FruitModel.get_image_metrics_and_images,
  *                        fruit_nerf/fruit_nerf.py:403-458): PSNR, SSIM and fruit-mask agreement of a rendered view
+ *   fnr_texture_atlas_size, fnr_texel_rays, fnr_mesh_mean_edge
+ *                        NeRF textures of the `tsdf` / `poisson` meshes (nerfstudio texture_utils.export_textured_mesh,
+ *                        unwrap_method="custom"): the per-face UV atlas, one ray per texel, the ray length
  */
 #ifndef FRUITNERF_B200_H
 #define FRUITNERF_B200_H
@@ -683,6 +686,45 @@ int fnr_image_stats(const float* rgb, const float* semantics, const float* accum
                     int32_t height, int32_t width, void* scratch, size_t scratch_bytes, double* record, void* stream);
 int fnr_ssim(const float* rgb, const float* image, int32_t height, int32_t width, void* scratch, size_t scratch_bytes, double* record,
              void* stream);
+
+/* ---- NeRF textures of exported meshes (`--texture-method nerf --unwrap-method custom`, nerfstudio
+ * texture_utils.export_textured_mesh with unwrap_method="custom"; fnr_texture.cu; DESIGN section 4.3p) ----
+ * The atlas of F faces at p = px_per_uv_triangle texels per triangle (2 <= p, 1 <= F <= FNR_TEXTURE_MAX_FACES): blocks
+ * of p rows by p + 3 columns, two faces each (faces 2k and 2k + 1 in block k), blocks row-major, bx per row, where bx is
+ * the smallest b >= 1 with b^2 (p + 3) >= ceil(F / 2) p.  width = bx (p + 3), height = ceil(ceil(F / 2) / bx) p; a side over
+ * FNR_TEXTURE_MAX_SIDE is refused.  Texel (row, col), row 0 at the top (OBJ v = 1 - (row + 0.5) / height), lies in block
+ * (row / p) bx + col / (p + 3) at (a, b) = (col % (p + 3), row % p); it belongs to slot 2 block + (a + b >= p + 1), whose
+ * frame coordinates are (a, b) for the first slot and (p + 2 - a, p - 1 - b) for the second.  In its frame a slot's UV
+ * triangle has its face's vertices 0, 1, 2 at the texel centres (0, 0), (p - 1, 0), (0, p - 1).  A bilinear lookup inside
+ * the triangle reads only texels of its own slot, and slots >= F (after the last face) are never sampled; their texels
+ * take the rays of face F - 1.
+ *
+ * fnr_texel_rays writes the rays of texels [texel_start, texel_start + num_texels) (row-major) of that atlas: vertices,
+ * normals DEVICE [V,3] fp32; faces DEVICE [F,3] int64, every index in [0, V) (not checked); origins, directions DEVICE
+ * [num_texels,3] fp32.  Per texel, in fp32 without FMA: the frame coordinates (la, lb) give the closest point (xs, ys) of
+ * the triangle, (la, lb) itself when la + lb <= p - 1, else xs = clamp(la - 0.5, 0, p - 1), ys = (p - 1) - xs;
+ * s = xs / (p - 1), t = ys / (p - 1), w0 = (1 - s) - t; x = (w0 v0 + s v1) + t v2 and n = (w0 n0 + s n1) + t n2 per
+ * component; |n| = sqrt((n.x^2 + n.y^2) + n.z^2).  When |n| > 1e-12 fails, n is the face normal (v1 - v0) x (v2 - v0)
+ * (each component a rounded difference of rounded products), and when that fails too, (0, 0, 1).  With n_k = n_k / |n|:
+ * direction = -n, origin_k = x_k + (0.5 raylen) n_k.  The rays are nerfstudio's: origin 0.5 raylen outside the surface,
+ * nears 0 and fars raylen (set by the caller).  FNR_ERR_INVALID_ARGUMENT: a NULL pointer, p < 2, F < 1, a width / height
+ * other than the layout's, a texel range outside [0, width * height), a raylen that is not finite and positive.
+ *
+ * fnr_mesh_mean_edge writes out[0] = the mean over faces of |v1 - v0| (fp64 differences of the fp32 vertices, sum
+ * (d.x^2 + d.y^2) + d.z^2, no FMA): block b of FNR_MEAN_EDGE_PARTIALS sums faces [b per, (b + 1) per), per =
+ * ceil(F / FNR_MEAN_EDGE_PARTIALS), into out[1 + b] in a fixed tree, and one finish adds the partials in a fixed tree.  No
+ * atomics: repeated calls give identical bits.  out: DEVICE double[FNR_MEAN_EDGE_DOUBLES].
+ *
+ * fnr_texture_atlas_size writes the layout's HOST width and height (also when a side exceeds FNR_TEXTURE_MAX_SIDE). */
+#define FNR_TEXTURE_MAX_SIDE 16384
+#define FNR_TEXTURE_MAX_FACES (2LL * FNR_TEXTURE_MAX_SIDE * FNR_TEXTURE_MAX_SIDE)
+#define FNR_MEAN_EDGE_PARTIALS 256
+#define FNR_MEAN_EDGE_DOUBLES (1 + FNR_MEAN_EDGE_PARTIALS)
+int fnr_texture_atlas_size(int64_t num_faces, int32_t px_per_uv_triangle, int64_t* width, int64_t* height);
+int fnr_texel_rays(const float* vertices, const float* normals, const int64_t* faces, int64_t num_faces, int32_t px_per_uv_triangle,
+                   int32_t width, int32_t height, float raylen, int64_t texel_start, int32_t num_texels, float* origins, float* directions,
+                   void* stream);
+int fnr_mesh_mean_edge(const float* vertices, const int64_t* faces, int64_t num_faces, double* out, void* stream);
 
 /* Hash-grid row indices (exact-integer parity hook): rows[N,L,8] in nerfstudio corner order for
  * the masked [0,1]^3 positions of the given samples; also writes positions[N,3] if non-NULL. */
