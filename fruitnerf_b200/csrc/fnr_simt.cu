@@ -174,6 +174,13 @@ struct Layers {
     else
       linear_fwd<K, N, RELU>(W, b, x, y);
   }
+  // m = relu(W0 x + b0), y = act(W1 m + b1): two steps
+  template <int S0, int S1, int K0, int N0, int N1, bool RELU1>
+  static __device__ __forceinline__ void fwd2(const float* __restrict__ W0, const float* __restrict__ b0, const float* __restrict__ W1,
+                                              const float* __restrict__ b1, const float (&x)[K0], float (&m)[N0], float (&y)[N1]) {
+    fwd<S0, K0, N0, true>(W0, b0, x, m);
+    fwd<S1, N0, N1, RELU1>(W1, b1, m, y);
+  }
   template <int SLOT, int K, int N>
   static __device__ __forceinline__ void dx(const float* __restrict__ W, const float (&dy)[N], float (&dxv)[K]) {
     if constexpr (tensor(N))
@@ -189,6 +196,13 @@ struct Layers {
     else
       tile_weight_grad<K, N>(sX, sY, x, dy, gW, gb);
     FNR_PHASE(kPhDw);
+  }
+  // Both gradients of one layer: dxv = W^T dy, then dW / db from (x, dy).
+  template <int SLOT, int K, int N>
+  static __device__ __forceinline__ void grad(const float* __restrict__ W, float* sX, float* sY, const float (&x)[K], const float (&dy)[N],
+                                              float (&dxv)[K], float* gW, float* gb) {
+    dx<SLOT, K, N>(W, dy, dxv);
+    dw<SLOT, K, N>(sX, sY, x, dy, gW, gb);
   }
 };
 
@@ -247,7 +261,7 @@ struct BackwardPlan {
 };
 
 // The layers of the small family's tensor-core kernels on the resident image (Plan: the kernel's shared-memory plan).
-// fwd is the same code in the forward, the export and the backward's recompute; acc / lock / part, prepare, flush, dx
+// fwd and fwd2 are the same code in the forward, the export and the backward's recompute; acc / lock / part, prepare, flush, dx
 // and dw exist in the backward's plan only.
 template <class Plan>
 struct ResidentLayers {
@@ -347,25 +361,33 @@ struct ResidentLayers {
     flush<kCol2>(G);
   }
 
+  // The fp32 heads only: every tensor-core layer runs in a chained pair (fwd2).
   template <int SLOT, int Kv, int Nv, bool RELU>
   static __device__ __forceinline__ void fwd(const float* __restrict__ W, const float* __restrict__ b, const float (&x)[Kv], float (&y)[Nv]) {
-    static_assert(K(SLOT) == Kv && N(SLOT) == Nv, "slot shape");
-    if constexpr (tensor(Nv)) {
-      wg::resident_rowgemm<wg::padn(Nv), wg::pad16(Kv), false>(step(), smem() + img_off(SLOT), x, y);
+    static_assert(K(SLOT) == Kv && N(SLOT) == Nv && !tensor(Nv), "slot shape");
+    linear_fwd<Kv, Nv, RELU>(W, b, x, y);
+  }
+  // Two tensor-core layers chained (wg::resident_chain), m = relu(W0 x + b0), y = act(W1 m + b1).  In the forward and
+  // the export, m goes from the first layer's accumulators to the second layer's operand tile without a round trip
+  // through rows, and is left unset.  The backward, whose weight gradients and ReLU masks read m, gets it as rows.  The
+  // bias and ReLU are the same fp32 operations either way, so m and y have the same bits.
+  template <int S0, int S1, int K0, int N0, int N1, bool RELU1>
+  static __device__ __forceinline__ void fwd2(const float* __restrict__, const float* __restrict__ b0, const float* __restrict__,
+                                              const float* __restrict__ b1, const float (&x)[K0], float (&m)[N0], float (&y)[N1]) {
+    static_assert(K(S0) == K0 && N(S0) == N0 && K(S1) == N0 && N(S1) == N1 && tensor(N0) && tensor(N1), "slot shapes");
+    wg::resident_chain<wg::padn(N0), wg::pad16(K0), wg::padn(N1), std::is_same<Plan, BackwardPlan>::value>(
+        step(), smem() + img_off(S0), smem() + img_off(S1), x, m, y, [&](int c, float v) { return fmaxf(v + __ldg(b0 + c), 0.f); });
 #pragma unroll
-      for (int n = 0; n < Nv; ++n) {  // as wg::linear
-        const float v = y[n] + __ldg(b + n);
-        y[n] = RELU ? fmaxf(v, 0.f) : v;
-      }
-    } else {
-      linear_fwd<Kv, Nv, RELU>(W, b, x, y);
+    for (int n = 0; n < N1; ++n) {  // as wg::linear
+      const float v = y[n] + __ldg(b1 + n);
+      y[n] = RELU1 ? fmaxf(v, 0.f) : v;
     }
   }
   template <int SLOT, int Kv, int Nv>
   static __device__ __forceinline__ void dx(const float* __restrict__ W, const float (&dy)[Nv], float (&dxv)[Kv]) {
     static_assert(K(SLOT) == Kv && N(SLOT) == Nv, "slot shape");
     if constexpr (tensor(Nv))
-      wg::resident_rowgemm<wg::padn(Nv), wg::pad16(Kv), true>(step(), smem() + img_off(SLOT), dy, dxv);
+      wg::resident_rowgemm_t<wg::padn(Nv), wg::pad16(Kv)>(step(), smem() + img_off(SLOT), dy, dxv);
     else
       linear_bwd_input<Kv, Nv>(W, dy, dxv);
     FNR_PHASE(kPhDx);
@@ -378,6 +400,14 @@ struct ResidentLayers {
     else
       wg::head_weight_grad_acc<Kv, Nv>(part(), x, dy, acc<SLOT>(), lock(SLOT));
     FNR_PHASE(kPhDw);
+  }
+  // Both gradients of one layer, the weight gradient first: dy is then last read when dx stages it, so it is not live
+  // next to dxv.  For a 64-wide layer that is 64 fewer live registers at the backward's peak (DESIGN.md section 4.3).
+  template <int SLOT, int Kv, int Nv>
+  static __device__ __forceinline__ void grad(const float* __restrict__ W, float* sX, float* sY, const float (&x)[Kv],
+                                              const float (&dy)[Nv], float (&dxv)[Kv], float* gW, float* gb) {
+    dw<SLOT, Kv, Nv>(sX, sY, x, dy, gW, gb);
+    dx<SLOT, Kv, Nv>(W, dy, dxv);
   }
 };
 using ResidentForward = ResidentLayers<ForwardPlan>;
@@ -405,8 +435,8 @@ struct Acts {
 template <class C, class Lin>
 __device__ __forceinline__ void base_fwd(const KParams& P, const float (&enc)[C::ENC], float (&h1)[C::BASE_H],
                                          float (&out)[C::BASE_OUT], float (&geo)[C::GEO]) {
-  Lin::template fwd<kBase0, C::ENC, C::BASE_H, true>(P.base_w[0], P.base_b[0], enc, h1);
-  Lin::template fwd<kBase1, C::BASE_H, C::BASE_OUT, false>(P.base_w[1], P.base_b[1], h1, out);
+  Lin::template fwd2<kBase0, kBase1, C::ENC, C::BASE_H, C::BASE_OUT, false>(P.base_w[0], P.base_b[0], P.base_w[1], P.base_b[1], enc,
+                                                                            h1, out);
 #pragma unroll
   for (int i = 0; i < C::GEO; ++i) geo[i] = out[1 + i];
 }
@@ -415,12 +445,12 @@ __device__ __forceinline__ void base_fwd(const KParams& P, const float (&enc)[C:
 template <class C, class Lin>
 __device__ __forceinline__ void semantic_fwd(const KParams& P, const float (&geo)[C::GEO], float (&z1)[C::SEM_H],
                                              float (&z2)[C::SEM_LAYERS == 3 ? C::SEM_H : 1], float (&zo)[C::SEM_OUT]) {
-  Lin::template fwd<kSem0, C::GEO, C::SEM_H, true>(P.sem_w[0], P.sem_b[0], geo, z1);
   if constexpr (C::SEM_LAYERS == 3) {
+    Lin::template fwd<kSem0, C::GEO, C::SEM_H, true>(P.sem_w[0], P.sem_b[0], geo, z1);
     Lin::template fwd<kSem1, C::SEM_H, C::SEM_H, true>(P.sem_w[1], P.sem_b[1], z1, z2);
     Lin::template fwd<kSem2, C::SEM_H, C::SEM_OUT, false>(P.sem_w[2], P.sem_b[2], z2, zo);
   } else {
-    Lin::template fwd<kSem1, C::SEM_H, C::SEM_OUT, false>(P.sem_w[1], P.sem_b[1], z1, zo);
+    Lin::template fwd2<kSem0, kSem1, C::GEO, C::SEM_H, C::SEM_OUT, false>(P.sem_w[0], P.sem_b[0], P.sem_w[1], P.sem_b[1], geo, z1, zo);
   }
 }
 
@@ -434,8 +464,7 @@ __device__ __forceinline__ void colour_fwd(const KParams& P, const float* __rest
   for (int i = 0; i < C::GEO; ++i) cin[C::SH + i] = geo[i];
 #pragma unroll
   for (int i = 0; i < C::APP; ++i) cin[C::SH + C::GEO + i] = app[i];
-  Lin::template fwd<kCol0, C::COL_IN, C::COL_H, true>(P.col_w[0], P.col_b[0], cin, c1);
-  Lin::template fwd<kCol1, C::COL_H, C::COL_H, true>(P.col_w[1], P.col_b[1], c1, c2);
+  Lin::template fwd2<kCol0, kCol1, C::COL_IN, C::COL_H, C::COL_H, true>(P.col_w[0], P.col_b[0], P.col_w[1], P.col_b[1], cin, c1, c2);
   Lin::template fwd<kCol2, C::COL_H, 3, false>(P.col_w[2], P.col_b[2], c2, o3);
 }
 
@@ -812,7 +841,7 @@ __global__ void __launch_bounds__(backward_threads<C, TC>()) simt_field_backward
     }
     const int cam = (F.appearance_mode == FNR_APP_PER_CAMERA) ? Rr.camera_indices[r] : 0;
     float appv[C::APP];
-    load_appearance(P, F.appearance_mode, cam, s_app, appv);
+    if constexpr (!kResident) load_appearance(P, F.appearance_mode, cam, s_app, appv);
     // upstream per-point grads (zero for padding threads)
     const float* pg = B.point_grads + 5 * (size_t)pc;
     const float vm = valid ? 1.f : 0.f;
@@ -839,20 +868,16 @@ __global__ void __launch_bounds__(backward_threads<C, TC>()) simt_field_backward
       FNR_PHASE(kPhRecompute);
       float dlg[1] = {d_logit};
       float dzo[C::SEM_OUT];
-      Lin::template dx<kHead, C::SEM_OUT, 1>(P.head_w, dlg, dzo);
-      Lin::template dw<kHead, C::SEM_OUT, 1>(sX, sY, zo, dlg, G.head_w, G.head_b);
+      Lin::template grad<kHead, C::SEM_OUT, 1>(P.head_w, sX, sY, zo, dlg, dzo, G.head_w, G.head_b);
       float dz1[C::SEM_H];
       if constexpr (C::SEM_LAYERS == 3) {
         float dz2[C::SEM_H];
-        Lin::template dx<kSem2, C::SEM_H, C::SEM_OUT>(P.sem_w[2], dzo, dz2);
-        Lin::template dw<kSem2, C::SEM_H, C::SEM_OUT>(sX, sY, z2, dzo, G.sem_w[2], G.sem_b[2]);
+        Lin::template grad<kSem2, C::SEM_H, C::SEM_OUT>(P.sem_w[2], sX, sY, z2, dzo, dz2, G.sem_w[2], G.sem_b[2]);
 #pragma unroll
         for (int i = 0; i < C::SEM_H; ++i) dz2[i] = z2[i] > 0.f ? dz2[i] : 0.f;
-        Lin::template dx<kSem1, C::SEM_H, C::SEM_H>(P.sem_w[1], dz2, dz1);
-        Lin::template dw<kSem1, C::SEM_H, C::SEM_H>(sX, sY, z1, dz2, G.sem_w[1], G.sem_b[1]);
+        Lin::template grad<kSem1, C::SEM_H, C::SEM_H>(P.sem_w[1], sX, sY, z1, dz2, dz1, G.sem_w[1], G.sem_b[1]);
       } else {
-        Lin::template dx<kSem1, C::SEM_H, C::SEM_OUT>(P.sem_w[1], dzo, dz1);
-        Lin::template dw<kSem1, C::SEM_H, C::SEM_OUT>(sX, sY, z1, dzo, G.sem_w[1], G.sem_b[1]);
+        Lin::template grad<kSem1, C::SEM_H, C::SEM_OUT>(P.sem_w[1], sX, sY, z1, dzo, dz1, G.sem_w[1], G.sem_b[1]);
       }
 #pragma unroll
       for (int i = 0; i < C::SEM_H; ++i) dz1[i] = z1[i] > 0.f ? dz1[i] : 0.f;
@@ -867,6 +892,9 @@ __global__ void __launch_bounds__(backward_threads<C, TC>()) simt_field_backward
     // ---- colour branch ---------------------------------------------------------------------
     {
       float cin[C::COL_IN], c1[C::COL_H], c2[C::COL_H], o3[3];
+      // the resident kernel loads it here rather than with the point's inputs, so that it is not live through the base
+      // and semantic branches (fewer spills, DESIGN.md section 4.3)
+      if constexpr (kResident) load_appearance(P, F.appearance_mode, cam, s_app, appv);
       colour_fwd<C, Lin>(P, d, geo, appv, cin, c1, c2, o3);
       FNR_PHASE(kPhRecompute);
       float do3[3];
@@ -876,16 +904,13 @@ __global__ void __launch_bounds__(backward_threads<C, TC>()) simt_field_backward
         do3[i] = d_rgb[i] * rgb * (1.0f - rgb);
       }
       float dc2[C::COL_H], dc1[C::COL_H], dcin[C::COL_IN];
-      Lin::template dx<kCol2, C::COL_H, 3>(P.col_w[2], do3, dc2);
-      Lin::template dw<kCol2, C::COL_H, 3>(sX, sY, c2, do3, G.col_w[2], G.col_b[2]);
+      Lin::template grad<kCol2, C::COL_H, 3>(P.col_w[2], sX, sY, c2, do3, dc2, G.col_w[2], G.col_b[2]);
 #pragma unroll
       for (int i = 0; i < C::COL_H; ++i) dc2[i] = c2[i] > 0.f ? dc2[i] : 0.f;
-      Lin::template dx<kCol1, C::COL_H, C::COL_H>(P.col_w[1], dc2, dc1);
-      Lin::template dw<kCol1, C::COL_H, C::COL_H>(sX, sY, c1, dc2, G.col_w[1], G.col_b[1]);
+      Lin::template grad<kCol1, C::COL_H, C::COL_H>(P.col_w[1], sX, sY, c1, dc2, dc1, G.col_w[1], G.col_b[1]);
 #pragma unroll
       for (int i = 0; i < C::COL_H; ++i) dc1[i] = c1[i] > 0.f ? dc1[i] : 0.f;
-      Lin::template dx<kCol0, C::COL_IN, C::COL_H>(P.col_w[0], dc1, dcin);
-      Lin::template dw<kCol0, C::COL_IN, C::COL_H>(sX, sY, cin, dc1, G.col_w[0], G.col_b[0]);
+      Lin::template grad<kCol0, C::COL_IN, C::COL_H>(P.col_w[0], sX, sY, cin, dc1, dcin, G.col_w[0], G.col_b[0]);
 #pragma unroll
       for (int i = 0; i < C::GEO; ++i) d_geo[i] += dcin[C::SH + i];
       // appearance-embedding gradient (only the per-camera rows are parameters of the graph;
@@ -921,12 +946,10 @@ __global__ void __launch_bounds__(backward_threads<C, TC>()) simt_field_backward
 #pragma unroll
       for (int i = 0; i < C::GEO; ++i) dout[1 + i] = d_geo[i];
       float dh1[C::BASE_H];
-      Lin::template dx<kBase1, C::BASE_H, C::BASE_OUT>(P.base_w[1], dout, dh1);
-      Lin::template dw<kBase1, C::BASE_H, C::BASE_OUT>(sX, sY, h1, dout, G.base_w[1], G.base_b[1]);
+      Lin::template grad<kBase1, C::BASE_H, C::BASE_OUT>(P.base_w[1], sX, sY, h1, dout, dh1, G.base_w[1], G.base_b[1]);
 #pragma unroll
       for (int i = 0; i < C::BASE_H; ++i) dh1[i] = h1[i] > 0.f ? dh1[i] : 0.f;
-      Lin::template dx<kBase0, C::ENC, C::BASE_H>(P.base_w[0], dh1, denc);
-      Lin::template dw<kBase0, C::ENC, C::BASE_H>(sX, sY, enc, dh1, G.base_w[0], G.base_b[0]);
+      Lin::template grad<kBase0, C::ENC, C::BASE_H>(P.base_w[0], sX, sY, enc, dh1, denc, G.base_w[0], G.base_b[0]);
     }
     // ---- hash-table gradient -----------------------------------------------------------------
     if constexpr (kResident) {

@@ -9,7 +9,8 @@
 // product ~2^-17 (the rounding of the lo halves), fp32-class for the parity bar of the tests.  The small family's forward,
 // export and backward (CTAs of several warpgroups) split their weights once per CTA into a resident image, and the backward
 // accumulates dW / db in shared memory; the big family's kernels (one warpgroup per CTA) stage the weight tile from global
-// memory at every step.
+// memory at every step.  Where a layer's only consumer is the next layer (resident_chain), its fragments are stored
+// straight into the next layer's operand tile instead of going through rows.
 //
 // Operand layout (no swizzle, core matrices of 8 rows x 16 bytes).  K-major: element (row, k) of a ROWS x KP tile is at
 //     (k / 8) * (ROWS * 16) + row * 16 + (k % 8) * 2
@@ -244,26 +245,146 @@ __device__ __forceinline__ void rowgemm(uint8_t* smem, const float (&x)[R], floa
   read_row<NO>(ys, S::kYStride, 4, y);
 }
 
-// The same GEMM with the weights from a resident split image (W [NPF][KPF] K-major, as rowgemm stages it).  TRANS = false:
-// y = W x (the forward); TRANS = true: y = W^T x (dx), the image read MN-major through the transpose bit.  smem is the
-// warpgroup's kResidentStepBytes.
-template <int NPF, int KPF, bool TRANS, int R, int NO>
-__device__ __forceinline__ void resident_rowgemm(uint8_t* smem, const uint8_t* img, const float (&x)[R], float (&y)[NO]) {
-  constexpr int KP = pad16(R), NP = padn(NO);
-  static_assert(TRANS ? (KP <= NPF && NP <= KPF) : (KP == KPF && NP == NPF), "layer outside the resident image");
-  static_assert(2 * 128 * KP * 2 <= kResidentStepBytes && NP * 128 * 4 <= kResidentStepBytes, "resident step plan");
-  uint8_t* xhi = smem;
-  uint8_t* xlo = smem + 128 * KP * 2;
-  float* ys = reinterpret_cast<float*>(smem);
+// The MMA sequence of layer_mma with both M halves' chains issued back to back into d[0] and d[1], then one wait and one
+// warpgroup barrier: after it, every read of the X tile is done and the tile may be overwritten.  The fragments stay in
+// registers, in layer_mma's fragment order.  Every thread of the warpgroup must call it.
+template <int KP, int NP, int TB>
+__device__ __forceinline__ void layer_mma_frag(uint32_t ax, uint32_t xlo, const BOperand& w, float (&d)[2][NP / 2]) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int i = 0; i < NP / 2; ++i) d[h][i] = 0.f;
+  fence_operands();
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+#pragma unroll
+    for (int ks = 0; ks < KP / 16; ++ks) {
+      const uint32_t xa = ax + ks * 2 * (128 * 16) + h * 64 * 16, wa = w.hi + ks * w.kstep;
+      const uint64_t dxh = desc(xa, 128 * 16, 128), dxl = desc(xa + xlo, 128 * 16, 128);
+      const uint64_t dwh = desc(wa, w.lbo, w.sbo), dwl = desc(wa + w.lo, w.lbo, w.sbo);
+      mma_m64k16<NP, 0, TB>(d[h], dxh, dwh, ks > 0);
+      mma_m64k16<NP, 0, TB>(d[h], dxl, dwh, 1);
+      mma_m64k16<NP, 0, TB>(d[h], dxh, dwl, 1);
+      mma_m64k16<NP, 0, TB>(d[h], dxl, dwl, 1);
+    }
+  }
+  commit();
+  wait_all();
+  sync();
+}
+
+// stmatrix of four 8 x 8 b16 matrices: lane l gives the address of row l % 8 of matrix l / 8 (16 contiguous bytes), and
+// register m holds the lane's elements (row lane / 4, columns 2 (lane % 4) and + 1) of matrix m, the first in the low half.
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3])
+               : "memory");
+}
+
+// The fragments of layer_mma_frag (NP columns) as the next layer's K-major A tile of K = NP at `tile` (lo 128 * NP * 2 bytes
+// further), split hi / lo per element as split_store8 splits a row, so the bytes are the ones split_store_chunk would write
+// from the same values.  An m64nN accumulator fragment has the layout of stmatrix.m8n8: the warp's rows 16 warp + [0, 8) and
+// + [8, 16) of k chunks i and i + 1 are four core matrices, one x4 store into hi and one into lo.
+template <int NP>
+__device__ __forceinline__ void store_a_tile(uint32_t tile, const float (&d)[2][NP / 2]) {
+  const int t = tid(), warp = t >> 5, lane = t & 31, m = lane >> 3;
+  constexpr uint32_t LO = 128 * NP * 2;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    // matrix m: k chunk i + m / 2, rows + 8 (m % 2); its fragment values are d[h][4 (i + m / 2) + 2 (m % 2) + {0, 1}]
+    const uint32_t row = h * 64 + 16 * warp + 8 * (m & 1) + (lane & 7);
+#pragma unroll
+    for (int i = 0; i < NP / 8; i += 2) {
+      uint32_t hr[4], lr[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const float v0 = d[h][4 * (i + q / 2) + 2 * (q & 1)], v1 = d[h][4 * (i + q / 2) + 2 * (q & 1) + 1];
+        const __nv_bfloat162 hv = __floats2bfloat162_rn(v0, v1);
+        const float2 hf = __bfloat1622float2(hv);
+        const __nv_bfloat162 lv = __floats2bfloat162_rn(v0 - hf.x, v1 - hf.y);
+        hr[q] = *reinterpret_cast<const uint32_t*>(&hv);
+        lr[q] = *reinterpret_cast<const uint32_t*>(&lv);
+      }
+      const uint32_t a = tile + (i + (m >> 1)) * (128 * 16) + row * 16;
+      stmatrix_x4(a, hr);
+      stmatrix_x4(a + LO, lr);
+    }
+  }
+}
+
+// The resident image's B operand of slot image `img` (W [NPF][KPF] K-major): read K-major for y = W x, MN-major through
+// the transpose bit for y = W^T x.
+template <int NPF, int KPF, bool TRANS>
+__device__ __forceinline__ BOperand image_operand(const uint8_t* img) {
+  const uint32_t iw = smem_u32(img), lo = NPF * KPF * 2;
+  return TRANS ? BOperand{iw, lo, 128, NPF * 16, 2 * 128} : BOperand{iw, lo, NPF * 16, 128, 2 * NPF * 16};
+}
+
+// The row tile of a resident step: every thread splits its row x[R] into the warpgroup's K-major X tile, after the
+// previous step's readers are done with it.
+template <int R>
+__device__ __forceinline__ void stage_rows(uint8_t* smem, const float (&x)[R]) {
+  constexpr int KP = pad16(R);
   const int t = tid();
   sync();  // the previous step's readers are done with the tile
 #pragma unroll
-  for (int kc = 0; kc < KP / 8; ++kc) split_store_chunk(xhi, xlo, kc * (128 * 16) + t * 16, x, kc);
+  for (int kc = 0; kc < KP / 8; ++kc) split_store_chunk(smem, smem + 128 * KP * 2, kc * (128 * 16) + t * 16, x, kc);
   fence_proxy_async();
   sync();
-  const uint32_t iw = smem_u32(img), lo = NPF * KPF * 2;
-  const BOperand w = TRANS ? BOperand{iw, lo, 128, NPF * 16, 2 * 128} : BOperand{iw, lo, NPF * 16, 128, 2 * NPF * 16};
-  layer_mma<KP, NP, TRANS ? 1 : 0, true>(smem_u32(xhi), 128 * KP * 2, w, ys, 4, kRowsGroupStride);
+}
+
+// The same GEMM with the weights from a resident split image (W [NPF][KPF] K-major, as rowgemm stages it), y = W^T x
+// (dx): the image read MN-major through the transpose bit.  smem is the warpgroup's kResidentStepBytes.
+template <int NPF, int KPF, int R, int NO>
+__device__ __forceinline__ void resident_rowgemm_t(uint8_t* smem, const uint8_t* img, const float (&x)[R], float (&y)[NO]) {
+  constexpr int KP = pad16(R), NP = padn(NO);
+  static_assert(KP <= NPF && NP <= KPF, "layer outside the resident image");
+  static_assert(2 * 128 * KP * 2 <= kResidentStepBytes && NP * 128 * 4 <= kResidentStepBytes, "resident step plan");
+  float* ys = reinterpret_cast<float*>(smem);
+  stage_rows(smem, x);
+  layer_mma<KP, NP, 1, true>(smem_u32(smem), 128 * KP * 2, image_operand<NPF, KPF, true>(img), ys, 4, kRowsGroupStride);
+  sync();
+  read_row<NO>(ys, 4, kRowsGroupStride, y);
+}
+
+// Two forward layers chained fragment to fragment: m = epi0(W0 x), y = W1 m (before its bias), both weights from the
+// resident image (img0: W0 [NPF0][KPF0], img1: W1 [NPF1][NPF0]).  The first layer's MMAs end in registers (both M halves
+// in flight); epi0(c, v) (column c of value v: the bias and ReLU) runs on them in fragment order, and they are stored as
+// the second layer's A tile in place of the first's, split hi / lo.  Only the second layer's result goes back to rows.
+// KEEP_MID (the backward, whose weight gradients and ReLU masks read m as rows): the first layer runs the row path
+// instead, one M half at a time, with epi0 on the rows and m staged from them; its 64 live accumulators would add to the
+// backward's spills (DESIGN.md section 4.3).  Both give the same bytes in the second layer's tile.  smem is the
+// warpgroup's kResidentStepBytes.
+template <int NPF0, int KPF0, int NPF1, bool KEEP_MID, int R, int NM, int NO, class Epi>
+__device__ __forceinline__ void resident_chain(uint8_t* smem, const uint8_t* img0, const uint8_t* img1, const float (&x)[R],
+                                               float (&mid)[NM], float (&y)[NO], Epi epi0) {
+  constexpr int KP = pad16(R), NP = padn(NO);
+  static_assert(KP == KPF0 && NM == NPF0 && NP == NPF1, "layers outside the resident image");
+  static_assert(2 * 128 * NM * 2 <= kResidentStepBytes && 2 * 128 * KP * 2 <= kResidentStepBytes && NM * 128 * 4 <= kResidentStepBytes,
+                "resident step plan");
+  const uint32_t tile = smem_u32(smem);
+  float* ys = reinterpret_cast<float*>(smem);
+  stage_rows(smem, x);
+  if constexpr (KEEP_MID) {
+    layer_mma<KP, NM, 0, true>(tile, 128 * KP * 2, image_operand<NPF0, KPF0, false>(img0), ys, 4, kRowsGroupStride);
+    sync();
+    read_row<NM>(ys, 4, kRowsGroupStride, mid);
+#pragma unroll
+    for (int n = 0; n < NM; ++n) mid[n] = epi0(n, mid[n]);
+    stage_rows(smem, mid);
+  } else {
+    const int lane = tid() & 31;
+    float d[2][NM / 2];
+    layer_mma_frag<KP, NM, 0>(tile, 128 * KP * 2, image_operand<NPF0, KPF0, false>(img0), d);
+    // fragment (i, j): column 8 i + 2 (lane % 4) + (j & 1)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int e = 0; e < NM / 2; ++e) d[h][e] = epi0(8 * (e / 4) + 2 * (lane & 3) + (e & 1), d[h][e]);
+    store_a_tile<NM>(tile, d);
+    fence_proxy_async();
+    sync();
+  }
+  layer_mma<NM, NP, 0, true>(tile, 128 * NM * 2, image_operand<NPF1, NM, false>(img1), ys, 4, kRowsGroupStride);
   sync();
   read_row<NO>(ys, 4, kRowsGroupStride, y);
 }
