@@ -62,16 +62,19 @@ def count_fruits(points: np.ndarray, eps: float, min_samples: int, cluster_merge
 
     With ``template`` (a [m,3] fruit point cloud, see ``load_template``) stage 3 runs on the merged groups and the result
     also holds 'count_after_merge' (the stage-2 count), 'num_split_extra' and 'num_pruned'; 'count' and 'centers' are then
-    the stage-3 values.  ``seed`` selects the hashed surface samples of ``alpha_shape``."""
+    the stage-3 values.  ``seed`` selects the hashed surface samples of ``alpha_shape``.
+
+    On a CUDA tensor this is ``count_sweep`` with one config."""
     if _on_device(points):
-        return _device_count_fruits(points, eps, min_samples, cluster_merge_distance, down_sample, remove_outliers_nb_points,
-                                    remove_outliers_radius, template, seed)
+        config = dict(eps=eps, min_samples=min_samples, cluster_merge_distance=cluster_merge_distance, down_sample=down_sample,
+                      remove_outliers_nb_points=remove_outliers_nb_points, remove_outliers_radius=remove_outliers_radius, seed=seed)
+        return _device_count_sweep(points, [config], [template], lambda stage: None)[0]
     pts = np.asarray(points, dtype=np.float64).reshape(-1, 3)
     if remove_outliers_nb_points > 0 and remove_outliers_radius > 0:
         pts = remove_radius_outliers(pts, remove_outliers_nb_points, remove_outliers_radius)
     pts = voxel_down_sample(pts, down_sample)
     if pts.shape[0] == 0:
-        return _with_stage3({"count": 0, "count_before_merge": 0, "centers": np.zeros((0, 3)), "num_points": 0}, [], template, seed, None)
+        return _with_stage3({"count": 0, "count_before_merge": 0, "centers": np.zeros((0, 3)), "num_points": 0}, [], template, seed)
     labels = DBSCAN(eps=eps, min_samples=min_samples, n_jobs=-1).fit(pts).labels_
     centers, members = [], []
     first_stage = 0
@@ -92,14 +95,18 @@ def count_fruits(points: np.ndarray, eps: float, min_samples: int, cluster_merge
         members.append(cluster)
     res = {"count": len(centers), "count_before_merge": first_stage, "centers": np.vstack(centers) if centers else np.zeros((0, 3)),
            "num_points": int(pts.shape[0])}
-    return _with_stage3(res, members, template, seed, None)
+    return _with_stage3(res, members, template, seed)
 
 
-def _with_stage3(res: Dict, groups: List[np.ndarray], template, seed: int, device) -> Dict:
+def _with_stage3(res: Dict, groups: List[np.ndarray], template, seed: int) -> Dict:
     """Stage 3 on the merged ``groups`` when a template is given; ``res`` unchanged otherwise."""
     if template is None:
         return res
-    split = split_clusters(groups, template, seed=seed, device=device)
+    return _with_split(res, split_clusters(groups, template, seed=seed, device=None))
+
+
+def _with_split(res: Dict, split: Dict) -> Dict:
+    """The stage-2 result ``res`` after stage 3, ``split`` being what ``split_clusters`` returned for its groups."""
     return {**res, "count_after_merge": res["count"], "count": res["count"] + split["num_split_extra"] - split["num_pruned"],
             "num_split_extra": split["num_split_extra"], "num_pruned": split["num_pruned"], "centers": split["centers"]}
 
@@ -112,24 +119,6 @@ def _device_remove_radius_outliers(points, nb_points: int, radius: float):
         return pts
     counts = ops.radius_count(pts, radius, cap=nb_points + 1)  # nb_points neighbours + the point itself
     return pts[counts - 1 >= nb_points]
-
-
-def _device_count_fruits(points, eps: float, min_samples: int, cluster_merge_distance: float, down_sample: float,
-                         remove_outliers_nb_points: int, remove_outliers_radius: float, template=None, seed: int = 0) -> Dict:
-    pts = ops.cluster_points(points)
-    if remove_outliers_nb_points > 0 and remove_outliers_radius > 0:
-        pts = _device_remove_radius_outliers(pts, remove_outliers_nb_points, remove_outliers_radius)
-    pts = ops.voxel_down_sample(pts, down_sample)
-    if pts.shape[0] == 0:
-        return _with_stage3({"count": 0, "count_before_merge": 0, "centers": np.zeros((0, 3)), "num_points": 0}, [], template, seed,
-                            pts.device)
-    labels, k = ops.dbscan(pts, eps, min_samples)
-    sums, counts = ops.cluster_sums(pts, labels, k)
-    res, group_of = _merge_groups(sums.cpu().numpy(), counts.cpu().numpy(), cluster_merge_distance)
-    res["num_points"] = int(pts.shape[0])
-    if template is None:
-        return res
-    return _with_stage3(res, _device_groups(pts, labels, group_of), template, seed, pts.device)
 
 
 def _device_groups(pts, labels, group_of: np.ndarray) -> List[np.ndarray]:
@@ -474,44 +463,107 @@ def hausdorff(a: np.ndarray, b: np.ndarray) -> float:
     return float(np.sqrt(max(directed2(a, b), directed2(b, a))))
 
 
+def _decide(vt: float, volume: float, sample: Optional[np.ndarray]) -> str:
+    """'split', 'prune' or 'one' for a group of alpha = 10 volume ``volume`` and surface ``sample``, the template's
+    volume being ``vt`` (clustering_base.py:372, :422)."""
+    if sample is None:  # empty alpha = 100 boundary: nothing to sample, the group counts as one fruit
+        return "one"
+    if vt < SPLIT_RATIO * volume:
+        return "split"
+    return "prune" if PRUNE_RATIO * vt > abs(volume) else "one"
+
+
+def _alpha(jobs) -> Tuple[List[Tuple[List[str], Dict[int, tuple]]], Dict[tuple, np.ndarray]]:
+    """The host half of stage 3 for every job (groups, template [m,3] float64, seed).  The template volume is computed
+    once per template, the alpha shapes once per group content and the surface sample once per (content, seed, group
+    index), since the sample's hash includes the group index.  Returns, per job, (decisions [G], {group to split: sample
+    key}) and the samples {sample key: [SURFACE_SAMPLES,3]}."""
+    template_vol, shapes, samples, plans = {}, {}, {}, []  # template bytes -> V_t; content -> (V, boundary)
+    for groups, tmpl, seed in jobs:
+        tkey = tmpl.tobytes()
+        if tkey not in template_vol:
+            template_vol[tkey] = float(alpha_shape(tmpl, (ALPHA_VOLUME,))[0][0])
+        decisions, picks = [], {}
+        for g, grp in enumerate(groups):
+            p64 = np.asarray(grp, dtype=np.float64).reshape(-1, 3)
+            content = (p64.shape[0], p64.tobytes())
+            skey = (content, seed, g)
+            if content not in shapes:
+                volumes, boundaries, samples[skey] = alpha_shape(p64, (ALPHA_VOLUME, ALPHA_SURFACE), seed=seed, group=g)
+                shapes[content] = (volumes[0], boundaries[-1])
+            elif skey not in samples:
+                samples[skey] = _surface_sample(p64, shapes[content][1], SURFACE_SAMPLES, seed, g)
+            decisions.append(_decide(template_vol[tkey], shapes[content][0], samples[skey]))
+            if decisions[-1] == "split":
+                picks[g] = skey
+        plans.append((decisions, picks))
+    return plans, samples
+
+
 def alpha_stage(groups: Sequence[np.ndarray], template: np.ndarray, seed: int = 0):
     """The host half of stage 3 (clustering_base.py:350-429): per group 'one', 'prune' or 'split' and, for each group
     to split, its surface sample.  Returns (decisions [G], samples {group: [SURFACE_SAMPLES,3]})."""
-    vt = float(alpha_shape(template, (ALPHA_VOLUME,))[0][0])
-    decisions, samples = [], {}
-    for g, pts in enumerate(groups):
-        volumes, _, sample = alpha_shape(pts, (ALPHA_VOLUME, ALPHA_SURFACE), seed=seed, group=g)
-        if sample is None:  # empty alpha = 100 boundary: nothing to sample, the group counts as one fruit
-            decisions.append("one")
-        elif vt < SPLIT_RATIO * volumes[0]:
-            decisions.append("split")
-            samples[g] = sample
-        elif PRUNE_RATIO * vt > abs(volumes[0]):
-            decisions.append("prune")
-        else:
-            decisions.append("one")
-    return decisions, samples
+    plans, samples = _alpha([(groups, np.asarray(template, dtype=np.float64), seed)])
+    decisions, picks = plans[0]
+    return decisions, {g: samples[k] for g, k in picks.items()}
 
 
 def match_candidates(samples: Sequence[np.ndarray], template: np.ndarray, device=None):
     """ICP (k = 1), Ward sub-centres (k = 2..6) and the six Hausdorff distances of each surface sample.  Returns
     (T [B,4,4], sub-centres [B,20,3], distances [B,6], ICP iterations [B]) as numpy arrays; ``device`` (a CUDA device)
     runs one launch of each kernel over all samples, None the numpy code."""
-    B = len(samples)
-    if B == 0:
+    return _match(list(samples), [(np.asarray(template, dtype=np.float64), list(range(len(samples))))], device)
+
+
+def _match(samples: List[np.ndarray], fits: List[Tuple[np.ndarray, List[int]]], device):
+    """``match_candidates`` for several templates: ``fits`` holds (template [m,3] float64, the indices of the samples it
+    is fitted to) per template.  Returns (T [P,4,4], sub-centres [S,20,3], distances [P,6], ICP iterations [P]): the
+    sub-centres of each sample, the rest for the P (template, sample) pairs in the order of ``fits``.  ``device`` runs
+    one ICP launch per template, one Ward launch over all samples and one Hausdorff launch over all pairs."""
+    if not samples:
         return np.zeros((0, 4, 4)), np.zeros((0, 20, 3)), np.zeros((0, MAX_FRUIT_PER_GROUP)), np.zeros(0, dtype=np.int64)
-    tmpl = np.asarray(template, dtype=np.float64)
-    inits = np.stack([_translation(s.mean(axis=0)) for s in samples])
-    if device is not None:
-        return _device_match(samples, tmpl, inits, device)
-    T, cuts, its = np.zeros((B, 4, 4)), np.zeros((B, 20, 3)), np.zeros(B, dtype=np.int64)
-    d = np.zeros((B, MAX_FRUIT_PER_GROUP))
-    for i, s in enumerate(samples):
-        T[i], _, _, its[i] = icp_scaled(tmpl, s, inits[i])
-        cuts[i] = ward_cut_centres(s)
-        for j, copies in enumerate(_template_copies(tmpl, T[i], cuts[i])):
-            d[i, j] = hausdorff(s, copies)
-    return T, cuts, d, its
+    inits = [s.mean(axis=0) for s in samples]  # ICP starts from a translation to the sample's mean
+    if device is None:
+        cuts = np.stack([ward_cut_centres(s) for s in samples])
+        T, d, its = [], [], []
+        for tmpl, rows in fits:
+            for j in rows:
+                Tj, _, _, it = icp_scaled(tmpl, samples[j], _translation(inits[j]))
+                T.append(Tj)
+                its.append(it)
+                d.append([hausdorff(samples[j], copies) for copies in _template_copies(tmpl, Tj, cuts[j])])
+        return np.stack(T), cuts, np.array(d), np.array(its, dtype=np.int64)
+    f64 = dict(dtype=torch.float64, device=device)
+    offsets = _offsets(samples)
+    targets = torch.from_numpy(np.concatenate(samples)).to(**f64)
+    cuts = ops.ward_cut(targets, offsets)
+    T, its, hyp, a_ranges = [], [], [], []
+    for tmpl, rows in fits:
+        t = torch.from_numpy(tmpl).to(**f64)
+        sub = [samples[j] for j in rows]
+        Tt, _, _, it = ops.icp_scaled(t, torch.from_numpy(np.concatenate(sub)).to(**f64), _offsets(sub),
+                                      torch.from_numpy(np.stack([inits[j] for j in rows])).to(**f64))
+        # the six hypotheses of every sample as segments of one array, in the order (sample, k)
+        x, y, z = t[:, 0], t[:, 1], t[:, 2]
+        R = Tt[:, :3, :]
+        fitted = torch.stack([((R[:, r, 0:1] * x + R[:, r, 1:2] * y) + R[:, r, 2:3] * z) + R[:, r, 3:4] for r in range(3)], dim=2)
+        for b, j in enumerate(rows):
+            hyp.append(fitted[b])
+            for k in range(2, MAX_FRUIT_PER_GROUP + 1):
+                centres = cuts[j, CUT_OFFSETS[k - 2]:CUT_OFFSETS[k - 1]]
+                hyp.append((t[None, :, :] + centres[:, None, :]).reshape(-1, 3))
+            a_ranges += [offsets[j:j + 2]] * MAX_FRUIT_PER_GROUP
+        T.append(Tt)
+        its.append(it)
+    b_offsets = _offsets(hyp)
+    d = ops.hausdorff(targets, np.stack(a_ranges), torch.cat(hyp), np.stack([b_offsets[:-1], b_offsets[1:]], axis=1))
+    return (torch.cat(T).cpu().numpy(), cuts.cpu().numpy(), d.view(-1, MAX_FRUIT_PER_GROUP).cpu().numpy(),
+            torch.cat(its).cpu().numpy().astype(np.int64))
+
+
+def _offsets(segments) -> np.ndarray:
+    """Ascending int64 offsets [len + 1] of consecutive segments (arrays or tensors) of one concatenation."""
+    return np.concatenate([[0], np.cumsum([s.shape[0] for s in segments], dtype=np.int64)])
 
 
 def _translation(t) -> np.ndarray:
@@ -529,31 +581,24 @@ def _template_copies(tmpl: np.ndarray, T: np.ndarray, cuts: np.ndarray) -> List[
     return out
 
 
-def _device_match(samples, tmpl: np.ndarray, inits: np.ndarray, device):
-    import torch
-
-    f64 = dict(dtype=torch.float64, device=device)
-    offsets = np.concatenate([[0], np.cumsum([s.shape[0] for s in samples])])
-    targets = torch.from_numpy(np.concatenate(samples)).to(**f64)
-    t = torch.from_numpy(tmpl).to(**f64)
-    T, _, _, its = ops.icp_scaled(t, targets, offsets, torch.from_numpy(inits[:, :3, 3].copy()).to(**f64))
-    cuts = ops.ward_cut(targets, offsets)
-    # the six hypotheses of every sample as segments of one array, in the order (sample, k)
-    x, y, z = t[:, 0], t[:, 1], t[:, 2]
-    R = T[:, :3, :]
-    fitted = torch.stack([((R[:, r, 0:1] * x + R[:, r, 1:2] * y) + R[:, r, 2:3] * z) + R[:, r, 3:4] for r in range(3)], dim=2)
-    hyp, sizes = [], []
-    for i in range(len(samples)):
-        hyp.append(fitted[i])
-        sizes.append(t.shape[0])
-        for k in range(2, MAX_FRUIT_PER_GROUP + 1):
-            centres = cuts[i, CUT_OFFSETS[k - 2]:CUT_OFFSETS[k - 1]]
-            hyp.append((t[None, :, :] + centres[:, None, :]).reshape(-1, 3))
-            sizes.append(k * t.shape[0])
-    b_offsets = np.concatenate([[0], np.cumsum(sizes)])
-    a_ranges = np.repeat(np.stack([offsets[:-1], offsets[1:]], axis=1), MAX_FRUIT_PER_GROUP, axis=0)
-    d = ops.hausdorff(targets, a_ranges, torch.cat(hyp), np.stack([b_offsets[:-1], b_offsets[1:]], axis=1))
-    return (T.cpu().numpy(), cuts.cpu().numpy(), d.view(-1, MAX_FRUIT_PER_GROUP).cpu().numpy(), its.cpu().numpy().astype(np.int64))
+def _assemble(groups: Sequence[np.ndarray], tmpl: np.ndarray, decisions: List[str], matched: Dict[int, tuple]) -> Dict:
+    """``split_clusters``' result from the decisions of the alpha stage and the match of each group to split:
+    ``matched`` {group: (T [4,4], sub-centres [20,3], distances [6], ICP iterations)}."""
+    centers, per_group, its = [], np.zeros(len(groups), dtype=np.int64), []
+    for g, (pts, dec) in enumerate(zip(groups, decisions)):
+        if dec == "one":
+            centers.append(np.asarray(pts, dtype=np.float64).mean(axis=0)[None])
+            per_group[g] = 1
+        elif dec == "split":
+            T, cuts, d, it = matched[g]
+            k = int(np.argmin(d)) + 1
+            per_group[g] = k
+            centers.append(transform_points(tmpl, T).mean(axis=0)[None] if k == 1 else cuts[CUT_OFFSETS[k - 2]:CUT_OFFSETS[k - 1]])
+            its.append(it)
+    split = per_group[np.array([dec == "split" for dec in decisions], dtype=bool)]
+    return {"centers": np.concatenate(centers) if centers else np.zeros((0, 3)), "fruit_per_group": per_group,
+            "num_split_extra": int((split - 1).sum()), "num_pruned": int(sum(dec == "prune" for dec in decisions)),
+            "icp_iterations": np.array(its, dtype=np.int64)}
 
 
 def split_clusters(groups: Sequence[np.ndarray], template: np.ndarray, seed: int = 0, device=None) -> Dict:
@@ -565,28 +610,30 @@ def split_clusters(groups: Sequence[np.ndarray], template: np.ndarray, seed: int
     pruned, and any other group is one fruit centred at its mean.  Returns {'centers' [m,3], 'fruit_per_group' [G]
     (0 = pruned), 'num_split_extra', 'num_pruned', 'icp_iterations' (per split group)}; ``device`` as in
     ``match_candidates``."""
-    decisions, samples = alpha_stage(groups, template, seed)
-    cand = sorted(samples)
-    T, cuts, d, its = match_candidates([samples[g] for g in cand], template, device)
-    tmpl = np.asarray(template, dtype=np.float64)
-    centers, per_group = [], np.zeros(len(groups), dtype=np.int64)
-    pos = {g: i for i, g in enumerate(cand)}
-    for g, (pts, dec) in enumerate(zip(groups, decisions)):
-        if dec == "one":
-            centers.append(np.asarray(pts, dtype=np.float64).mean(axis=0)[None])
-            per_group[g] = 1
-        elif dec == "split":
-            i = pos[g]
-            k = int(np.argmin(d[i])) + 1
-            per_group[g] = k
-            if k == 1:
-                centers.append(transform_points(tmpl, T[i]).mean(axis=0)[None])
-            else:
-                centers.append(cuts[i, CUT_OFFSETS[k - 2]:CUT_OFFSETS[k - 1]])
-    split = per_group[np.array([dec == "split" for dec in decisions], dtype=bool)]
-    return {"centers": np.concatenate(centers) if centers else np.zeros((0, 3)), "fruit_per_group": per_group,
-            "num_split_extra": int((split - 1).sum()), "num_pruned": int(sum(dec == "prune" for dec in decisions)),
-            "icp_iterations": its}
+    return _stage3([(groups, np.asarray(template, dtype=np.float64), seed)], device)[0]
+
+
+def _stage3(jobs, device, on_stage: Callable[[str], None] = lambda stage: None) -> List[Dict]:
+    """``split_clusters`` for every job (groups, template [m,3] float64, seed), sharing the host work of ``_alpha`` and
+    the launches of ``_match`` between the jobs.  ``on_stage`` is called with 'alpha' and 'match' as they end."""
+    plans, samples = _alpha(jobs)
+    on_stage("alpha")
+    keys = list(dict.fromkeys(k for _, picks in plans for k in picks.values()))  # the distinct samples to split
+    row = {k: j for j, k in enumerate(keys)}
+    fits: Dict[bytes, Tuple[np.ndarray, Dict[int, None]]] = {}  # template bytes -> (template, rows fitted to it), in first use
+    for (_, tmpl, _), (_, picks) in zip(jobs, plans):
+        fits.setdefault(tmpl.tobytes(), (tmpl, {}))[1].update(dict.fromkeys(row[k] for k in picks.values()))
+    pair = {p: i for i, p in enumerate((tkey, j) for tkey, (_, rows) in fits.items() for j in rows)}
+    T, cuts, d, its = _match([samples[k] for k in keys], [(tmpl, list(rows)) for tmpl, rows in fits.values() if rows], device)
+    on_stage("match")
+    out = []
+    for (groups, tmpl, _), (decisions, picks) in zip(jobs, plans):
+        matched = {}
+        for g, k in picks.items():
+            i = pair[(tmpl.tobytes(), row[k])]
+            matched[g] = (T[i], cuts[row[k]], d[i], its[i])
+        out.append(_assemble(groups, tmpl, decisions, matched))
+    return out
 
 
 def load_obj_centres(path) -> np.ndarray:
@@ -683,8 +730,9 @@ def count_sweep(points, configs: Sequence[Dict], templates: Optional[Sequence[Op
     returns alone.  ``configs``: dicts of count_fruits' keyword arguments (``COUNT_ARGS``); ``templates``: one fruit
     template (or None: no stage 3) per config, all None when omitted.
 
-    numpy input runs that loop.  A CUDA tensor shares the work the configs have in common: the radius counts of each
-    distinct outlier radius (one multi-radius walk, cap = the largest nb_points + 1), the voxel down-sampling of each
+    numpy input runs that loop; on a CUDA tensor ``count_fruits`` is this function with one config.  A CUDA tensor
+    shares the work the configs have in common: the radius counts of each distinct outlier radius (one walk per run
+    of radii ``_radius_chunks`` makes, cap = the largest nb_points + 1), the voxel down-sampling of each
     distinct filtered set, DBSCAN once per distinct (set, eps, min_samples), stage 2 once per distinct (set, eps,
     min_samples, merge distance); stage 3's alpha shapes once per group content, its surface sample
     once per (content, seed, group index), and one ICP launch per template, one Ward launch over every distinct sample
@@ -717,14 +765,10 @@ def _radius_chunks(values: Sequence) -> List[List]:
 
 def _device_count_sweep(points, configs: List[Dict], templates: List, on_stage) -> List[Dict]:
     pts = ops.cluster_points(points)
-    if pts.shape[0] == 0:
-        return [_device_count_fruits(pts, c["eps"], c["min_samples"], c["cluster_merge_distance"], c["down_sample"],
-                                     c["remove_outliers_nb_points"], c["remove_outliers_radius"], t, c["seed"])
-                for c, t in zip(configs, templates)]
 
-    def outlier_key(c):  # None: no outlier removal
+    def outlier_key(c):  # None: no outlier removal (an empty cloud has no outliers to count)
         nb, r = c["remove_outliers_nb_points"], c["remove_outliers_radius"]
-        return (int(nb), float(r)) if nb > 0 and r > 0 else None
+        return (int(nb), float(r)) if nb > 0 and r > 0 and pts.shape[0] else None
 
     # radius counts: each distinct radius once, saturated at the largest nb_points + 1 it is used with
     caps: Dict[float, int] = {}
@@ -734,8 +778,10 @@ def _device_count_sweep(points, configs: List[Dict], templates: List, on_stage) 
             caps[k[1]] = max(caps.get(k[1], 0), k[0] + 1)
     counts = {}
     for chunk in _radius_chunks(list(caps)):
-        rows = ops.radius_count_multi(pts, chunk, [caps[r] for r in chunk])
-        counts.update({r: rows[i] for i, r in enumerate(chunk)})
+        if len(chunk) == 1:  # fnr_radius_count: bit-equal to a one-radius fnr_radius_count_multi, and its errors name it
+            counts[chunk[0]] = ops.radius_count(pts, chunk[0], caps[chunk[0]])
+        else:
+            counts.update(zip(chunk, ops.radius_count_multi(pts, chunk, [caps[r] for r in chunk])))
     filtered = {None: pts}
     for c in configs:
         k = outlier_key(c)
@@ -780,111 +826,8 @@ def _device_count_sweep(points, configs: List[Dict], templates: List, on_stage) 
             continue
         if entry[2] is None:
             entry[2] = _device_groups(*entry[1])
-        jobs.append((i, entry[0], entry[2], np.asarray(t, dtype=np.float64), int(c["seed"])))
+        jobs.append((i, entry[0], (entry[2], np.asarray(t, dtype=np.float64), int(c["seed"]))))
     on_stage("merge")
-    if jobs:
-        for i, res in _sweep_stage3(jobs, pts.device, on_stage):
-            results[i] = res
-    else:
-        on_stage("alpha")
-        on_stage("match")
+    for (i, res, _), split in zip(jobs, _stage3([job for _, _, job in jobs], pts.device, on_stage)):
+        results[i] = _with_split(res, split)
     return results
-
-
-def _sweep_stage3(jobs, device, on_stage):
-    """``_with_stage3`` for every job (index, stage-2 result, groups, template, seed), sharing the alpha shapes, the
-    surface samples and the device launches between the jobs.  Yields (index, result)."""
-    template_vol, shapes, samples = {}, {}, {}  # template bytes -> V_t; content -> (volumes, boundary); (content, seed, g) -> sample
-    plans = []
-    for i, res, groups, tmpl, seed in jobs:
-        tkey = tmpl.tobytes()
-        if tkey not in template_vol:
-            template_vol[tkey] = float(alpha_shape(tmpl, (ALPHA_VOLUME,))[0][0])
-        vt = template_vol[tkey]
-        decisions, picks = [], {}
-        for g, grp in enumerate(groups):
-            p64 = np.asarray(grp, dtype=np.float64).reshape(-1, 3)
-            content = (p64.shape[0], p64.tobytes())
-            skey = (content, seed, g)
-            if content not in shapes:
-                volumes, boundaries, sample = alpha_shape(p64, (ALPHA_VOLUME, ALPHA_SURFACE), seed=seed, group=g)
-                shapes[content] = (volumes, boundaries[-1])
-                samples[skey] = sample
-            elif skey not in samples:
-                samples[skey] = _surface_sample(p64, shapes[content][1], SURFACE_SAMPLES, seed, g)
-            volumes, sample = shapes[content][0], samples[skey]
-            if sample is None:  # as alpha_stage
-                decisions.append("one")
-            elif vt < SPLIT_RATIO * volumes[0]:
-                decisions.append("split")
-                picks[g] = skey
-            elif PRUNE_RATIO * vt > abs(volumes[0]):
-                decisions.append("prune")
-            else:
-                decisions.append("one")
-        plans.append((i, res, groups, tmpl, tkey, decisions, picks))
-    on_stage("alpha")
-
-    # the distinct samples to split (Ward: template-free) and, per template, the samples it is fitted to (ICP)
-    sample_keys = list(dict.fromkeys(k for p in plans for _, k in sorted(p[6].items())))
-    per_template: Dict[bytes, Tuple[np.ndarray, Dict]] = {}  # template -> (template, {sample key: None}), in first-use order
-    for p in plans:
-        per_template.setdefault(p[4], (p[3], {}))[1].update(dict.fromkeys(k for _, k in sorted(p[6].items())))
-    matched = _device_match_sweep([samples[k] for k in sample_keys], sample_keys, per_template, device) if sample_keys else {}
-    on_stage("match")
-
-    for i, res, groups, tmpl, tkey, decisions, picks in plans:
-        centers, per_group = [], np.zeros(len(groups), dtype=np.int64)
-        for g, (grp, dec) in enumerate(zip(groups, decisions)):  # split_clusters' assembly
-            if dec == "one":
-                centers.append(np.asarray(grp, dtype=np.float64).mean(axis=0)[None])
-                per_group[g] = 1
-            elif dec == "split":
-                T, cuts, d = matched[(tkey, picks[g])]
-                k = int(np.argmin(d)) + 1
-                per_group[g] = k
-                centers.append(transform_points(tmpl, T).mean(axis=0)[None] if k == 1 else cuts[CUT_OFFSETS[k - 2]:CUT_OFFSETS[k - 1]])
-        split = per_group[np.array([dec == "split" for dec in decisions], dtype=bool)]
-        extra, pruned = int((split - 1).sum()), int(sum(dec == "prune" for dec in decisions))
-        yield i, {**res, "count_after_merge": res["count"], "count": res["count"] + extra - pruned, "num_split_extra": extra,
-                  "num_pruned": pruned, "centers": np.concatenate(centers) if centers else np.zeros((0, 3))}
-
-
-def _device_match_sweep(sample_list: List[np.ndarray], sample_keys: List, per_template: Dict, device) -> Dict:
-    """``_device_match`` over several templates: one ICP launch per template on the samples it is fitted to, one Ward
-    launch over all samples, one Hausdorff launch over every (template, sample) pair.  ``per_template``: {template key:
-    (template, ordered sample keys)}.  Returns {(template key, sample
-    key): (T [4,4], sub-centres [20,3], distances [6])}."""
-    f64 = dict(dtype=torch.float64, device=device)
-    offsets = np.concatenate([[0], np.cumsum([s.shape[0] for s in sample_list])])
-    row = {k: j for j, k in enumerate(sample_keys)}
-    targets = torch.from_numpy(np.concatenate(sample_list)).to(**f64)
-    cuts = ops.ward_cut(targets, offsets)
-    fits, hyp, sizes, a_ranges, pairs = {}, [], [], [], []
-    for tkey, (tmpl, keys) in per_template.items():
-        if not keys:
-            continue
-        t = torch.from_numpy(tmpl).to(**f64)
-        sub = [sample_list[row[k]] for k in keys]
-        sub_offsets = np.concatenate([[0], np.cumsum([s.shape[0] for s in sub])])
-        inits = np.stack([s.mean(axis=0) for s in sub])  # match_candidates' initial translations
-        T, _, _, _ = ops.icp_scaled(t, torch.from_numpy(np.concatenate(sub)).to(**f64), sub_offsets, torch.from_numpy(inits).to(**f64))
-        x, y, z = t[:, 0], t[:, 1], t[:, 2]
-        R = T[:, :3, :]
-        fitted = torch.stack([((R[:, r, 0:1] * x + R[:, r, 1:2] * y) + R[:, r, 2:3] * z) + R[:, r, 3:4] for r in range(3)], dim=2)
-        T_host = T.cpu().numpy()
-        for b, k in enumerate(keys):
-            j = row[k]
-            pairs.append((tkey, k, T_host[b], j))
-            hyp.append(fitted[b])
-            sizes.append(t.shape[0])
-            for kk in range(2, MAX_FRUIT_PER_GROUP + 1):
-                centres = cuts[j, CUT_OFFSETS[kk - 2]:CUT_OFFSETS[kk - 1]]
-                hyp.append((t[None, :, :] + centres[:, None, :]).reshape(-1, 3))
-                sizes.append(kk * t.shape[0])
-            a_ranges.extend([[offsets[j], offsets[j + 1]]] * MAX_FRUIT_PER_GROUP)
-    b_offsets = np.concatenate([[0], np.cumsum(sizes)])
-    d = ops.hausdorff(targets, np.asarray(a_ranges, dtype=np.int64), torch.cat(hyp), np.stack([b_offsets[:-1], b_offsets[1:]], axis=1))
-    d = d.view(-1, MAX_FRUIT_PER_GROUP).cpu().numpy()
-    cuts_host = cuts.cpu().numpy()
-    return {(tkey, k): (T, cuts_host[j], d[p]) for p, (tkey, k, T, j) in enumerate(pairs)}

@@ -150,6 +150,28 @@ def test_count_sweep_matches_count_fruits(native_lib, cuda_device):
                           {**clustering.count_fruits(x, **c), "count_after_merge": 0, "num_split_extra": 0, "num_pruned": 0}, atol=0)
 
 
+def test_count_fruits_is_the_op_chain(native_lib, cuda_device):
+    """Device count_fruits is the one-config count_sweep, so the test above compares the sweep with itself; this holds
+    it to the chain of the public ops instead."""
+    pts, _ = touching_fruit_cloud(seed=3)
+    no_ties(pts, 0.015, 0.02)
+    x = dev(pts, cuda_device)
+    got = clustering.count_fruits(x, eps=0.02, min_samples=100, cluster_merge_distance=0.04, down_sample=0.001, remove_outliers_nb_points=120,
+                                  remove_outliers_radius=0.015)
+    down = ops.voxel_down_sample(clustering.remove_radius_outliers(x, 120, 0.015), 0.001)
+    labels, k = ops.dbscan(down, 0.02, 100)
+    sums, counts = ops.cluster_sums(down, labels, k)
+    want = {**clustering.merge_cluster_centers(sums.cpu().numpy(), counts.cpu().numpy(), 0.04), "num_points": int(down.shape[0])}
+    assert got.keys() == want.keys()
+    for key in want:
+        assert type(got[key]) is type(want[key]), key
+    for key in ("count", "count_before_merge", "num_points"):
+        assert got[key] == want[key], key
+    assert got["centers"].dtype == want["centers"].dtype
+    np.testing.assert_array_equal(got["centers"], want["centers"])
+    assert got["count"] > 0
+
+
 def write_obj(path, centres, n=12, radius=0.03):
     with open(path, "w") as f:
         for i, c in enumerate(centres):

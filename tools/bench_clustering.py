@@ -4,9 +4,9 @@ numpy / scikit-learn path in the same run.
 
     python tools/bench_clustering.py --json out/bench_clustering.json
 
-GPU stages are timed with CUDA events after one warm-up run of the whole pipeline at the same size; each wrapper ends
-in the host read of its device-side size, so a stage's window covers all of its work.  The card's name and power
-limit are written next to the numbers.
+GPU stages are the stages of ``count_sweep`` with one config, which is what a device ``count_fruits`` runs, timed with
+CUDA events after one warm-up run at the same size; each stage ends in a host read, so its window covers all of its
+work.  The card's name and power limit are written next to the numbers.
 """
 from __future__ import annotations
 
@@ -23,7 +23,7 @@ import torch
 
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 
-from fruitnerf_b200 import clustering, ops  # noqa: E402
+from fruitnerf_b200 import clustering  # noqa: E402
 from fruitnerf_b200.synthetic import fruit_shell_cloud  # noqa: E402
 
 REAL_TREE = dict(eps=0.02, min_samples=100, cluster_merge_distance=0.04, down_sample=0.001, remove_outliers_nb_points=120,
@@ -32,20 +32,19 @@ STAGES = ("radius_count", "voxel", "dbscan", "sums_merge")
 
 
 def gpu_stages(x: torch.Tensor, p=REAL_TREE):
-    """The device pipeline of clustering.count_fruits, one CUDA-event window per stage."""
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(len(STAGES) + 1)]
-    ev[0].record()
-    pts = clustering.remove_radius_outliers(x, p["remove_outliers_nb_points"], p["remove_outliers_radius"])
-    ev[1].record()
-    pts = ops.voxel_down_sample(pts, p["down_sample"])
-    ev[2].record()
-    labels, k = ops.dbscan(pts, p["eps"], p["min_samples"])
-    ev[3].record()
-    sums, counts = ops.cluster_sums(pts, labels, k)
-    res = clustering.merge_cluster_centers(sums.cpu().numpy(), counts.cpu().numpy(), p["cluster_merge_distance"])
-    ev[4].record()
+    """clustering.count_sweep with the one config of a device count_fruits, one CUDA-event window per stage (its
+    'merge' reported as 'sums_merge')."""
+    ev = {"start": torch.cuda.Event(enable_timing=True)}
+    ev["start"].record()
+
+    def mark(stage):
+        ev[stage] = torch.cuda.Event(enable_timing=True)
+        ev[stage].record()
+
+    res = clustering.count_sweep(x, [p], on_stage=mark)[0]
     torch.cuda.synchronize()
-    return {s: ev[i].elapsed_time(ev[i + 1]) for i, s in enumerate(STAGES)}, res, int(pts.shape[0])
+    names = ["start", "radius_count", "voxel", "dbscan", "merge"]
+    return {s: ev[names[i]].elapsed_time(ev[names[i + 1]]) for i, s in enumerate(STAGES)}, res, res["num_points"]
 
 
 def cpu_stages(pts: np.ndarray, p=REAL_TREE):

@@ -1,7 +1,9 @@
 """Time of stage 3 of the fruit count (clustering.split_clusters) on a seeded touching-fruit cloud the size of an export
 (`synthetic.touching_fruit_cloud`, about 3.5·10^5 points at the defaults): the host alpha-shape step, each kernel
 (ICP, Ward, Hausdorff), the whole stage on the device path and the same stage on the numpy path, plus the ICP iteration
-counts.  Stage 3 runs on the merged groups of the device count at the reference's real-tree parameters.
+counts.  The whole device stage is the span from the 'merge' to the 'match' stage of ``count_sweep`` with the one
+config a device ``count_fruits`` runs, at the reference's real-tree parameters.  The per-step timings run on the merged
+groups of the numpy path, which are the device path's groups.
 
     python tools/bench_fruit_split.py --json out/bench_fruit_split.json
 
@@ -71,26 +73,13 @@ def main(argv=None) -> dict:
     tmpl = sphere_template(0.035, 1000)
     x = torch.from_numpy(pts).to(dev)
 
-    captured = {}
-    orig = cl.split_clusters
-
-    def spy(groups, template, seed=0, device=None):
-        captured["groups"] = groups
-        t0 = time.perf_counter()
-        out = orig(groups, template, seed=seed, device=device)
-        captured["ms"] = 1e3 * (time.perf_counter() - t0)
-        return out
-
-    cl.split_clusters = spy
-    try:
-        cl.count_fruits(x, **REAL_TREE, template=tmpl)  # warm-up of every kernel
-        t0 = time.perf_counter()
-        res = cl.count_fruits(x, **REAL_TREE, template=tmpl)
-        total_ms = 1e3 * (time.perf_counter() - t0)
-    finally:
-        cl.split_clusters = orig
-    groups = captured["groups"]
-    stage3_gpu_ms = captured["ms"]
+    cl.count_fruits(x, **REAL_TREE, template=tmpl)  # warm-up of every kernel
+    marks = {}
+    t0 = time.perf_counter()
+    res = cl.count_sweep(x, [REAL_TREE], [tmpl], on_stage=lambda stage: marks.setdefault(stage, time.perf_counter()))[0]
+    total_ms = 1e3 * (time.perf_counter() - t0)
+    stage3_gpu_ms = 1e3 * (marks["match"] - marks["merge"])  # both stages end in a host read
+    groups = host_groups(pts, tmpl)
 
     t0 = time.perf_counter()
     _, samples = cl.alpha_stage(groups, tmpl)
@@ -126,6 +115,23 @@ def main(argv=None) -> dict:
         with open(a.json, "w") as f:
             json.dump(out, f, indent=1)
     return out
+
+
+def host_groups(pts: np.ndarray, tmpl: np.ndarray):
+    """The merged groups the numpy count hands to stage 3.  Its ``split_clusters`` is stubbed out meanwhile: the numpy
+    matching is timed on its own, and only with ``--no-cpu`` off."""
+    captured = []
+
+    def stub(groups, template, seed=0, device=None):
+        captured.append(groups)
+        return {"centers": np.zeros((0, 3)), "num_split_extra": 0, "num_pruned": 0}
+
+    orig, cl.split_clusters = cl.split_clusters, stub
+    try:
+        cl.count_fruits(pts, **REAL_TREE, template=tmpl)
+    finally:
+        cl.split_clusters = orig
+    return captured[0]
 
 
 def ops_distances(samp, tmpl, dev):
