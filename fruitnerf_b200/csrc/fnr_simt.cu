@@ -250,14 +250,17 @@ struct ForwardPlan {
   static constexpr int kBytes = kStepOff + kGroups * wg::kResidentStepBytes;
 };
 // Dynamic shared memory of the resident backward CTA: weight image | accumulators | locks | per-warpgroup step tiles |
-// per-warpgroup warp partials.
+// per-warpgroup dW operand regions.
 struct BackwardPlan {
   static constexpr int kGroups = 2;
   static constexpr int kAccOff = resident::kImageBytes;
   static constexpr int kLockOff = kAccOff + resident::acc_off(resident::kSlots) * 4;
   static constexpr int kStepOff = resident::align128(kLockOff + resident::kSlots * 4);
-  static constexpr int kPartOff = kStepOff + kGroups * wg::kResidentStepBytes;
-  static constexpr int kBytes = kPartOff + kGroups * 4 * wg::kWarpPartial * 4;
+  static constexpr int kDwOff = kStepOff + kGroups * wg::kResidentStepBytes;
+  static constexpr int kBytes = kDwOff + kGroups * wg::kDwXBytes;
+  // with the kernel's static shared memory (s_app, 128 B; the phase timers' 112 B in that diagnostic build), within the
+  // 232 448 bytes an H100 CTA can have
+  static_assert(kBytes + 256 <= 232448, "backward shared-memory plan");
 };
 
 // The layers of the small family's tensor-core kernels on the resident image (Plan: the kernel's shared-memory plan).
@@ -279,7 +282,7 @@ struct ResidentLayers {
     return wg_smem;
   }
   static __device__ __forceinline__ uint8_t* step() { return smem() + Plan::kStepOff + wg::group() * wg::kResidentStepBytes; }
-  static __device__ __forceinline__ float* part() { return reinterpret_cast<float*>(smem() + Plan::kPartOff) + wg::group() * 4 * wg::kWarpPartial; }
+  static __device__ __forceinline__ uint8_t* dw_region() { return smem() + Plan::kDwOff + wg::group() * wg::kDwXBytes; }
   template <int S>
   static __device__ __forceinline__ float* acc() {
     constexpr int off = acc_off(S);
@@ -396,18 +399,24 @@ struct ResidentLayers {
   static __device__ __forceinline__ void dw(float*, float*, const float (&x)[Kv], const float (&dy)[Nv], float*, float*) {
     static_assert(K(SLOT) == Kv && N(SLOT) == Nv, "slot shape");
     if constexpr (tensor(Nv))
-      wg::weight_grad_acc<Kv, Nv>(step(), part(), x, dy, acc<SLOT>(), lock(SLOT));
+      wg::weight_grad_acc<Kv, Nv>(step(), dw_region(), x, dy, acc<SLOT>(), lock(SLOT));
     else
-      wg::head_weight_grad_acc<Kv, Nv>(part(), x, dy, acc<SLOT>(), lock(SLOT));
+      wg::head_weight_grad_acc<Kv, Nv>(reinterpret_cast<float*>(dw_region()), x, dy, acc<SLOT>(), lock(SLOT));
     FNR_PHASE(kPhDw);
   }
-  // Both gradients of one layer, the weight gradient first: dy is then last read when dx stages it, so it is not live
-  // next to dxv.  For a 64-wide layer that is 64 fewer live registers at the backward's peak (DESIGN.md section 4.3).
+  // Both gradients of one layer, the weight gradient first.  A tensor-core layer stages dy once: dW reads the tile
+  // weight_grad_acc leaves in step(), and dx runs its MMAs on the same tile, so dy is dead once staged and not live next
+  // to dxv (for a 64-wide layer, 64 registers at the backward's peak; DESIGN.md section 4.3).
   template <int SLOT, int Kv, int Nv>
   static __device__ __forceinline__ void grad(const float* __restrict__ W, float* sX, float* sY, const float (&x)[Kv],
                                               const float (&dy)[Nv], float (&dxv)[Kv], float* gW, float* gb) {
     dw<SLOT, Kv, Nv>(sX, sY, x, dy, gW, gb);
-    dx<SLOT, Kv, Nv>(W, dy, dxv);
+    if constexpr (tensor(Nv)) {
+      wg::resident_rowgemm_t_staged<wg::padn(Nv), wg::pad16(Kv), Nv>(step(), smem() + img_off(SLOT), dxv);
+      FNR_PHASE(kPhDx);
+    } else {
+      dx<SLOT, Kv, Nv>(W, dy, dxv);
+    }
   }
 };
 using ResidentForward = ResidentLayers<ForwardPlan>;

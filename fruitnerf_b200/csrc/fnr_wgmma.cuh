@@ -332,18 +332,25 @@ __device__ __forceinline__ void stage_rows(uint8_t* smem, const float (&x)[R]) {
   sync();
 }
 
-// The same GEMM with the weights from a resident split image (W [NPF][KPF] K-major, as rowgemm stages it), y = W^T x
-// (dx): the image read MN-major through the transpose bit.  smem is the warpgroup's kResidentStepBytes.
+// y = W^T x (dx) on the row tile of x[R] already staged in smem (stage_rows' bytes), with the weights from a resident
+// split image (W [NPF][KPF] K-major, as rowgemm stages it) read MN-major through the transpose bit; the result rows are
+// stored over the tile.  smem is the warpgroup's kResidentStepBytes.
 template <int NPF, int KPF, int R, int NO>
-__device__ __forceinline__ void resident_rowgemm_t(uint8_t* smem, const uint8_t* img, const float (&x)[R], float (&y)[NO]) {
+__device__ __forceinline__ void resident_rowgemm_t_staged(uint8_t* smem, const uint8_t* img, float (&y)[NO]) {
   constexpr int KP = pad16(R), NP = padn(NO);
   static_assert(KP <= NPF && NP <= KPF, "layer outside the resident image");
   static_assert(2 * 128 * KP * 2 <= kResidentStepBytes && NP * 128 * 4 <= kResidentStepBytes, "resident step plan");
   float* ys = reinterpret_cast<float*>(smem);
-  stage_rows(smem, x);
   layer_mma<KP, NP, 1, true>(smem_u32(smem), 128 * KP * 2, image_operand<NPF, KPF, true>(img), ys, 4, kRowsGroupStride);
   sync();
   read_row<NO>(ys, 4, kRowsGroupStride, y);
+}
+
+// The same with x staged first.
+template <int NPF, int KPF, int R, int NO>
+__device__ __forceinline__ void resident_rowgemm_t(uint8_t* smem, const uint8_t* img, const float (&x)[R], float (&y)[NO]) {
+  stage_rows(smem, x);
+  resident_rowgemm_t_staged<NPF, KPF, R, NO>(smem, img, y);
 }
 
 // Two forward layers chained fragment to fragment: m = epi0(W0 x), y = W1 m (before its bias), both weights from the
@@ -511,9 +518,10 @@ __device__ __forceinline__ float warp_reduce_scatter(float* v, int lane) {
 constexpr int pow2_at_least(int n) { return n <= 1 ? 1 : 2 * pow2_at_least((n + 1) / 2); }
 constexpr int log2_exact(int n) { return n <= 1 ? 0 : 1 + log2_exact(n / 2); }
 
-// out[i] = sum over the warp's 32 lanes of v(i), i < M, in fp32 (32-value reduce-scatters; no serial loops).
-template <int M, class V>
-__device__ __forceinline__ void warp_column_sums(V v, float* out, int lane) {
+// put(i, sum over the warp's 32 lanes of v(i)) for i < M, in fp32 (32-value reduce-scatters; no serial loops), each i
+// put by one lane.
+template <int M, class V, class Put>
+__device__ __forceinline__ void warp_column_sums(V v, Put put, int lane) {
 #pragma unroll
   for (int c = 0; c < M; c += 32) {
     constexpr int kLeft = M % 32 == 0 ? 32 : M % 32;
@@ -524,7 +532,7 @@ __device__ __forceinline__ void warp_column_sums(V v, float* out, int lane) {
     for (int j = 0; j < P; ++j) u[j] = c + j < M ? v(c + j < M ? c + j : 0) : 0.f;
     const float s = warp_reduce_scatter<P>(u, lane);
     const int i = c + (lane >> SH);
-    if ((lane & ((1 << SH) - 1)) == 0 && i < M) out[i] = s;
+    if ((lane & ((1 << SH) - 1)) == 0 && i < M) put(i, s);
   }
 }
 
@@ -545,9 +553,13 @@ __device__ __forceinline__ void release(int* lock) {
   }
 }
 
-// Floats of per-warp partial sums a warpgroup needs (kWarpPartial per warp), and of a layer's accumulator: dW in
-// fragment order (the rows of warps that hold outputs n < N, KP / 2 floats per thread) followed by db[N].
+// Bytes of a warpgroup's dW operand region: the MN-major X tile of one weight_grad_acc round, hi | lo.  The fp32 heads'
+// per-warp partial sums (kWarpPartial floats per warp) use the same region, which no MMA reads while a head runs.
+// Floats of a layer's accumulator: dW in fragment order (the rows of warps that hold outputs n < N, KP / 2 floats per
+// thread) followed by db[N].
+constexpr int kDwXBytes = 16 * 1024;
 constexpr int kWarpPartial = 256;
+static_assert(4 * kWarpPartial * 4 <= kDwXBytes, "head partials within the dW operand region");
 template <int K, int N>
 struct DwAcc {
   static constexpr int KP = padn(K), kWarps = (N + 15) / 16;
@@ -560,84 +572,88 @@ struct DwAcc {
   }
 };
 
-// Weight gradient of the warpgroup's 128-point tile added to the layer's accumulator acc (DwAcc<K, N>): dW = dY^T X
-// with both operands MN-major over the points (16-byte split stores of 8 outputs / inputs of one point), in two 64-point
-// halves (the operands of all 128 points would take 64 KiB).  Each half's fragments are added on their own, so that no
-// accumulator registers are live while the next half is staged (that kept the kernel's spills below the staged
-// kernel's); db from warp reduce-scatters of dY.  smem: the warpgroup's kResidentStepBytes; part: its 4 x kWarpPartial
-// floats.  Every thread of the warpgroup must call it.
+// Weight gradient of the warpgroup's 128-point tile added to the layer's accumulator acc (DwAcc<K, N>), with dY staged
+// once for it and for the layer's dx.  Every thread splits its dy row into the step tile `smem` as dx's K-major A tile
+// (stage_rows' bytes: element (point p, output n) at (n / 8) * 2048 + p * 16 + (n % 8) * 2), which dW = dY^T X reads
+// MN-major through the transpose bit; rows of dY past N read bytes that are never accumulated.  X goes MN-major into the
+// dW operand region `xs` (16-byte split stores of 8 inputs of one point), PTS points per round: one round for KP <= 32,
+// two 64-point rounds for KP = 64.  The k16 steps over all 128 points are one MMA chain, and the accumulator takes it
+// under the layer's lock once per tile.  It is added before dx runs, so that its KP / 2 registers are not live next to
+// dx's accumulators.  db: each warp's column sums of dy added to acc's bias row with shared-memory float adds, no lock.
+// The dY tile is left in smem for resident_rowgemm_t_staged.  Every thread of the warpgroup must call it.
 template <int K, int N>
-__device__ __forceinline__ void weight_grad_acc(uint8_t* smem, float* part, const float (&x)[K], const float (&dy)[N],
+__device__ __forceinline__ void weight_grad_acc(uint8_t* smem, uint8_t* xs, const float (&x)[K], const float (&dy)[N],
                                                 float* acc, int* lock) {
   using A = DwAcc<K, N>;
-  constexpr int KP = A::KP, MC = (N + 7) / 8;  // MMA width; 8-output chunks of dY that are stored
-  static_assert(N <= 64 && N <= kWarpPartial, "one M tile of outputs");
-  constexpr uint32_t ALO = 64 * 64 * 2, BLO = KP * 64 * 2;
-  static_assert(2 * ALO + 2 * BLO <= kResidentStepBytes, "resident step plan");
-  uint8_t* ahi = smem;
-  uint8_t* bhi = smem + 2 * ALO;
+  constexpr int KP = A::KP, YP = pad16(N);  // MMA width; dY tile width
+  constexpr int PTS = kDwXBytes / (4 * KP) < 128 ? kDwXBytes / (4 * KP) : 128, ROUNDS = 128 / PTS;
+  constexpr uint32_t YLO = 128 * YP * 2, XLO = PTS * KP * 2;
+  static_assert(N <= 64 && 2 * YLO <= kResidentStepBytes && 2 * XLO <= kDwXBytes && PTS % 16 == 0, "dW plan");
   const int t = tid(), warp = t >> 5, lane = t & 31;
-  warp_column_sums<N>([&](int n) { return dy[n]; }, part + warp * kWarpPartial, lane);
-#pragma unroll 1
-  for (int half = 0; half < 2; ++half) {
-    sync();  // the previous readers of the tile are done
-    if ((t >> 6) == half) {
-      // element (row, point p) at (row / 8) * 1024 + p * 16 + (row % 8) * 2; rows of dY past N are never accumulated
-      const int p = (t & 63) * 16;
+  float* db = acc + A::kW;
+  warp_column_sums<N>([&](int n) { return dy[n]; }, [&](int n, float s) { atomicAdd(db + n, s); }, lane);
+  sync();  // the previous readers of the step tile and of xs are done
 #pragma unroll
-      for (int c = 0; c < MC; ++c) split_store_chunk(ahi, ahi + ALO, c * 1024 + p, dy, c);
+  for (int c = 0; c < YP / 8; ++c) split_store_chunk(smem, smem + YLO, c * (128 * 16) + t * 16, dy, c);
+  const uint32_t ay = smem_u32(smem), ax = smem_u32(xs);
+  float d[KP / 2];
 #pragma unroll
-      for (int c = 0; c < KP / 8; ++c) split_store_chunk(bhi, bhi + BLO, c * 1024 + p, x, c);
+  for (int i = 0; i < KP / 2; ++i) d[i] = 0.f;
+#pragma unroll
+  for (int r = 0; r < ROUNDS; ++r) {
+    if (r > 0) {  // the previous round's MMAs are done with xs
+      wait_all();
+      sync();
+    }
+    if (t / PTS == r) {
+#pragma unroll
+      for (int c = 0; c < KP / 8; ++c) split_store_chunk(xs, xs + XLO, c * (PTS * 16) + (t % PTS) * 16, x, c);
     }
     fence_proxy_async();
     sync();
-    const uint32_t aa = smem_u32(ahi), ab = smem_u32(bhi);
-    float d[KP / 2];
-#pragma unroll
-    for (int i = 0; i < KP / 2; ++i) d[i] = 0.f;
     fence_operands();
 #pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-      const uint64_t dah = desc(aa + ks * 256, 128, 1024), dal = desc(aa + ALO + ks * 256, 128, 1024);
-      const uint64_t dbh = desc(ab + ks * 256, 128, 1024), dbl = desc(ab + BLO + ks * 256, 128, 1024);
-      mma_m64k16<KP, 1, 1>(d, dah, dbh, ks > 0);
+    for (int ks = 0; ks < PTS / 16; ++ks) {
+      const uint32_t ya = ay + (r * (PTS / 16) + ks) * 256, xa = ax + ks * 256;
+      const uint64_t dah = desc(ya, 128, 128 * 16), dal = desc(ya + YLO, 128, 128 * 16);
+      const uint64_t dbh = desc(xa, 128, PTS * 16), dbl = desc(xa + XLO, 128, PTS * 16);
+      mma_m64k16<KP, 1, 1>(d, dah, dbh, r > 0 || ks > 0);
       mma_m64k16<KP, 1, 1>(d, dal, dbh, 1);
       mma_m64k16<KP, 1, 1>(d, dah, dbl, 1);
       mma_m64k16<KP, 1, 1>(d, dal, dbl, 1);
     }
     commit();
-    wait_all();
-    FNR_PHASE(kPhDw);
-    acquire(lock);
-    if (warp < A::kWarps) {
-      float4* a4 = reinterpret_cast<float4*>(acc) + warp * (KP / 8) * 32 + lane;
-#pragma unroll
-      for (int q = 0; q < KP / 8; ++q) {
-        float4 v = a4[q * 32];
-        v.x += d[4 * q];
-        v.y += d[4 * q + 1];
-        v.z += d[4 * q + 2];
-        v.w += d[4 * q + 3];
-        a4[q * 32] = v;
-      }
-    }
-    if (half == 1 && t < N) acc[A::kW + t] += part[t] + part[kWarpPartial + t] + part[2 * kWarpPartial + t] + part[3 * kWarpPartial + t];
-    release(lock);
-    FNR_PHASE(kPhDwFlush);
   }
+  wait_all();
+  FNR_PHASE(kPhDw);
+  acquire(lock);
+  if (warp < A::kWarps) {
+    float4* a4 = reinterpret_cast<float4*>(acc) + warp * (KP / 8) * 32 + lane;
+#pragma unroll
+    for (int q = 0; q < KP / 8; ++q) {
+      float4 v = a4[q * 32];
+      v.x += d[4 * q];
+      v.y += d[4 * q + 1];
+      v.z += d[4 * q + 2];
+      v.w += d[4 * q + 3];
+      a4[q * 32] = v;
+    }
+  }
+  release(lock);
+  FNR_PHASE(kPhDwFlush);
 }
 
 // Weight gradient of a narrow fp32 head (N = 1, 3 outputs) over the warpgroup's tile, exact fp32 on the CUDA cores: warp
-// reduce-scatters of dy[n] x[k] and dy[n] into per-warp partials, then the warps' sums are added to acc ([N][K] then
-// [N]).  Every thread of the warpgroup must call it.
+// reduce-scatters of dy[n] x[k] and dy[n] into per-warp partials (part: 4 x kWarpPartial floats), then the warps' sums
+// are added to acc ([N][K] then [N]).  Every thread of the warpgroup must call it.
 template <int K, int N>
 __device__ __forceinline__ void head_weight_grad_acc(float* part, const float (&x)[K], const float (&dy)[N], float* acc, int* lock) {
   static_assert(K % 32 == 0 && N * K + N <= kWarpPartial, "head partials");
   const int t = tid(), warp = t >> 5, lane = t & 31;
   float* pw = part + warp * kWarpPartial;
 #pragma unroll
-  for (int n = 0; n < N; ++n) warp_column_sums<K>([&](int k) { return dy[n] * x[k]; }, pw + n * K, lane);
-  warp_column_sums<N>([&](int n) { return dy[n]; }, pw + N * K, lane);
+  for (int n = 0; n < N; ++n) warp_column_sums<K>([&](int k) { return dy[n] * x[k]; }, [&](int k, float s) { pw[n * K + k] = s; }, lane);
+  warp_column_sums<N>([&](int n) { return dy[n]; }, [&](int n, float s) { pw[N * K + n] = s; }, lane);
   acquire(lock);  // its barrier also orders the partial stores before the reads below
   for (int e = t; e < N * K + N; e += 128)
     acc[e] += part[e] + part[kWarpPartial + e] + part[2 * kWarpPartial + e] + part[3 * kWarpPartial + e];
