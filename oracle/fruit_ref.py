@@ -224,12 +224,23 @@ class DensitySpec:
         return ns.hash_scalings(self.num_levels, self.base_res, self.max_res)
 
 
-def proposal_weights(pp: Dict[str, Tensor], spec: DensitySpec, origins, directions, starts, ends, aabb, contraction: bool = True) -> Tensor:
-    """density_fn(frustum midpoints) -> get_weights for one level.  starts/ends [R,S] -> weights [R,S]."""
+def proposal_weights(pp: Dict[str, Tensor], spec: DensitySpec, origins, directions, starts, ends, aabb, contraction: bool = True,
+                     relu_margin: bool = False):
+    """density_fn(frustum midpoints) -> get_weights for one level.  starts/ends [R,S] -> weights [R,S].
+
+    ``relu_margin`` (test hook, as field_forward's): also return [R,S] min |hidden pre-activation| / rms of the hidden layer
+    over the batch, +inf for samples outside the selector (their density is 0 and they pass no gradient)."""
     pos = ns.frustum_positions(origins[:, None, :], directions[:, None, :], starts[..., None], ends[..., None])
+    hook = {} if relu_margin else None
     dens = ns.proposal_density(pos, pp["encoding.hash_table"], spec.scalings(), spec.log2_hashmap_size, pp["mlp_base.1.layers.0.weight"],
-                               pp["mlp_base.1.layers.0.bias"], pp["mlp_base.1.layers.1.weight"], pp["mlp_base.1.layers.1.bias"], aabb, contraction)
-    return ns.get_weights((ends - starts)[..., None], dens)[..., 0]
+                               pp["mlp_base.1.layers.0.bias"], pp["mlp_base.1.layers.1.weight"], pp["mlp_base.1.layers.1.bias"], aabb, contraction,
+                               hook=hook)
+    weights = ns.get_weights((ends - starts)[..., None], dens)[..., 0]
+    if not relu_margin:
+        return weights
+    pre = hook["preacts"]
+    margin = (pre.abs() / pre.pow(2).mean().sqrt().clamp_min(1e-20)).amin(dim=-1)
+    return weights, margin.masked_fill(~hook["selector"], float("inf"))
 
 
 def proposal_sampler(prop_params, prop_specs, origins, directions, nears, fars, num_prop_samples, num_nerf_samples, aabb, t_rand0=None,

@@ -332,10 +332,17 @@ def spacing_to_euclidean(bins: Tensor, nears: Tensor, fars: Tensor) -> Tensor:
     return lindisp_piecewise_inv(bins * s_far + (1 - bins) * s_near)
 
 
+def select_density(density: Tensor, selector: Tensor) -> Tensor:
+    """``density * selector`` of HashMLPDensityField.get_density: samples outside the selector have density 0 and pass no
+    gradient to the network."""
+    return density * selector[..., None]
+
+
 def proposal_density(positions: Tensor, table: Tensor, scalings: Tensor, log2_hashmap_size: int, w0: Tensor, b0: Tensor, w1: Tensor,
-                     b1: Tensor, aabb: Tensor, contraction: bool = True) -> Tensor:
+                     b1: Tensor, aabb: Tensor, contraction: bool = True, hook: Optional[Dict] = None) -> Tensor:
     """[NS] HashMLPDensityField.get_density (through Field.density_fn): contraction -> (x+2)/4 ->
-    selector mask -> hash grid -> Linear/ReLU/Linear -> trunc_exp * selector.  positions [...,3] -> [...,1]."""
+    selector mask -> hash grid -> Linear/ReLU/Linear -> trunc_exp * selector.  positions [...,3] -> [...,1].
+    ``hook`` (test hook) receives the detached hidden pre-activations [..., hidden] and the selector [...]."""
     pos = positions
     if contraction:
         pos = (scene_contraction_inf(pos) + 2.0) / 4.0
@@ -344,12 +351,15 @@ def proposal_density(positions: Tensor, table: Tensor, scalings: Tensor, log2_ha
     selector = ((pos > 0.0) & (pos < 1.0)).all(dim=-1)
     pos = pos * selector[..., None]
     flat = pos.reshape(-1, 3)
-    out = []
+    out, pre = [], []
     for a in range(0, flat.shape[0], 65536):
         enc = hash_encode(flat[a : a + 65536], table, scalings, log2_hashmap_size)
-        out.append(mlp_forward(enc, [w0, w1], [b0, b1]))
+        out.append(mlp_forward(enc, [w0, w1], [b0, b1], preacts=pre))
     dba = torch.cat(out).view(*pos.shape[:-1], 1)
-    return trunc_exp(dba) * selector[..., None]
+    if hook is not None:
+        hook["preacts"] = torch.cat(pre).view(*pos.shape[:-1], -1)
+        hook["selector"] = selector
+    return select_density(trunc_exp(dba), selector)
 
 
 def pdf_sample(weights: Tensor, existing_bins: Tensor, num_samples: int, u_rand: Optional[Tensor], histogram_padding: float = 0.01,

@@ -213,9 +213,20 @@ def test_render_frames_equals_the_camera_ray_bundle_path(trained_run, cuda_devic
     w = entrypoint(["camera-path", "--load-config", str(trained_run / "config.yml"), "--camera-path-filename", str(pf), "--output-path", str(out),
                     "--output-format", "images", "--image-format", "png", "--rendered-output-names", *names])
     assert w.count == 1
-    img = np.asarray(Image.open(tmp_path / "renders" / "cp" / "00000.png")).astype(np.int16)
-    want3 = torch_frame(ref, names, H, W).astype(np.int16)
-    assert img.shape == want3.shape and int(np.abs(img - want3).max()) <= 1
+    # The file gives the data set's camera back up to the fp32 rounding of the focal length through its fov.  A ray moved by
+    # that rounding can move a pixel's median depth to the neighbouring sample or its semantic label across 0.9, so the
+    # frame is not compared with the data-set camera's: the file's camera is checked against that camera, and the CLI's
+    # frame against the in-process render of the file's camera, byte for byte.
+    cp = R.get_path_from_json(path)
+    assert torch.equal(cp.camera_to_worlds, one.camera_to_worlds.cpu()) and (cp.height, cp.width) == (H, W)
+    assert torch.equal(cp.cx, one.cx.cpu()) and torch.equal(cp.cy, one.cy.cpu())
+    assert torch.allclose(cp.fx, one.fx.cpu(), rtol=1e-6, atol=0) and torch.allclose(cp.fy, one.fy.cpu(), rtol=1e-6, atol=0)
+    img = np.asarray(Image.open(tmp_path / "renders" / "cp" / "00000.png"))
+    want3 = R.render_frames(pipeline, cp, names)[0]
+    assert img.shape == want3.shape and np.array_equal(img, want3), int(np.abs(img.astype(np.int16) - want3).max())
+    # and that render is the data-set camera's frame, except where a pixel sits on such a discontinuity
+    near = np.abs(want3.astype(np.int16) - torch_frame(ref, names, H, W).astype(np.int16)).max(axis=-1) <= 1
+    assert near.mean() >= 0.99, float(near.mean())
 
     # interpolate and spiral write the expected number of frames of the expected size
     out = tmp_path / "renders" / "interp.mp4"

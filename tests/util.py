@@ -8,6 +8,7 @@ import torch
 from fruitnerf_b200 import synthetic as syn
 from fruitnerf_b200.fruit_field import FruitField, SceneContraction
 from oracle import fruit_ref as fr
+from oracle import ns_torch as ns
 
 REL = 1e-3  # north_star tolerance: 1e-3 relative on RGB / density / semantics
 FLOOR = 0.01  # elements below 1% of the tensor's max magnitude are compared absolutely (against rel * 1% * max)
@@ -54,11 +55,12 @@ GRAD_FLOOR = 0.05  # elements below 5% of their group's scale are compared again
 RELU_MARGIN = 1e-4  # samples with a hidden pre-activation within 1e-4 (relative to the layer rms) of zero
 
 
-def _grad_scales(want: torch.Tensor, key: str, num_levels: int, own_rows=None) -> torch.Tensor:
-    """Per-element scale of a gradient tensor: its max |value|; for the hash table the max of each level, and ``own_rows``
-    (flat table rows) each scaled by themselves, outside their level's scale."""
+def _grad_scales(want: torch.Tensor, key: str, num_levels: int, own_rows=None, hash_key: str = HASH_KEY) -> torch.Tensor:
+    """Per-element scale of a gradient tensor: its max |value|; for the hash table (``hash_key``: the field's, or a proposal
+    network's PROP_HASH_KEY) the max of each of its ``num_levels`` levels, and ``own_rows`` (flat table rows) each scaled by
+    themselves, outside their level's scale."""
     b = want.abs()
-    if key != HASH_KEY:
+    if key != hash_key:
         return b.amax().expand_as(b)
     lv = b.reshape(num_levels, -1, b.shape[-1])
     own = torch.zeros(lv.shape[:2], dtype=torch.bool)
@@ -69,7 +71,7 @@ def _grad_scales(want: torch.Tensor, key: str, num_levels: int, own_rows=None) -
     return torch.where(own[..., None], row_scale, level_scale).reshape(b.shape)
 
 
-def grad_errors(got: dict, want: dict, num_levels: int = 16, floor: float = GRAD_FLOOR, own_rows=None) -> dict:
+def grad_errors(got: dict, want: dict, num_levels: int = 16, floor: float = GRAD_FLOOR, own_rows=None, hash_key: str = HASH_KEY) -> dict:
     """Worst normalized error per tensor: max |a - b| / max(|b|, floor * scale), scales from ``_grad_scales``.  A tensor
     whose reference is exactly zero gets an infinite error for any nonzero element (and 0 when it is zero too)."""
     res = {}
@@ -78,7 +80,7 @@ def grad_errors(got: dict, want: dict, num_levels: int = 16, floor: float = GRAD
         b = b.detach().double().cpu()
         assert a.shape == b.shape, (key, a.shape, b.shape)
         assert bool(torch.isfinite(a).all()), f"grad {key}: non-finite values"
-        den = torch.maximum(b.abs(), floor * _grad_scales(b, key, num_levels, own_rows))
+        den = torch.maximum(b.abs(), floor * _grad_scales(b, key, num_levels, own_rows, hash_key))
         err = (a - b).abs()
         ratio = torch.where(err == 0, torch.zeros_like(err), err / den)  # den == 0 and err > 0 -> inf
         res[key] = float(ratio.max()) if ratio.numel() else 0.0
@@ -194,3 +196,166 @@ def make_field(name: str, sd, spec, device, contraction=True, test_mode=None, **
     assert not unexpected, unexpected
     assert all(k.startswith("mlp_base.") or k in ("max_res", "num_levels", "log2_hashmap_size") for k in missing), missing
     return f.to(device)
+
+
+# ---- proposal stage ------------------------------------------------------------------------------------------------------------
+PROP_HASH_KEY = "encoding.hash_table"
+PROP_KEYS = (PROP_HASH_KEY, "mlp_base.1.layers.0.weight", "mlp_base.1.layers.0.bias", "mlp_base.1.layers.1.weight",
+             "mlp_base.1.layers.1.bias")
+
+
+def proposal_rays(R: int, S: int, salt: int = 0, far: float = 30.0):
+    """(origins, directions, starts, ends) float32: syn.ray_batch rays with nears 0.05 and fars ``far``, S bins spaced by the
+    piecewise linear-in-disparity map of the initial sampler (one jitter per ray)."""
+    o, d, _, _, _ = syn.ray_batch(R, 4, salt=salt)
+    nears, fars = torch.full((R, 1), 0.05), torch.full((R, 1), far)
+    bins = ns.spaced_bins(R, S, (syn.hash_uniform(R, 77 + salt).view(R, 1) + 1) * 0.5)
+    e = ns.spacing_to_euclidean(bins, nears, fars)
+    return o, d, e[:, :-1].contiguous(), e[:, 1:].contiguous()
+
+
+def weight_coefficients(R: int, S: int, salt: int = 0) -> torch.Tensor:
+    """[R,S] U(-1,1) coefficients of a linear loss on the proposal weights.  Signed: with one-signed coefficients the gradient
+    of the output bias (a sum of d loss / d log-density over every sample) cancels ~3000-fold, and fp32 arithmetic alone
+    (the float32 oracle's) leaves it 2e-3 off the float64 value."""
+    return syn.hash_uniform(R * S, 91 + salt).view(R, S)
+
+
+@dataclass
+class ProposalRun:
+    grads: dict
+    weights: torch.Tensor
+    ray_weights: torch.Tensor
+
+
+def proposal_oracle_backward(sd, spec, rays, coef, contraction=True, dtype=torch.float64, ray_weights=None, chunk=1024,
+                             min_rays=8) -> ProposalRun:
+    """Gradients of sum(ray_w * coef * w) by autograd through fr.proposal_weights with the parameters in ``dtype``, formed
+    over chunks of ``chunk`` rays (the loss is a sum over rays).  Rays stay float32, so sample positions, hash rows and
+    trilinear offsets are the kernels'.  ``ray_weights`` default: 1 for the rays whose samples all keep RELU_MARGIN."""
+    o, d, s, e = rays
+    params = {k: v.detach().to(dtype, copy=True).requires_grad_(True) for k, v in sd.items() if k != "aabb"}
+    aabb = sd["aabb"]
+    R = s.shape[0]
+    ws, rws = [], []
+    for a in range(0, R, chunk):
+        b = min(R, a + chunk)
+        w, margin = fr.proposal_weights(params, spec, o[a:b], d[a:b], s[a:b], e[a:b], aabb, contraction, relu_margin=True)
+        rw = (margin > RELU_MARGIN).all(dim=1).to(dtype) if ray_weights is None else ray_weights[a:b].to(dtype)
+        (rw[:, None] * coef[a:b].to(dtype) * w).sum().backward()
+        ws.append(w.detach())
+        rws.append(rw)
+    rw = torch.cat(rws)
+    assert rw.sum() >= min_rays, f"only {int(rw.sum())} of {R} rays keep a ReLU margin"
+    grads = {k: (p.grad if p.grad is not None else torch.zeros_like(p)).detach() for k, p in params.items()}
+    return ProposalRun(grads, torch.cat(ws), rw)
+
+
+def proposal_net(sd, spec, contraction=True, device="cuda"):
+    """HashMLPDensityField of ``spec`` holding the parameters of a syn.density_state dict."""
+    from fruitnerf_b200.density_field import HashMLPDensityField
+
+    net = HashMLPDensityField(sd["aabb"], hidden_dim=spec.hidden_dim, log2_hashmap_size=spec.log2_hashmap_size, num_levels=spec.num_levels,
+                              max_res=spec.max_res, spatial_distortion=SceneContraction() if contraction else None)
+    missing, unexpected = net.load_state_dict(sd, strict=False)
+    assert not unexpected and all(k.startswith("mlp_base.0") or k in ("max_res", "num_levels", "log2_hashmap_size") for k in missing)
+    return net.to(device)
+
+
+def proposal_edge_case(spec, R: int = 509, S: int = 96, salt: int = 3):
+    """AABB-mode batch (positions normalized by the box, no contraction) of R ordinary rays out to t = 30, most of which leave
+    the box, and three edge rays appended:
+      R     every sample outside the box (selector 0 everywhere: density 0, no gradient);
+      R + 1 every other bin of zero width;
+      R + 2 S bins of 1e-8 around t = 1e-3, all in the same grid cells, whose table rows are set so that the density's
+            pre-activation h is 17: past trunc_exp's backward clamp at 15, with sigma * delta ~ 0.25 per bin.
+    Returns (state, (origins, directions, starts, ends)) with R + 3 rays."""
+    sd = syn.density_state(num_levels=spec.num_levels, log2_hashmap_size=spec.log2_hashmap_size, salt=7000 + salt)
+    o, d, s, e = proposal_rays(R, S, salt=salt)
+    out_o, out_d = torch.tensor([[3.0, 3.0, 3.0]]), torch.tensor([[0.6, 0.0, 0.8]])
+    zw_s, zw_e = s[:1].clone(), e[:1].clone()
+    zw_e[:, 1::2] = zw_s[:, 1::2]
+    cl_o, cl_d = torch.tensor([[0.3, -0.2, 0.1]]), torch.tensor([[0.0, 0.6, 0.8]])
+    cl_s = (1e-3 + 1e-8 * torch.arange(S, dtype=torch.float32))[None]
+    cl_e = (1e-3 + 1e-8 * torch.arange(1, S + 1, dtype=torch.float32))[None]
+    o = torch.cat([o, out_o, o[:1], cl_o]).contiguous()
+    d = torch.cat([d, out_d, d[:1], cl_d]).contiguous()
+    s = torch.cat([s, s[:1], zw_s, cl_s]).contiguous()
+    e = torch.cat([e, e[:1], zw_e, cl_e]).contiguous()
+    # the clamp ray: every corner row of its cells, every level, holds (a, a); h(a) = 17 solved by bisection on the side of a
+    # along which h grows without bound
+    p = ns.normalized_positions(ns.frustum_positions(cl_o[:, None], cl_d[:, None], cl_s[..., None], cl_e[..., None]), sd["aabb"])
+    rows = ns.hash_corner_indices(p.reshape(-1, 3), spec.scalings(), spec.log2_hashmap_size)[0].unique()
+    w0, b0 = sd["mlp_base.1.layers.0.weight"].double(), sd["mlp_base.1.layers.0.bias"].double()
+    w1, b1 = sd["mlp_base.1.layers.1.weight"].double()[0], float(sd["mlp_base.1.layers.1.bias"])
+    rs = w0.sum(dim=1)
+
+    def h(a):
+        return b1 + float((w1 * torch.relu(a * rs + b0)).sum())
+
+    sign = 1.0 if h(1e4) > h(-1e4) else -1.0
+    lo, hi = 0.0, sign * 1e4
+    assert h(hi) > 17.0 > h(lo), "the density MLP does not reach the clamp along (a, a)"
+    for _ in range(100):
+        mid = 0.5 * (lo + hi)
+        lo, hi = (mid, hi) if h(mid) < 17.0 else (lo, mid)
+    sd["encoding.hash_table"][rows] = float(hi)
+    return sd, (o, d, s, e)
+
+
+def interlevel_inputs(R: int, prop_samples, Sc: int, salt: int = 0):
+    """Final-level bins c [R,Sc+1] and weights w [R,Sc] and, per proposal level, bins cp [R,Sp+1] and weights wp [R,Sp]:
+    sorted U(0,1) interior bin edges and softmax weights (sums 0.9 and 0.8)."""
+    def edges(n, s):
+        return torch.sort(torch.cat([torch.zeros(R, 1), (syn.hash_uniform(R * (n - 1), s).view(R, n - 1) + 1) * 0.5, torch.ones(R, 1)], 1), 1).values
+
+    c = edges(Sc, 1 + 100 * salt)
+    w = torch.softmax(syn.hash_uniform(R * Sc, 2 + 100 * salt).view(R, Sc) * 3, -1) * 0.9
+    props = [(edges(Sp, 10 + k + 100 * salt), torch.softmax(syn.hash_uniform(R * Sp, 20 + k + 100 * salt).view(R, Sp) * 2, -1) * 0.8)
+             for k, Sp in enumerate(prop_samples)]
+    return c, w, props
+
+
+def interlevel_reference(c, w, props, ray_weights=None, mult: float = 1.0, dtype=torch.float64):
+    """nerfstudio interlevel_loss (ns.interlevel_loss) with per-ray weights: sum over levels of sum(ray_w * lossfun_outer) / (R*Sc),
+    and its gradient with respect to each level's weights.  Returns (loss, [d loss / d wp])."""
+    R, Sc = w.shape
+    rw = torch.ones(R, dtype=dtype) if ray_weights is None else ray_weights.to(dtype)
+    wps = [wp.detach().to(dtype).requires_grad_(True) for _, wp in props]
+    loss = 0.0
+    for (cp, _), wp in zip(props, wps):
+        loss = loss + (rw[:, None] * ns.lossfun_outer(c, w.to(dtype), cp, wp)).sum() / (R * Sc) * mult
+    loss.backward()
+    return loss.detach(), [wp.grad for wp in wps]
+
+
+def proposal_configs():
+    """{"<method>/L<k>": (DensitySpec, samples per ray, rays per batch)} for each proposal level of the fruit_nerf, fruit_nerf_big
+    and fruit_nerf_huge methods, read from their configs; and {"<method>": (proposal samples, nerf samples)}."""
+    from fruitnerf_b200.fruit_nerf_config import METHODS
+
+    levels, interlevel = {}, {}
+    for name in ("fruit_nerf", "fruit_nerf_big", "fruit_nerf_huge"):
+        m = METHODS[name].pipeline.model
+        R = METHODS[name].pipeline.datamanager.train_num_rays_per_batch
+        for k, S in enumerate(m.num_proposal_samples_per_ray):
+            a = m.proposal_net_args_list[min(k, len(m.proposal_net_args_list) - 1)]
+            spec = fr.DensitySpec(num_levels=a["num_levels"], max_res=a["max_res"], log2_hashmap_size=a["log2_hashmap_size"],
+                                  hidden_dim=a["hidden_dim"])
+            levels[f"{name}/L{k}"] = (spec, S, R)
+        interlevel[name] = (tuple(m.num_proposal_samples_per_ray), m.num_nerf_samples_per_ray)
+    return levels, interlevel
+
+
+def interlevel_bar(f32_grads, ref_grads) -> float:
+    """Bar of the interlevel gradient: GRAD_REL, or twice the float32 oracle's distance from the float64 one if that is larger.
+    The gradient -2 (w - w_outer) / w of each final interval divides the rounding of w_outer, a difference of two entries of
+    the proposal weights' cumulative sum (~2^-24 absolute), by the final weight w: at Sc = 128 final samples the smallest
+    w are ~1e-4 and fp32 arithmetic alone leaves the gradient ~1.1e-3 off the float64 value."""
+    errs = grad_errors({k: g for k, g in enumerate(f32_grads)}, {k: g for k, g in enumerate(ref_grads)})
+    bar = max(GRAD_REL, 2.0 * max(errs.values()))
+    assert bar <= INTERLEVEL_BAR_CAP, f"the float32 interlevel gradient is {max(errs.values()):.3g} off: more than rounding explains"
+    return bar
+
+
+INTERLEVEL_BAR_CAP = 2.5e-3  # fp32 rounding reaches 1.1e-3 at the training shapes; a bar past 2.5e-3 means the reference drifted
