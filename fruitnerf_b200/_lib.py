@@ -249,6 +249,8 @@ EXPORTED_SYMBOLS = (
     "fnr_texture_atlas_size",
     "fnr_texel_rays",
     "fnr_mesh_mean_edge",
+    "fnr_mesh_decimate_scratch_bytes",
+    "fnr_mesh_decimate",
 )
 
 _lib = None
@@ -387,6 +389,10 @@ def load() -> C.CDLL:
     lib.fnr_texel_rays.argtypes = [vp, vp, vp, i64, i32, i32, i32, f32, i64, i32, vp, vp, vp]
     lib.fnr_mesh_mean_edge.restype = C.c_int
     lib.fnr_mesh_mean_edge.argtypes = [vp, vp, i64, vp, vp]
+    lib.fnr_mesh_decimate_scratch_bytes.restype = C.c_int
+    lib.fnr_mesh_decimate_scratch_bytes.argtypes = [i64, i64, C.POINTER(C.c_size_t)]
+    lib.fnr_mesh_decimate.restype = C.c_int
+    lib.fnr_mesh_decimate.argtypes = [vp, vp, i64, i64, i64, vp, sz, vp, vp, vp, _i64p, _i64p, C.POINTER(C.c_int32), vp]
     if lib.fnr_version() != ABI_VERSION:
         raise FruitNerfNativeError(f"ABI version mismatch: library reports {lib.fnr_version()}")
     _lib = lib

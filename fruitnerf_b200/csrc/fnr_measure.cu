@@ -22,6 +22,7 @@
 #include <cmath>
 #include "fnr_common.cuh"
 #include "fnr_kernels.h"
+#include "fnr_mesh_edges.cuh"
 
 namespace fnr {
 
@@ -175,8 +176,7 @@ __global__ void __launch_bounds__(kThreads) sort_inputs_kernel(const int64_t* __
     gkeys[f] = (uint32_t)(g + 1);  // unassigned faces (-1) sort first
     fidx[f] = (int)f;
     for (int k = 0; k < 3; ++k) {
-      const unsigned long long a = (unsigned long long)faces[3 * f + k], b = (unsigned long long)faces[3 * f + (k + 1) % 3];
-      ekeys[3 * f + k] = (a < b ? a : b) * (unsigned long long)V + (a < b ? b : a);
+      ekeys[3 * f + k] = half_edge_key((unsigned long long)faces[3 * f + k], (unsigned long long)faces[3 * f + (k + 1) % 3], (unsigned long long)V);
       egroup[3 * f + k] = g;
     }
   }
@@ -548,12 +548,6 @@ int check_faces(const char* what, const int64_t* faces, long long F, long long V
   return FNR_OK;
 }
 
-int bits_for(unsigned long long n) {  // bits that hold every value below n
-  int b = 1;
-  while (b < 64 && (n - 1) >> b) ++b;
-  return b;
-}
-
 }  // namespace
 
 }  // namespace fnr
@@ -673,9 +667,7 @@ int fnr_mesh_measure_groups(const double* vertices, const int64_t* faces, int64_
                             "cub SortPairs (groups)"))
       return rc;
     tb = s.cub_bytes;
-    if (int rc = check_cuda(cub::DeviceRadixSort::SortPairs(s.cub, tb, s.ekeys_in, s.ekeys, s.egroup_in, s.egroup, (int)(3 * F), 0,
-                                                            bits_for((unsigned long long)V * (unsigned long long)V), st),
-                            "cub SortPairs (edges)"))
+    if (int rc = check_cuda(sort_half_edges(s.cub, tb, s.ekeys_in, s.ekeys, s.egroup_in, s.egroup, 3 * F, V, st), "cub SortPairs (edges)"))
       return rc;
     if (G > 0) {
       edge_classify_kernel<<<blocks(3 * F), kThreads, 0, st>>>(s.ekeys, s.egroup, 3 * F, (unsigned long long*)boundary_edges,

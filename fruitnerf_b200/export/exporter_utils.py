@@ -519,19 +519,46 @@ def export_textured_mesh(pipeline, mesh: Dict, output_dir, prefix: str = "", px_
     return {**paths, "width": W, "height": H, "raylen": raylen}
 
 
-def export_textured_meshes(pipeline, result: Dict, output_dir, px_per_uv_triangle: int = 4) -> Dict[str, str]:
+def decimate_for_texture(mesh: Dict, target_num_faces: int, device) -> Dict:
+    """``mesh`` decimated on the device (fnr_mesh_decimate, DESIGN section 4.3q) to target_num_faces faces or one more,
+    as {'vertices', 'normals' [V',3] fp32, 'faces' [F',3] int64, 'rounds'}; a mesh with at most target_num_faces faces
+    comes back as it is.  A mesh on which no edge can collapse before the target stops early, with a one-line note."""
+    from .. import ops
+
+    faces = np.asarray(mesh["faces"], np.int64).reshape(-1, 3)
+    if len(faces) <= target_num_faces:
+        return mesh
+    t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a, dt)).to(device)  # noqa: E731
+    r = ops.mesh_decimate(t(mesh["vertices"], np.float64).reshape(-1, 3), t(faces, np.int64), int(target_num_faces))
+    out = {"vertices": r["vertices"].to(torch.float32).cpu().numpy(), "normals": r["normals"].to(torch.float32).cpu().numpy(),
+           "faces": r["faces"].cpu().numpy(), "rounds": r["rounds"]}
+    if len(out["faces"]) > target_num_faces + 1:
+        print(f"note: decimation stopped at {len(out['faces'])} faces (target {target_num_faces}): no edge left that can collapse")
+    return out
+
+
+def export_textured_meshes(pipeline, result: Dict, output_dir, px_per_uv_triangle: int = 4,
+                           target_num_faces: Optional[int] = None) -> Dict[str, str]:
     """Texture the scene mesh (``mesh.obj`` / ``material_0.{mtl,png}``) and, unless it is empty, the fruit mesh
     (``fruit_mesh.obj`` / ``fruit_material_0.{mtl,png}``) of an ``export_tsdf_mesh`` / ``export_poisson_mesh`` result.
-    Both atlases are sized first, so an atlas that is too large (texture.AtlasTooLargeError) writes nothing.  Returns the
-    paths, keyed 'mesh_obj', 'mesh_mtl', 'mesh_png' and 'fruit_mesh_obj', ...."""
+    With ``target_num_faces`` each mesh is first decimated to that many faces on its own (``decimate_for_texture``); the
+    PLYs are never decimated.  Both atlases are then sized, so an atlas that is too large for the (decimated) face count
+    (texture.AtlasTooLargeError) writes nothing, and only then rendered.  Returns the paths, keyed 'mesh_obj',
+    'mesh_mtl', 'mesh_png' and 'fruit_mesh_obj', ...."""
     from .. import texture
 
     jobs = [(key, prefix) for key, prefix in (("mesh", ""), ("fruit_mesh", "fruit_")) if len(result[key]["faces"]) > 0]
+    meshes = {key: result[key] for key, _ in jobs}
+    if target_num_faces is not None:
+        dev = next(pipeline.model.parameters()).device
+        if dev.type != "cuda":
+            raise RuntimeError("decimation before texturing needs the model on a CUDA device: fnr_mesh_decimate is a CUDA kernel")
+        meshes = {key: decimate_for_texture(m, int(target_num_faces), dev) for key, m in meshes.items()}
     for key, _ in jobs:
-        texture.atlas_size(len(result[key]["faces"]), px_per_uv_triangle)
+        texture.atlas_size(len(meshes[key]["faces"]), px_per_uv_triangle)
     paths = {}
     for key, prefix in jobs:
-        r = export_textured_mesh(pipeline, result[key], output_dir, prefix, px_per_uv_triangle)
+        r = export_textured_mesh(pipeline, meshes[key], output_dir, prefix, px_per_uv_triangle)
         paths.update({f"{key}_{kind}": r[kind] for kind in ("obj", "mtl", "png")})
     return paths
 

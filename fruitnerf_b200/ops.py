@@ -1290,3 +1290,24 @@ def mesh_mean_edge(vertices: Tensor, faces: Tensor) -> Tensor:
     out = torch.empty(L.FNR_MEAN_EDGE_DOUBLES, dtype=torch.float64, device=dev)
     L.check(L.load().fnr_mesh_mean_edge(_ptr(v), _ptr(f), int(f.shape[0]), _ptr(out), _stream(dev)))
     return out[0]
+
+
+# ======================================================================================================
+# Quadric edge-collapse decimation (fnr_decimate.cu)
+# ======================================================================================================
+def mesh_decimate(vertices: Tensor, faces: Tensor, target_num_faces: int) -> dict:
+    """Decimate a mesh to target_num_faces faces, or one more (fnr_mesh_decimate; decimate.py states the method):
+    {'vertices' [V',3] fp64, 'normals' [V',3] fp64, 'faces' [F',3] int64 on the device, 'rounds'}.  F' is above
+    target + 1 only when a round found no edge it could collapse."""
+    dev, v, f = _mesh_inputs(vertices, faces)
+    V, F = int(v.shape[0]), int(f.shape[0])
+    nbytes = C.c_size_t(0)
+    L.check(L.load().fnr_mesh_decimate_scratch_bytes(V, F, C.byref(nbytes)))
+    buf = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+    ov = torch.empty((V, 3), dtype=torch.float64, device=dev)
+    on = torch.empty((V, 3), dtype=torch.float64, device=dev)
+    of = torch.empty((F, 3), dtype=torch.int64, device=dev)
+    nv, nf, rounds = C.c_int64(0), C.c_int64(0), C.c_int32(0)
+    L.check(L.load().fnr_mesh_decimate(_ptr(v), _ptr(f), V, F, int(target_num_faces), _ptr(buf), nbytes.value, _ptr(ov), _ptr(on), _ptr(of),
+                                       C.byref(nv), C.byref(nf), C.byref(rounds), _stream(dev)))
+    return {"vertices": ov[: nv.value], "normals": on[: nv.value], "faces": of[: nf.value], "rounds": int(rounds.value)}

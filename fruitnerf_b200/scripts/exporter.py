@@ -145,8 +145,9 @@ class ExportTSDFMesh(Exporter):
     """nerfstudio 0.3.2 ExportTSDFMesh: a surface mesh of the scene by TSDF fusion of rendered depth maps, plus the mesh of
     the fruit surfaces (faces whose vertices have a fused fruit probability >= 0.5).  Single GPU.  The PLYs carry vertex
     colours.  ``texture_method="nerf"`` with ``unwrap_method="custom"`` also writes both meshes as OBJs textured by the
-    NeRF, ``px_per_uv_triangle`` texels per face (DESIGN section 4.3p); the xatlas unwrap is not available.  Unlike
-    nerfstudio, the full mesh is textured (no ``target_num_faces`` decimation)."""
+    NeRF, ``px_per_uv_triangle`` texels per face (DESIGN section 4.3p); the xatlas unwrap is not available.
+    ``target_num_faces`` decimates each textured mesh on the GPU first (DESIGN section 4.3q); unlike nerfstudio's 50 000
+    its default is None, the full mesh."""
 
     downscale_factor: int = 2
     depth_output_name: str = "depth"
@@ -161,9 +162,11 @@ class ExportTSDFMesh(Exporter):
     refinement_epsilon: float = 1e-2
     unwrap_method: str = "xatlas"
     px_per_uv_triangle: int = 4
+    target_num_faces: Optional[int] = None
 
     def validate(self) -> None:
         """Refuse what cannot run, before anything is loaded."""
+        _validate_target_num_faces(self.texture_method, self.target_num_faces)
         if self.texture_method not in ("tsdf", "nerf"):
             raise ValueError(f"texture_method must be 'tsdf' or 'nerf', got {self.texture_method!r}")
         _validate_nerf_texture(self.texture_method, self.unwrap_method, self.px_per_uv_triangle, "tsdf")
@@ -195,7 +198,8 @@ class ExportTSDFMesh(Exporter):
                                refine_mesh_using_initial_aabb_estimate=self.refine_mesh_using_initial_aabb_estimate,
                                refinement_epsilon=self.refinement_epsilon)
         if self.texture_method == "nerf":
-            out["paths"].update(export_textured_meshes(pipeline, out, Path(self.output_dir), self.px_per_uv_triangle))
+            out["paths"].update(export_textured_meshes(pipeline, out, Path(self.output_dir), self.px_per_uv_triangle,
+                                                         self.target_num_faces))
         return out
 
 
@@ -205,8 +209,8 @@ class ExportPoissonMesh(Exporter):
     cloud, trimmed at the 0.1 quantile of vertex density, plus the mesh of the fruit surfaces (faces whose vertices have a
     fruit probability >= 0.5).  Single GPU.  The PLYs carry vertex colours.  ``texture_method="nerf"`` with
     ``unwrap_method="custom"`` also writes both meshes as OBJs textured by the NeRF, ``px_per_uv_triangle`` texels per
-    face (DESIGN section 4.3p); the xatlas unwrap is not available.  Unlike nerfstudio, the full mesh is textured (no
-    ``target_num_faces`` decimation).  ``depth`` (open3d's octree depth, here the dense grid's 2^depth cells per axis) is
+    face (DESIGN section 4.3p); the xatlas unwrap is not available.  ``target_num_faces`` decimates each textured mesh on
+    the GPU first (DESIGN section 4.3q); unlike nerfstudio's 50 000 its default is None, the full mesh.  ``depth`` (open3d's octree depth, here the dense grid's 2^depth cells per axis) is
     the one option upstream does not have."""
 
     num_points: int = 1000000
@@ -227,11 +231,13 @@ class ExportPoissonMesh(Exporter):
     depth: int = 9
     unwrap_method: str = "xatlas"
     px_per_uv_triangle: int = 4
+    target_num_faces: Optional[int] = None
 
     def validate(self) -> None:
         """Refuse what cannot run, before anything is loaded."""
         from .. import poisson
 
+        _validate_target_num_faces(self.texture_method, self.target_num_faces)
         if self.texture_method not in ("point_cloud", "nerf"):
             raise ValueError(f"texture_method must be 'point_cloud' or 'nerf', got {self.texture_method!r}")
         _validate_nerf_texture(self.texture_method, self.unwrap_method, self.px_per_uv_triangle, "point_cloud")
@@ -261,7 +267,8 @@ class ExportPoissonMesh(Exporter):
                                   use_bounding_box=self.use_bounding_box, bounding_box_min=self.bounding_box_min,
                                   bounding_box_max=self.bounding_box_max, std_ratio=self.std_ratio, depth=self.depth)
         if self.texture_method == "nerf":
-            out["paths"].update(export_textured_meshes(pipeline, out, Path(self.output_dir), self.px_per_uv_triangle))
+            out["paths"].update(export_textured_meshes(pipeline, out, Path(self.output_dir), self.px_per_uv_triangle,
+                                                         self.target_num_faces))
         return out
 
 
@@ -275,6 +282,17 @@ def _validate_nerf_texture(texture_method: str, unwrap_method: str, px_per_uv_tr
         raise ValueError(f"texture_method 'nerf' with the xatlas UV unwrap needs the xatlas package, which is not available; use "
                          f"--unwrap-method custom (one atlas triangle per face) or texture_method '{vertex_colours}' (vertex colours)")
     check_px_per_uv_triangle(px_per_uv_triangle)
+
+
+def _validate_target_num_faces(texture_method: str, target_num_faces: Optional[int]) -> None:
+    """Decimation only feeds NeRF texturing: without it the option would do nothing."""
+    if target_num_faces is None:
+        return
+    if int(target_num_faces) < 1:
+        raise ValueError(f"target_num_faces must be >= 1, got {target_num_faces}")
+    if texture_method != "nerf":
+        raise ValueError("--target-num-faces decimates the mesh before NeRF texturing and needs --texture-method nerf; the PLYs "
+                         "are never decimated")
 
 
 def _require_normal_output(pipeline, normal_output_name: str) -> None:
@@ -341,6 +359,9 @@ def add_tsdf_parser(sub) -> argparse.ArgumentParser:
     p.add_argument("--refinement-epsilon", type=float, default=d.refinement_epsilon)
     p.add_argument("--unwrap-method", choices=("xatlas", "custom"), default=d.unwrap_method)
     p.add_argument("--px-per-uv-triangle", type=int, default=d.px_per_uv_triangle)
+    p.add_argument("--target-num-faces", type=int, default=None,
+                   help="decimate each textured mesh to this many faces on the GPU first (with --texture-method nerf); "
+                        "default: no decimation, unlike nerfstudio's 50000, so the full mesh is textured")
     return p
 
 
@@ -367,6 +388,9 @@ def add_poisson_parser(sub) -> argparse.ArgumentParser:
     p.add_argument("--depth", type=int, default=d.depth)
     p.add_argument("--unwrap-method", choices=("xatlas", "custom"), default=d.unwrap_method)
     p.add_argument("--px-per-uv-triangle", type=int, default=d.px_per_uv_triangle)
+    p.add_argument("--target-num-faces", type=int, default=None,
+                   help="decimate each textured mesh to this many faces on the GPU first (with --texture-method nerf); "
+                        "default: no decimation, unlike nerfstudio's 50000, so the full mesh is textured")
     return p
 
 
@@ -377,7 +401,7 @@ def poisson_exporter_from_args(a) -> ExportPoissonMesh:
                              use_bounding_box=a.use_bounding_box, bounding_box_min=tuple(a.bounding_box_min),
                              bounding_box_max=tuple(a.bounding_box_max), num_rays_per_batch=a.num_rays_per_batch,
                              texture_method=a.texture_method, std_ratio=a.std_ratio, depth=a.depth, unwrap_method=a.unwrap_method,
-                             px_per_uv_triangle=a.px_per_uv_triangle)
+                             px_per_uv_triangle=a.px_per_uv_triangle, target_num_faces=a.target_num_faces)
 
 
 def _run_mesh_export(exp, parser):
@@ -411,7 +435,7 @@ def tsdf_exporter_from_args(a) -> ExportTSDFMesh:
                           bounding_box_max=tuple(a.bounding_box_max), texture_method=a.texture_method,
                           refine_mesh_using_initial_aabb_estimate=a.refine_mesh_using_initial_aabb_estimate,
                           refinement_epsilon=a.refinement_epsilon, unwrap_method=a.unwrap_method,
-                          px_per_uv_triangle=a.px_per_uv_triangle)
+                          px_per_uv_triangle=a.px_per_uv_triangle, target_num_faces=a.target_num_faces)
 
 
 def entrypoint(argv=None):

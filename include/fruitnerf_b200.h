@@ -68,6 +68,9 @@
  *   fnr_texture_atlas_size, fnr_texel_rays, fnr_mesh_mean_edge
  *                        NeRF textures of the `tsdf` / `poisson` meshes (nerfstudio texture_utils.export_textured_mesh,
  *                        unwrap_method="custom"): the per-face UV atlas, one ray per texel, the ray length
+ *   fnr_mesh_decimate_scratch_bytes, fnr_mesh_decimate
+ *                        quadric edge-collapse decimation of the meshes before NeRF texturing (nerfstudio
+ *                        target_num_faces; pymeshlab meshing_decimation_quadric_edge_collapse)
  */
 #ifndef FRUITNERF_B200_H
 #define FRUITNERF_B200_H
@@ -725,6 +728,43 @@ int fnr_texel_rays(const float* vertices, const float* normals, const int64_t* f
                    int32_t width, int32_t height, float raylen, int64_t texel_start, int32_t num_texels, float* origins, float* directions,
                    void* stream);
 int fnr_mesh_mean_edge(const float* vertices, const int64_t* faces, int64_t num_faces, double* out, void* stream);
+
+/* ---- Quadric edge-collapse decimation (`--target-num-faces` of the tsdf / poisson exports with NeRF texturing;
+ * fnr_decimate.cu; DESIGN section 4.3q) ----
+ * vertices: DEVICE [V,3] fp64; faces: DEVICE [F,3] int64, every index in [0, V) (FNR_ERR_INVALID_ARGUMENT otherwise: a
+ * device check and one host read).  V <= 2^31 - 1 and F <= (2^31 - 1) / 3, else FNR_ERR_UNSUPPORTED; NULL pointers,
+ * negative counts and target_num_faces < 1 return FNR_ERR_INVALID_ARGUMENT.  DEVICE scratch:
+ * fnr_mesh_decimate_scratch_bytes(V, F); nothing is allocated.  Outputs sized to the input: out_vertices,
+ * out_normals DEVICE [V,3] fp64, out_faces DEVICE [F,3] int64, of which the first HOST *out_num_vertices /
+ * *out_num_faces rows are written; HOST *out_rounds counts the rounds that collapsed edges.
+ *
+ * In this order, every fp64 operation rounded where written (no FMA; decimate.py restates it bit for bit):
+ *  1. Quadrics (10 entries xx xy xz xw yy yz yw zz zw ww, each w * (p_i * p_j) of a plane p = (u, -u.x)).  Face f with
+ *     n = (v1 - v0) x (v2 - v0): the plane u = n / |n| through v0, w = |n| / 2.  Each boundary half-edge (its edge in
+ *     one face) from corner k to k + 1, e = v_k+1 - v_k: the plane u = (e x n) / |e x n| through v_k, w = 100 |e|^2.
+ *     A plane with a zero normal adds nothing.  Corner (f, k) adds the face plane, then the boundary planes of
+ *     half-edges k and k + 2; a vertex sums its corners in face order, from 0.
+ *  2. Each round, on the faces as they stand: the 3F half-edge keys min * V + max and the corners by vertex, each
+ *     stably radix-sorted.  An edge (a < b) is a run of equal keys; it is valid when it is in 1 or 2 faces, a != b,
+ *     |N(a) & N(b)| equals its face count, it is not in 2 faces with both ends on a boundary edge, in 2 faces its
+ *     opposite vertices differ and share no face, and every face around a or b not holding both keeps
+ *     dot(n_old, n_new) > 0 with a and b moved to the placement.
+ *  3. Placement: Gaussian elimination with partial pivoting (first largest |pivot|) of the 3x3 system of Q = Q_a + Q_b;
+ *     when a pivot is not above 1e-8 times the largest |diagonal|, the best of v_a, v_b and (v_a + v_b) * 0.5 (ties
+ *     in that order).  Cost = v^T Q v as ((x r0 + y r1) + z r2) + r3, r_i = ((q_i0 x + q_i1 y) + q_i2 z) + q_i3,
+ *     clamped at 0.
+ *  4. Rank = position in a stable sort of the valid edges by the cost's bits (edge order breaks ties); m1[v] = the
+ *     least rank at v, m2[v] = the least m1 over v and its neighbours; an edge is selected when rank = m2[a] = m2[b]
+ *     (selected edges share no face).  In rank order, a selected edge collapses while the face count before it is
+ *     above target + 1: v_a = the placement, Q_a = Q_a + Q_b, b -> a; faces with a repeated index are dropped, the
+ *     rest kept in order.
+ *  5. Rounds end when F <= target + 1 or when a round finds no valid edge (F is then returned as it stands).
+ *  6. Vertices no face uses are dropped in input order; normals = s / |s| with s the sum, in face order, of the
+ *     vertex's (v1 - v0) x (v2 - v0); 0 where s = 0.  One host read per round. */
+int fnr_mesh_decimate_scratch_bytes(int64_t num_vertices, int64_t num_faces, size_t* bytes);
+int fnr_mesh_decimate(const double* vertices, const int64_t* faces, int64_t num_vertices, int64_t num_faces, int64_t target_num_faces,
+                      void* scratch, size_t scratch_bytes, double* out_vertices, double* out_normals, int64_t* out_faces,
+                      int64_t* out_num_vertices, int64_t* out_num_faces, int32_t* out_rounds, void* stream);
 
 /* Hash-grid row indices (exact-integer parity hook): rows[N,L,8] in nerfstudio corner order for
  * the masked [0,1]^3 positions of the given samples; also writes positions[N,3] if non-NULL. */
