@@ -204,6 +204,14 @@ struct Layers {
     dx<SLOT, K, N>(W, dy, dxv);
     dw<SLOT, K, N>(sX, sY, x, dy, gW, gb);
   }
+  // grad of a layer whose input x is a ReLU's output, with dxv masked by that ReLU (x > 0)
+  template <int SLOT, int K, int N>
+  static __device__ __forceinline__ void grad_relu(const float* __restrict__ W, float* sX, float* sY, const float (&x)[K],
+                                                   const float (&dy)[N], float (&dxv)[K], float* gW, float* gb) {
+    grad<SLOT, K, N>(W, sX, sY, x, dy, dxv, gW, gb);
+#pragma unroll
+    for (int k = 0; k < K; ++k) dxv[k] = x[k] > 0.f ? dxv[k] : 0.f;
+  }
 };
 
 // The small family's tensor-core kernels (forward, export, backward) run persistent CTAs of G warpgroups, each warpgroup
@@ -407,16 +415,41 @@ struct ResidentLayers {
   // Both gradients of one layer, the weight gradient first.  A tensor-core layer stages dy once: dW reads the tile
   // weight_grad_acc leaves in step(), and dx runs its MMAs on the same tile, so dy is dead once staged and not live next
   // to dxv (for a 64-wide layer, 64 registers at the backward's peak; DESIGN.md section 4.3).
-  template <int SLOT, int Kv, int Nv>
+  // RELU (grad_relu): x is a ReLU's output and dxv is masked by it.  Once dW has read x, only its signs are needed, so
+  // they are kept as one bit per input (bit k % 32 of word k / 32) and the floats are dead before dx runs.
+  template <int SLOT, int Kv, int Nv, bool RELU = false>
   static __device__ __forceinline__ void grad(const float* __restrict__ W, float* sX, float* sY, const float (&x)[Kv],
                                               const float (&dy)[Nv], float (&dxv)[Kv], float* gW, float* gb) {
     dw<SLOT, Kv, Nv>(sX, sY, x, dy, gW, gb);
+    uint32_t live[RELU ? (Kv + 31) / 32 : 1] = {};
+    if constexpr (RELU) {
+#pragma unroll
+      for (int k = 0; k < Kv; ++k) live[k / 32] |= (x[k] > 0.f ? 1u : 0u) << (k % 32);
+    }
     if constexpr (tensor(Nv)) {
       wg::resident_rowgemm_t_staged<wg::padn(Nv), wg::pad16(Kv), Nv>(step(), smem() + img_off(SLOT), dxv);
       FNR_PHASE(kPhDx);
     } else {
       dx<SLOT, Kv, Nv>(W, dy, dxv);
     }
+    if constexpr (RELU) {
+#pragma unroll
+      for (int k = 0; k < Kv; ++k) dxv[k] = (live[k / 32] >> (k % 32)) & 1u ? dxv[k] : 0.f;
+    }
+  }
+  template <int SLOT, int Kv, int Nv>
+  static __device__ __forceinline__ void grad_relu(const float* __restrict__ W, float* sX, float* sY, const float (&x)[Kv],
+                                                   const float (&dy)[Nv], float (&dxv)[Kv], float* gW, float* gb) {
+    grad<SLOT, Kv, Nv, true>(W, sX, sY, x, dy, dxv, gW, gb);
+  }
+  // m = relu(W x + b) of a chained pair's first layer on its own, by the backward's row path of fwd2: the same tile
+  // bytes, MMAs and fp32 bias and ReLU, so m has the bits fwd2 gives.  The backward recomputes the base MLP's h1 with it.
+  template <int SLOT, int Kv, int Nv>
+  static __device__ __forceinline__ void fwd_relu(const float* __restrict__ b, const float (&x)[Kv], float (&m)[Nv]) {
+    static_assert(K(SLOT) == Kv && N(SLOT) == Nv && tensor(Nv), "slot shape");
+    wg::resident_rowgemm<wg::padn(Nv), wg::pad16(Kv)>(step(), smem() + img_off(SLOT), x, m);
+#pragma unroll
+    for (int n = 0; n < Nv; ++n) m[n] = fmaxf(m[n] + __ldg(b + n), 0.f);
   }
 };
 using ResidentForward = ResidentLayers<ForwardPlan>;
@@ -463,16 +496,23 @@ __device__ __forceinline__ void semantic_fwd(const KParams& P, const float (&geo
   }
 }
 
-// colour branch up to the sigmoid: cat[SH(dir), geo, appearance] -> MLP (fruit_field.py:270-278)
-template <class C, class Lin>
-__device__ __forceinline__ void colour_fwd(const KParams& P, const float* __restrict__ dir, const float (&geo)[C::GEO],
-                                           const float (&app)[C::APP], float (&cin)[C::COL_IN], float (&c1)[C::COL_H],
-                                           float (&c2)[C::COL_H], float (&o3)[3]) {
+// the colour MLP's input cat[SH(dir), geo, appearance]
+template <class C>
+__device__ __forceinline__ void colour_input(const float* __restrict__ dir, const float (&geo)[C::GEO], const float (&app)[C::APP],
+                                             float (&cin)[C::COL_IN]) {
   sh_degree4(dir[0], dir[1], dir[2], cin);
 #pragma unroll
   for (int i = 0; i < C::GEO; ++i) cin[C::SH + i] = geo[i];
 #pragma unroll
   for (int i = 0; i < C::APP; ++i) cin[C::SH + C::GEO + i] = app[i];
+}
+
+// colour branch up to the sigmoid: cat[SH(dir), geo, appearance] -> MLP (fruit_field.py:270-278)
+template <class C, class Lin>
+__device__ __forceinline__ void colour_fwd(const KParams& P, const float* __restrict__ dir, const float (&geo)[C::GEO],
+                                           const float (&app)[C::APP], float (&cin)[C::COL_IN], float (&c1)[C::COL_H],
+                                           float (&c2)[C::COL_H], float (&o3)[3]) {
+  colour_input<C>(dir, geo, app, cin);
   Lin::template fwd2<kCol0, kCol1, C::COL_IN, C::COL_H, C::COL_H, true>(P.col_w[0], P.col_b[0], P.col_w[1], P.col_b[1], cin, c1, c2);
   Lin::template fwd<kCol2, C::COL_H, 3, false>(P.col_w[2], P.col_b[2], c2, o3);
 }
@@ -835,19 +875,23 @@ __global__ void __launch_bounds__(backward_threads<C, TC>()) simt_field_backward
     bool sel;
     const Vec3 pos = field_position(o, d, Rr.starts[pc], Rr.ends[pc], F.position_mode, F.aabb, sel);
     float enc[C::ENC];
-    if (B.stash_encoding) {
-      const float4* st = reinterpret_cast<const float4*>(B.stash_encoding + (size_t)pc * C::ENC);
+    // the point's encoding: the forward's stash, else gathered again at position() (the resident kernel loads it twice)
+    auto load_encoding = [&](auto position) {
+      if (B.stash_encoding) {
+        const float4* st = reinterpret_cast<const float4*>(B.stash_encoding + (size_t)pc * C::ENC);
 #pragma unroll
-      for (int i = 0; i < C::ENC / 4; ++i) {
-        const float4 v = st[i];
-        enc[4 * i] = v.x;
-        enc[4 * i + 1] = v.y;
-        enc[4 * i + 2] = v.z;
-        enc[4 * i + 3] = v.w;
+        for (int i = 0; i < C::ENC / 4; ++i) {
+          const float4 v = st[i];
+          enc[4 * i] = v.x;
+          enc[4 * i + 1] = v.y;
+          enc[4 * i + 2] = v.z;
+          enc[4 * i + 3] = v.w;
+        }
+      } else {
+        hash_encode<C::L>(reinterpret_cast<const float2*>(P.hash_table), F.scalings, F.log2T, position(), enc);
       }
-    } else {
-      hash_encode<C::L>(reinterpret_cast<const float2*>(P.hash_table), F.scalings, F.log2T, pos, enc);
-    }
+    };
+    load_encoding([&] { return pos; });
     const int cam = (F.appearance_mode == FNR_APP_PER_CAMERA) ? Rr.camera_indices[r] : 0;
     float appv[C::APP];
     if constexpr (!kResident) load_appearance(P, F.appearance_mode, cam, s_app, appv);
@@ -860,9 +904,14 @@ __global__ void __launch_bounds__(backward_threads<C, TC>()) simt_field_backward
     FNR_PHASE(kPhLoad);
 
     // The forward is recomputed branch by branch with field_mlps' branch functions, and each branch is back-propagated
-    // right after its forward: only the base MLP's activations live across the whole tile.
+    // right after its forward: only the base MLP's activations live across the whole tile.  The resident kernel keeps
+    // of them only geo and the density's gradient, and recomputes enc and h1 for the base backward (DESIGN.md section 4.3).
     float h1[C::BASE_H], out[C::BASE_OUT], geo[C::GEO];
     base_fwd<C, Lin>(P, enc, h1, out, geo);
+    // trunc_exp backward: g * exp(clamp(x, -15, 15)); density = exp(h0) * selector
+    auto density_grad = [&] { return sel ? d_sigma * expf(fminf(fmaxf(out[0], -15.f), 15.f)) : 0.f; };
+    float dout0 = 0.f;
+    if constexpr (kResident) dout0 = density_grad();
     FNR_PHASE(kPhRecompute);
 
     float d_geo[C::GEO];
@@ -881,15 +930,11 @@ __global__ void __launch_bounds__(backward_threads<C, TC>()) simt_field_backward
       float dz1[C::SEM_H];
       if constexpr (C::SEM_LAYERS == 3) {
         float dz2[C::SEM_H];
-        Lin::template grad<kSem2, C::SEM_H, C::SEM_OUT>(P.sem_w[2], sX, sY, z2, dzo, dz2, G.sem_w[2], G.sem_b[2]);
-#pragma unroll
-        for (int i = 0; i < C::SEM_H; ++i) dz2[i] = z2[i] > 0.f ? dz2[i] : 0.f;
-        Lin::template grad<kSem1, C::SEM_H, C::SEM_H>(P.sem_w[1], sX, sY, z1, dz2, dz1, G.sem_w[1], G.sem_b[1]);
+        Lin::template grad_relu<kSem2, C::SEM_H, C::SEM_OUT>(P.sem_w[2], sX, sY, z2, dzo, dz2, G.sem_w[2], G.sem_b[2]);
+        Lin::template grad_relu<kSem1, C::SEM_H, C::SEM_H>(P.sem_w[1], sX, sY, z1, dz2, dz1, G.sem_w[1], G.sem_b[1]);
       } else {
-        Lin::template grad<kSem1, C::SEM_H, C::SEM_OUT>(P.sem_w[1], sX, sY, z1, dzo, dz1, G.sem_w[1], G.sem_b[1]);
+        Lin::template grad_relu<kSem1, C::SEM_H, C::SEM_OUT>(P.sem_w[1], sX, sY, z1, dzo, dz1, G.sem_w[1], G.sem_b[1]);
       }
-#pragma unroll
-      for (int i = 0; i < C::SEM_H; ++i) dz1[i] = z1[i] > 0.f ? dz1[i] : 0.f;
       Lin::template dw<kSem0, C::GEO, C::SEM_H>(sX, sY, geo, dz1, G.sem_w[0], G.sem_b[0]);
       if (F.pass_semantic_gradients) {
         float dg[C::GEO];
@@ -913,12 +958,13 @@ __global__ void __launch_bounds__(backward_threads<C, TC>()) simt_field_backward
         do3[i] = d_rgb[i] * rgb * (1.0f - rgb);
       }
       float dc2[C::COL_H], dc1[C::COL_H], dcin[C::COL_IN];
-      Lin::template grad<kCol2, C::COL_H, 3>(P.col_w[2], sX, sY, c2, do3, dc2, G.col_w[2], G.col_b[2]);
-#pragma unroll
-      for (int i = 0; i < C::COL_H; ++i) dc2[i] = c2[i] > 0.f ? dc2[i] : 0.f;
-      Lin::template grad<kCol1, C::COL_H, C::COL_H>(P.col_w[1], sX, sY, c1, dc2, dc1, G.col_w[1], G.col_b[1]);
-#pragma unroll
-      for (int i = 0; i < C::COL_H; ++i) dc1[i] = c1[i] > 0.f ? dc1[i] : 0.f;
+      Lin::template grad_relu<kCol2, C::COL_H, 3>(P.col_w[2], sX, sY, c2, do3, dc2, G.col_w[2], G.col_b[2]);
+      Lin::template grad_relu<kCol1, C::COL_H, C::COL_H>(P.col_w[1], sX, sY, c1, dc2, dc1, G.col_w[1], G.col_b[1]);
+      if constexpr (kResident) {
+        // cin again, from what built it, rather than carried through the col2 and col1 gradients
+        load_appearance(P, F.appearance_mode, cam, s_app, appv);
+        colour_input<C>(d, geo, appv, cin);
+      }
       Lin::template grad<kCol0, C::COL_IN, C::COL_H>(P.col_w[0], sX, sY, cin, dc1, dcin, G.col_w[0], G.col_b[0]);
 #pragma unroll
       for (int i = 0; i < C::GEO; ++i) d_geo[i] += dcin[C::SH + i];
@@ -950,14 +996,21 @@ __global__ void __launch_bounds__(backward_threads<C, TC>()) simt_field_backward
     float denc[C::ENC];
     {
       float dout[C::BASE_OUT];
-      // trunc_exp backward: g * exp(clamp(x, -15, 15)); density = exp(h0) * selector
-      dout[0] = sel ? d_sigma * expf(fminf(fmaxf(out[0], -15.f), 15.f)) : 0.f;
+      dout[0] = kResident ? dout0 : density_grad();
 #pragma unroll
       for (int i = 0; i < C::GEO; ++i) dout[1 + i] = d_geo[i];
+      if constexpr (kResident) {
+        // enc and h1 = relu(base0 enc + b0) again, h1 by the recompute's own row path, so its bits and ReLU mask are the
+        // forward's; base1's output is needed only as dout[0]
+        load_encoding([&] {
+          bool s;
+          return field_position(o, d, Rr.starts[pc], Rr.ends[pc], F.position_mode, F.aabb, s);
+        });
+        Lin::template fwd_relu<kBase0, C::ENC, C::BASE_H>(P.base_b[0], enc, h1);
+        FNR_PHASE(kPhRecompute);
+      }
       float dh1[C::BASE_H];
-      Lin::template grad<kBase1, C::BASE_H, C::BASE_OUT>(P.base_w[1], sX, sY, h1, dout, dh1, G.base_w[1], G.base_b[1]);
-#pragma unroll
-      for (int i = 0; i < C::BASE_H; ++i) dh1[i] = h1[i] > 0.f ? dh1[i] : 0.f;
+      Lin::template grad_relu<kBase1, C::BASE_H, C::BASE_OUT>(P.base_w[1], sX, sY, h1, dout, dh1, G.base_w[1], G.base_b[1]);
       Lin::template grad<kBase0, C::ENC, C::BASE_H>(P.base_w[0], sX, sY, enc, dh1, denc, G.base_w[0], G.base_b[0]);
     }
     // ---- hash-table gradient -----------------------------------------------------------------

@@ -353,6 +353,20 @@ __device__ __forceinline__ void resident_rowgemm_t(uint8_t* smem, const uint8_t*
   resident_rowgemm_t_staged<NPF, KPF, R, NO>(smem, img, y);
 }
 
+// y = W x (before its bias) with the weights from a resident split image (W [NPF][KPF]) read K-major, x staged as a row
+// tile and the result rows stored over it, one M half at a time.  smem is the warpgroup's kResidentStepBytes.
+template <int NPF, int KPF, int R, int NO>
+__device__ __forceinline__ void resident_rowgemm(uint8_t* smem, const uint8_t* img, const float (&x)[R], float (&y)[NO]) {
+  constexpr int KP = pad16(R), NP = padn(NO);
+  static_assert(KP == KPF && NP == NPF, "layer outside the resident image");
+  static_assert(2 * 128 * KP * 2 <= kResidentStepBytes && NP * 128 * 4 <= kResidentStepBytes, "resident step plan");
+  float* ys = reinterpret_cast<float*>(smem);
+  stage_rows(smem, x);
+  layer_mma<KP, NP, 0, true>(smem_u32(smem), 128 * KP * 2, image_operand<NPF, KPF, false>(img), ys, 4, kRowsGroupStride);
+  sync();
+  read_row<NO>(ys, 4, kRowsGroupStride, y);
+}
+
 // Two forward layers chained fragment to fragment: m = epi0(W0 x), y = W1 m (before its bias), both weights from the
 // resident image (img0: W0 [NPF0][KPF0], img1: W1 [NPF1][NPF0]).  The first layer's MMAs end in registers (both M halves
 // in flight); epi0(c, v) (column c of value v: the bias and ReLU) runs on them in fragment order, and they are stored as
@@ -370,15 +384,13 @@ __device__ __forceinline__ void resident_chain(uint8_t* smem, const uint8_t* img
                 "resident step plan");
   const uint32_t tile = smem_u32(smem);
   float* ys = reinterpret_cast<float*>(smem);
-  stage_rows(smem, x);
   if constexpr (KEEP_MID) {
-    layer_mma<KP, NM, 0, true>(tile, 128 * KP * 2, image_operand<NPF0, KPF0, false>(img0), ys, 4, kRowsGroupStride);
-    sync();
-    read_row<NM>(ys, 4, kRowsGroupStride, mid);
+    resident_rowgemm<NPF0, KPF0>(smem, img0, x, mid);
 #pragma unroll
     for (int n = 0; n < NM; ++n) mid[n] = epi0(n, mid[n]);
     stage_rows(smem, mid);
   } else {
+    stage_rows(smem, x);
     const int lane = tid() & 31;
     float d[2][NM / 2];
     layer_mma_frag<KP, NM, 0>(tile, 128 * KP * 2, image_operand<NPF0, KPF0, false>(img0), d);
