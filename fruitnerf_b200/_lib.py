@@ -187,6 +187,11 @@ FNR_MAX_ADAM_TENSORS = 48
 FNR_IMAGE_RECORD_DOUBLES = 12
 FNR_TEXTURE_MAX_SIDE = 16384
 FNR_MEAN_EDGE_DOUBLES = 1 + 256
+FNR_UNWRAP_MIN_SIDE = 16
+FNR_UNWRAP_MARGIN = 3
+FNR_UNWRAP_GUTTER = 2
+FNR_UNWRAP_BISECTIONS = 40
+FNR_UNWRAP_STAGES = 5
 # record slots of fnr_image_stats / fnr_ssim (FNR_REC_* of the header), in order
 IMAGE_RECORD_FIELDS = ("sse", "rgb_min", "rgb_max", "image_min", "image_max", "accumulation_sum", "fruit_tp", "fruit_fp", "fruit_fn",
                        "fruit_tn", "ssim", "data_range")
@@ -251,6 +256,9 @@ EXPORTED_SYMBOLS = (
     "fnr_mesh_mean_edge",
     "fnr_mesh_decimate_scratch_bytes",
     "fnr_mesh_decimate",
+    "fnr_chart_unwrap_scratch_bytes",
+    "fnr_chart_unwrap",
+    "fnr_chart_texel_rays",
 )
 
 _lib = None
@@ -393,6 +401,13 @@ def load() -> C.CDLL:
     lib.fnr_mesh_decimate_scratch_bytes.argtypes = [i64, i64, C.POINTER(C.c_size_t)]
     lib.fnr_mesh_decimate.restype = C.c_int
     lib.fnr_mesh_decimate.argtypes = [vp, vp, i64, i64, i64, vp, sz, vp, vp, vp, _i64p, _i64p, C.POINTER(C.c_int32), vp]
+    lib.fnr_chart_unwrap_scratch_bytes.restype = C.c_int
+    lib.fnr_chart_unwrap_scratch_bytes.argtypes = [i64, i64, i32, C.POINTER(C.c_size_t)]
+    lib.fnr_chart_unwrap.restype = C.c_int
+    lib.fnr_chart_unwrap.argtypes = [vp, vp, i64, i64, i32, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, C.POINTER(C.c_int32), _i64p, f64p, _i64p,
+                                     f64p, vp]
+    lib.fnr_chart_texel_rays.restype = C.c_int
+    lib.fnr_chart_texel_rays.argtypes = [vp, vp, vp, i64, vp, vp, i64, f32, i64, i32, vp, vp, vp]
     if lib.fnr_version() != ABI_VERSION:
         raise FruitNerfNativeError(f"ABI version mismatch: library reports {lib.fnr_version()}")
     _lib = lib

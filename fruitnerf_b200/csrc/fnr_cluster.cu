@@ -29,6 +29,7 @@
 #include "fnr_common.cuh"
 #include "fnr_grid.cuh"
 #include "fnr_kernels.h"
+#include "fnr_union_find.cuh"
 
 namespace fnr {
 
@@ -138,31 +139,7 @@ __global__ void __launch_bounds__(kThreads) radius_count_multi_kernel(Grid g, Ra
 }
 
 // ---- DBSCAN ---------------------------------------------------------------------------------------------------------
-// Union-find over input indices.  parent[i] <= i always holds (a root is only ever hooked under a smaller root), so the
-// root of a component is its smallest core index whatever order the CAS operations land in.
-__device__ __forceinline__ int find_root(volatile int* parent, int i) {
-  int cur = parent[i];
-  if (cur != i) {
-    int prev = i, next;
-    while (cur > (next = parent[cur])) {  // path halving; a stale read only sees a larger (still valid) ancestor
-      parent[prev] = next;
-      prev = cur;
-      cur = next;
-    }
-  }
-  return cur;
-}
-
-__device__ __forceinline__ void unite(int* parent, int a, int b) {
-  int ra = find_root(parent, a), rb = find_root(parent, b);
-  while (ra != rb) {
-    const int lo = min(ra, rb), hi = max(ra, rb);
-    const int old = atomicCAS(parent + hi, hi, lo);
-    if (old == hi) return;
-    ra = find_root(parent, old);
-    rb = find_root(parent, lo);
-  }
-}
+// Union-find over input indices (fnr_union_find.cuh): the root of a component is its smallest core index.
 
 __global__ void __launch_bounds__(kThreads) cell_min_core_kernel(Grid g, const int* __restrict__ core, int* __restrict__ cmin) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;

@@ -2,6 +2,7 @@
 // section 4.3p):
 //   texel_rays_kernel      the per-face UV atlas in closed form: texel -> (face, barycentrics of the closest point of the
 //                          face's UV triangle) -> one short ray from just outside the surface along the inverted normal
+//   chart_rays_kernel      the same ray (texel_ray) for the owned texels of a chart atlas (fnr_unwrap.cu, DESIGN 4.3r)
 //   mean_edge_partials     raylen = 2 * mean first-edge length: per-block fp64 sums over fixed face ranges, then one
 //   mean_edge_finish       fixed-order finish (no atomics, so repeated calls give identical bits)
 // The atlas layout is written out in include/fruitnerf_b200.h; fruitnerf_b200/texture.py restates both kernels.
@@ -46,39 +47,22 @@ __device__ __forceinline__ float norm3(const float v[3]) {
   return __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(v[0], v[0]), __fmul_rn(v[1], v[1])), __fmul_rn(v[2], v[2])));
 }
 
-__global__ void __launch_bounds__(kThreads) texel_rays_kernel(KTexelRays A) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= A.n) return;
-  const long long t = A.t0 + i;
-  const int row = (int)(t / A.width), col = (int)(t % A.width);
-  const int p = A.p, bw = p + 3;
-  const int a = col % bw, b = row % p;
-  const long long block = (long long)(row / p) * A.blocks_x + col / bw;
-  const int half = a + b >= p + 1;
-  const long long slot = 2 * block + half;
-  const long long f = slot < A.num_faces ? slot : A.num_faces - 1;
-  // the texel centre in its slot's frame, where the UV triangle is (0,0), (p-1,0), (0,p-1); its closest point (xs, ys)
-  const int la = half ? p + 2 - a : a, lb = half ? p - 1 - b : b;
-  float xs = (float)la, ys = (float)lb;
-  if (la + lb > p - 1) {  // gutter: project onto the hypotenuse x + y = p - 1, clamped to its end points
-    xs = fminf(fmaxf(xs - 0.5f, 0.f), (float)(p - 1));
-    ys = (float)(p - 1) - xs;
-  }
-  const float pm1 = (float)(p - 1);
-  const float s = __fdiv_rn(xs, pm1), u = __fdiv_rn(ys, pm1);
-  const float w0 = __fsub_rn(__fsub_rn(1.f, s), u);
-  const int64_t* fv = A.faces + 3 * f;
+// The ray of the surface point with barycentrics (w0, w1, w2) of face fv (texel_rays_kernel and chart_rays_kernel):
+// position and normal interpolated in fp32 without FMA, the face normal where the interpolated one vanishes, then the
+// origin 0.5 raylen outside the surface along the normal and the inverted normal as direction.
+__device__ __forceinline__ void texel_ray(const float* vertices, const float* normals, const int64_t* fv, float w0, float w1, float w2,
+                                          float half_len, float* origin, float* direction) {
   float v0[3], v1[3], v2[3], x[3], n[3];
-  load3(A.vertices, fv[0], v0);
-  load3(A.vertices, fv[1], v1);
-  load3(A.vertices, fv[2], v2);
-  interp3(w0, s, u, v0, v1, v2, x);
+  load3(vertices, fv[0], v0);
+  load3(vertices, fv[1], v1);
+  load3(vertices, fv[2], v2);
+  interp3(w0, w1, w2, v0, v1, v2, x);
   {
     float n0[3], n1[3], n2[3];
-    load3(A.normals, fv[0], n0);
-    load3(A.normals, fv[1], n1);
-    load3(A.normals, fv[2], n2);
-    interp3(w0, s, u, n0, n1, n2, n);
+    load3(normals, fv[0], n0);
+    load3(normals, fv[1], n1);
+    load3(normals, fv[2], n2);
+    interp3(w0, w1, w2, n0, n1, n2, n);
   }
   float len = norm3(n);
   if (!(len > 1e-12f)) {  // vanishing (or NaN) interpolated normal: the right-hand face normal
@@ -102,9 +86,46 @@ __global__ void __launch_bounds__(kThreads) texel_rays_kernel(KTexelRays A) {
 #pragma unroll
   for (int k = 0; k < 3; ++k) {
     const float nk = __fdiv_rn(n[k], len);
-    A.origins[3 * (size_t)i + k] = __fadd_rn(x[k], __fmul_rn(A.half_len, nk));
-    A.directions[3 * (size_t)i + k] = -nk;
+    origin[k] = __fadd_rn(x[k], __fmul_rn(half_len, nk));
+    direction[k] = -nk;
   }
+}
+
+__global__ void __launch_bounds__(kThreads) texel_rays_kernel(KTexelRays A) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= A.n) return;
+  const long long t = A.t0 + i;
+  const int row = (int)(t / A.width), col = (int)(t % A.width);
+  const int p = A.p, bw = p + 3;
+  const int a = col % bw, b = row % p;
+  const long long block = (long long)(row / p) * A.blocks_x + col / bw;
+  const int half = a + b >= p + 1;
+  const long long slot = 2 * block + half;
+  const long long f = slot < A.num_faces ? slot : A.num_faces - 1;
+  // the texel centre in its slot's frame, where the UV triangle is (0,0), (p-1,0), (0,p-1); its closest point (xs, ys)
+  const int la = half ? p + 2 - a : a, lb = half ? p - 1 - b : b;
+  float xs = (float)la, ys = (float)lb;
+  if (la + lb > p - 1) {  // gutter: project onto the hypotenuse x + y = p - 1, clamped to its end points
+    xs = fminf(fmaxf(xs - 0.5f, 0.f), (float)(p - 1));
+    ys = (float)(p - 1) - xs;
+  }
+  const float pm1 = (float)(p - 1);
+  const float s = __fdiv_rn(xs, pm1), u = __fdiv_rn(ys, pm1);
+  const float w0 = __fsub_rn(__fsub_rn(1.f, s), u);
+  texel_ray(A.vertices, A.normals, A.faces + 3 * f, w0, s, u, A.half_len, A.origins + 3 * (size_t)i, A.directions + 3 * (size_t)i);
+}
+
+// Rays of the owned texels of a chart atlas (fnr_chart_unwrap's compacted face and barycentrics per texel)
+__global__ void __launch_bounds__(kThreads) chart_rays_kernel(const float* __restrict__ vertices, const float* __restrict__ normals,
+                                                              const int64_t* __restrict__ faces, const int32_t* __restrict__ texel_faces,
+                                                              const float* __restrict__ barycentrics, long long t0, int n, float half_len,
+                                                              float* __restrict__ origins, float* __restrict__ directions) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const long long t = t0 + i;
+  const float* w = barycentrics + 3 * t;
+  texel_ray(vertices, normals, faces + 3 * (long long)texel_faces[t], w[0], w[1], w[2], half_len, origins + 3 * (size_t)i,
+            directions + 3 * (size_t)i);
 }
 
 // Sum over the block in a fixed tree (xor shuffles, then warp 0 over the warp sums); the total is valid in thread 0.
@@ -208,6 +229,24 @@ int fnr_texel_rays(const float* vertices, const float* normals, const int64_t* f
                origins, directions};
   texel_rays_kernel<<<(num_texels + kThreads - 1) / kThreads, kThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(A);
   return check_launch("texel_rays_kernel");
+}
+
+int fnr_chart_texel_rays(const float* vertices, const float* normals, const int64_t* faces, int64_t num_faces, const int32_t* texel_faces,
+                         const float* barycentrics, int64_t num_owned, float raylen, int64_t texel_start, int32_t num_texels, float* origins,
+                         float* directions, void* stream) {
+  if (!vertices || !normals || !faces || !texel_faces || !barycentrics || !origins || !directions) {
+    set_error("fnr_chart_texel_rays: NULL pointer");
+    return FNR_ERR_INVALID_ARGUMENT;
+  }
+  if (num_faces < 1 || num_texels < 0 || texel_start < 0 || texel_start + num_texels > num_owned || !(raylen > 0.f) || !std::isfinite(raylen)) {
+    set_error("fnr_chart_texel_rays: %lld faces, texels [%lld, %lld) of %lld owned, raylen %g", (long long)num_faces, (long long)texel_start,
+              (long long)texel_start + num_texels, (long long)num_owned, (double)raylen);
+    return FNR_ERR_INVALID_ARGUMENT;
+  }
+  if (num_texels == 0) return FNR_OK;
+  chart_rays_kernel<<<(num_texels + kThreads - 1) / kThreads, kThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      vertices, normals, faces, texel_faces, barycentrics, texel_start, num_texels, 0.5f * raylen, origins, directions);
+  return check_launch("chart_rays_kernel");
 }
 
 int fnr_mesh_mean_edge(const float* vertices, const int64_t* faces, int64_t num_faces, double* out, void* stream) {

@@ -469,16 +469,22 @@ def export_poisson_mesh(pipeline, output_dir, num_points: int = 1000000, remove_
 
 
 @torch.no_grad()
-def export_textured_mesh(pipeline, mesh: Dict, output_dir, prefix: str = "", px_per_uv_triangle: int = 4) -> Dict:
-    """nerfstudio texture_utils.export_textured_mesh with ``unwrap_method="custom"`` on the GPU, for one mesh dict of
-    ``export_tsdf_mesh`` / ``export_poisson_mesh`` ('vertices', 'normals', 'faces').  Every face gets its own triangle of
-    the atlas (texture.py), and every texel one ray from 0.5 raylen outside the surface along the inverted normal, near 0,
-    far raylen, camera 0, with raylen = 2 * the mean first-edge length (fnr_mesh_mean_edge).  The rays (fnr_texel_rays)
-    go through the model chunk by chunk on the device, the ``rgb`` output is quantised by fnr_compose_frame, and one
-    device-to-host copy gives the image.
+def export_textured_mesh(pipeline, mesh: Dict, output_dir, prefix: str = "", px_per_uv_triangle: int = 4, unwrap_method: str = "custom",
+                         num_pixels_per_side: int = 1024, unwrap: Optional[Dict] = None) -> Dict:
+    """nerfstudio texture_utils.export_textured_mesh on the GPU, for one mesh dict of ``export_tsdf_mesh`` /
+    ``export_poisson_mesh`` ('vertices', 'normals', 'faces').  The rays are cast from 0.5 raylen outside the surface along
+    the inverted normal, near 0, far raylen, camera 0, with raylen = 2 * the mean first-edge length (fnr_mesh_mean_edge);
+    they go through the model chunk by chunk on the device, the ``rgb`` output is quantised by fnr_compose_frame, and one
+    device-to-host copy gives the colours.
+
+    * ``unwrap_method="custom"`` (nerfstudio's): every face gets its own triangle of the atlas (texture.py), and every
+      texel a ray (fnr_texel_rays).
+    * ``unwrap_method="charts"`` (DESIGN section 4.3r): the ``num_pixels_per_side``-square chart atlas of
+      ``chart_unwrap_mesh`` (pass ``unwrap`` to reuse one); only the owned texels get a ray (fnr_chart_texel_rays), the
+      others stay black.
 
     Writes ``{prefix}mesh.obj``, ``{prefix}material_0.mtl`` and ``{prefix}material_0.png`` under ``output_dir``.  Returns
-    {'obj', 'mtl', 'png': paths, 'width', 'height', 'raylen'}.  An atlas side over texture.MAX_SIDE raises
+    {'obj', 'mtl', 'png': paths, 'width', 'height', 'raylen'}.  An atlas that cannot be made raises
     texture.AtlasTooLargeError before anything is rendered or written."""
     from PIL import Image
 
@@ -490,14 +496,22 @@ def export_textured_mesh(pipeline, mesh: Dict, output_dir, prefix: str = "", px_
     dev = next(model.parameters()).device
     if dev.type != "cuda":
         raise RuntimeError("export_textured_mesh needs the model on a CUDA device: the texel rays are a CUDA kernel")
-    p = texture.check_px_per_uv_triangle(px_per_uv_triangle)
+    if unwrap_method not in ("custom", "charts"):
+        raise ValueError(f"unwrap_method must be 'custom' or 'charts', got {unwrap_method!r}")
     faces = np.asarray(mesh["faces"], np.int64).reshape(-1, 3)
-    W, H = texture.atlas_size(len(faces), p)
+    if unwrap_method == "charts":
+        if unwrap is None:
+            unwrap = chart_unwrap_mesh(mesh, num_pixels_per_side, dev)
+        W = H = texture.check_num_pixels_per_side(num_pixels_per_side)
+        P = int(unwrap["num_owned"])
+    else:
+        p = texture.check_px_per_uv_triangle(px_per_uv_triangle)
+        W, H = texture.atlas_size(len(faces), p)
+        P = W * H
     t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a, dt)).to(dev)  # noqa: E731
     verts, nrms, fdev = t(mesh["vertices"], np.float32).reshape(-1, 3), t(mesh["normals"], np.float32).reshape(-1, 3), t(faces, np.int64)
     raylen = float(np.float32(2.0 * float(ops.mesh_mean_edge(verts, fdev))))
-    P = W * H
-    chunk = min(int(model.config.eval_num_rays_per_chunk), P)
+    chunk = max(1, min(int(model.config.eval_num_rays_per_chunk), P))
     o_buf = torch.empty((chunk, 3), dtype=torch.float32, device=dev)
     d_buf = torch.empty((chunk, 3), dtype=torch.float32, device=dev)
     cam_idx = torch.zeros((chunk, 1), dtype=torch.long, device=dev)
@@ -505,18 +519,39 @@ def export_textured_mesh(pipeline, mesh: Dict, output_dir, prefix: str = "", px_
     fars = torch.full((chunk, 1), raylen, dtype=torch.float32, device=dev)
 
     def chunk_rays(t0: int, n: int) -> RayBundle:
-        o, d = ops.texel_rays(verts, nrms, fdev, p, W, H, raylen, t0, n, out=(o_buf, d_buf))
+        if unwrap_method == "charts":
+            o, d = ops.chart_texel_rays(verts, nrms, fdev, unwrap["texel_faces"], unwrap["barycentrics"], raylen, t0, n, out=(o_buf, d_buf))
+        else:
+            o, d = ops.texel_rays(verts, nrms, fdev, p, W, H, raylen, t0, n, out=(o_buf, d_buf))
         return RayBundle(origins=o, directions=d, camera_indices=cam_idx[:n], nears=nears[:n], fars=fars[:n])
 
     bufs = render_into_buffers(model, chunk_rays, P, chunk, ["rgb"], {}, lambda _stage: None)
-    image = ops.compose_frame([ops.FrameImage(bufs["rgb"], "color")], None, H, W, _turbo_table(dev)).cpu().numpy()
+    if unwrap_method == "charts":  # the owned texels' colours, scattered into a black image
+        colours = ops.compose_frame([ops.FrameImage(bufs["rgb"], "color")], None, 1, P, _turbo_table(dev)).cpu().numpy().reshape(P, 3)
+        image = np.zeros((H * W, 3), np.uint8)
+        image[unwrap["texels"].cpu().numpy()] = colours
+        image = image.reshape(H, W, 3)
+        uv = texture.chart_vt(unwrap["uv"].cpu().numpy(), W)
+    else:
+        image = ops.compose_frame([ops.FrameImage(bufs["rgb"], "color")], None, H, W, _turbo_table(dev)).cpu().numpy()
+        uv = texture.uv_coordinates(len(faces), p)
     out_dir = pathlib.Path(output_dir)
     out_dir.mkdir(parents=True, exist_ok=True)
     mtl, png = f"{prefix}material_0.mtl", f"{prefix}material_0.png"
     paths = {"obj": str(out_dir / f"{prefix}mesh.obj"), "mtl": str(out_dir / mtl), "png": str(out_dir / png)}
     Image.fromarray(image).save(paths["png"])
-    texture.write_textured_obj(paths["obj"], mtl, png, mesh["vertices"], mesh["normals"], faces, texture.uv_coordinates(len(faces), p))
+    texture.write_textured_obj(paths["obj"], mtl, png, mesh["vertices"], mesh["normals"], faces, uv)
     return {**paths, "width": W, "height": H, "raylen": raylen}
+
+
+def chart_unwrap_mesh(mesh: Dict, num_pixels_per_side: int, device) -> Dict:
+    """The `charts` atlas of ``mesh`` (ops.chart_unwrap, DESIGN section 4.3r) on ``device``; texture.AtlasTooLargeError when
+    its charts do not fit into num_pixels_per_side^2 texels."""
+    from .. import texture
+
+    N = texture.check_num_pixels_per_side(num_pixels_per_side)
+    t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a, dt)).to(device)  # noqa: E731
+    return ops.chart_unwrap(t(mesh["vertices"], np.float32).reshape(-1, 3), t(np.asarray(mesh["faces"]).reshape(-1, 3), np.int64), N)
 
 
 def decimate_for_texture(mesh: Dict, target_num_faces: int, device) -> Dict:
@@ -538,27 +573,35 @@ def decimate_for_texture(mesh: Dict, target_num_faces: int, device) -> Dict:
 
 
 def export_textured_meshes(pipeline, result: Dict, output_dir, px_per_uv_triangle: int = 4,
-                           target_num_faces: Optional[int] = None) -> Dict[str, str]:
+                           target_num_faces: Optional[int] = None, unwrap_method: str = "custom",
+                           num_pixels_per_side: int = 1024) -> Dict[str, str]:
     """Texture the scene mesh (``mesh.obj`` / ``material_0.{mtl,png}``) and, unless it is empty, the fruit mesh
     (``fruit_mesh.obj`` / ``fruit_material_0.{mtl,png}``) of an ``export_tsdf_mesh`` / ``export_poisson_mesh`` result.
     With ``target_num_faces`` each mesh is first decimated to that many faces on its own (``decimate_for_texture``); the
-    PLYs are never decimated.  Both atlases are then sized, so an atlas that is too large for the (decimated) face count
-    (texture.AtlasTooLargeError) writes nothing, and only then rendered.  Returns the paths, keyed 'mesh_obj',
-    'mesh_mtl', 'mesh_png' and 'fruit_mesh_obj', ...."""
+    PLYs are never decimated.  Both atlases are then sized (``custom``) or unwrapped (``charts``), so an atlas that cannot
+    be made for either mesh (texture.AtlasTooLargeError) writes nothing, and only then rendered.  Returns the paths, keyed
+    'mesh_obj', 'mesh_mtl', 'mesh_png' and 'fruit_mesh_obj', ...."""
     from .. import texture
 
     jobs = [(key, prefix) for key, prefix in (("mesh", ""), ("fruit_mesh", "fruit_")) if len(result[key]["faces"]) > 0]
     meshes = {key: result[key] for key, _ in jobs}
+    dev = next(pipeline.model.parameters()).device
     if target_num_faces is not None:
-        dev = next(pipeline.model.parameters()).device
         if dev.type != "cuda":
             raise RuntimeError("decimation before texturing needs the model on a CUDA device: fnr_mesh_decimate is a CUDA kernel")
         meshes = {key: decimate_for_texture(m, int(target_num_faces), dev) for key, m in meshes.items()}
+    unwraps = {}
     for key, _ in jobs:
-        texture.atlas_size(len(meshes[key]["faces"]), px_per_uv_triangle)
+        if unwrap_method == "charts":
+            if dev.type != "cuda":
+                raise RuntimeError("the charts unwrap needs the model on a CUDA device: fnr_chart_unwrap is a CUDA kernel")
+            unwraps[key] = chart_unwrap_mesh(meshes[key], num_pixels_per_side, dev)
+        else:
+            texture.atlas_size(len(meshes[key]["faces"]), px_per_uv_triangle)
     paths = {}
     for key, prefix in jobs:
-        r = export_textured_mesh(pipeline, meshes[key], output_dir, prefix, px_per_uv_triangle)
+        r = export_textured_mesh(pipeline, meshes[key], output_dir, prefix, px_per_uv_triangle, unwrap_method, num_pixels_per_side,
+                                 unwraps.get(key))
         paths.update({f"{key}_{kind}": r[kind] for kind in ("obj", "mtl", "png")})
     return paths
 

@@ -1311,3 +1311,64 @@ def mesh_decimate(vertices: Tensor, faces: Tensor, target_num_faces: int) -> dic
     L.check(L.load().fnr_mesh_decimate(_ptr(v), _ptr(f), V, F, int(target_num_faces), _ptr(buf), nbytes.value, _ptr(ov), _ptr(on), _ptr(of),
                                        C.byref(nv), C.byref(nf), C.byref(rounds), _stream(dev)))
     return {"vertices": ov[: nv.value], "normals": on[: nv.value], "faces": of[: nf.value], "rounds": int(rounds.value)}
+
+
+# ======================================================================================================
+# The `charts` UV unwrap (fnr_unwrap.cu, fnr_texture.cu; texture.py restates it)
+# ======================================================================================================
+def chart_unwrap(vertices: Tensor, faces: Tensor, num_pixels_per_side: int, timing: bool = False) -> dict:
+    """The chart atlas of a mesh (fnr_chart_unwrap): vertices [V,3] fp32 and faces [F,3] int64 on the device ->
+    {'labels', 'charts' [F] int32, 'offsets' [C,2] int32, 'uv' [F,3,2] fp64 texel coordinates, 'owner' [N*N] int32,
+    'texels', 'texel_faces' [n] int32, 'barycentrics' [n,3] fp32 of the n owned texels in texel order, all on the device;
+    'rounds', 'num_charts', 'scale', 'num_owned'; with ``timing``, 'stage_ms' (wall milliseconds of the five stages,
+    the stream drained between them)}.  texture.AtlasTooLargeError when the charts do not fit at 7 x 7 texels each."""
+    from . import texture
+
+    dev, v, _, f = _texture_mesh(vertices, faces)
+    V, F, N = int(v.shape[0]), int(f.shape[0]), int(num_pixels_per_side)
+    nbytes = C.c_size_t(0)
+    L.check(L.load().fnr_chart_unwrap_scratch_bytes(V, F, N, C.byref(nbytes)))
+    buf = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+    i32 = dict(dtype=torch.int32, device=dev)
+    labels, charts, offsets = torch.empty(F, **i32), torch.empty(F, **i32), torch.empty((F, 2), **i32)
+    uv = torch.empty((F, 3, 2), dtype=torch.float64, device=dev)
+    NN = N * N if N >= 1 else 0
+    owner, texels, texel_faces = torch.empty(NN, **i32), torch.empty(NN, **i32), torch.empty(NN, **i32)
+    bary = torch.empty((NN, 3), dtype=torch.float32, device=dev)
+    rounds, num_charts, scale, owned = C.c_int32(0), C.c_int64(0), C.c_double(0), C.c_int64(0)
+    ms = (C.c_double * L.FNR_UNWRAP_STAGES)()
+    L.check(L.load().fnr_chart_unwrap(_ptr(v), _ptr(f), V, F, N, _ptr(buf), nbytes.value, _ptr(labels), _ptr(charts), _ptr(offsets), _ptr(uv),
+                                      _ptr(owner), _ptr(texels), _ptr(texel_faces), _ptr(bary), C.byref(rounds), C.byref(num_charts),
+                                      C.byref(scale), C.byref(owned), ms if timing else None, _stream(dev)))
+    if scale.value < 0:
+        raise texture.charts_too_many(num_charts.value, N)
+    n, nc = owned.value, num_charts.value
+    out = {"labels": labels, "charts": charts, "offsets": offsets[:nc], "uv": uv, "owner": owner, "texels": texels[:n],
+           "texel_faces": texel_faces[:n], "barycentrics": bary[:n], "rounds": int(rounds.value), "num_charts": nc, "scale": float(scale.value),
+           "num_owned": n}
+    if timing:
+        out["stage_ms"] = list(ms)
+    return out
+
+
+def chart_texel_rays(vertices: Tensor, normals: Tensor, faces: Tensor, texel_faces: Tensor, barycentrics: Tensor, raylen: float,
+                     texel_start: int, num_texels: int, out: Optional[Tuple[Tensor, Tensor]] = None) -> Tuple[Tensor, Tensor]:
+    """Origins and unit directions [n,3] of owned texels [texel_start, texel_start + n) of a chart atlas
+    (fnr_chart_texel_rays; texel_faces, barycentrics as chart_unwrap returns them).  ``out`` as for texel_rays."""
+    dev, v, n, f = _texture_mesh(vertices, faces, normals)
+    _require_cuda(texel_faces, barycentrics)
+    tf = texel_faces.reshape(-1).to(torch.int32).contiguous()
+    w = _f32c(barycentrics.reshape(-1, 3))
+    if w.shape[0] != tf.shape[0]:
+        raise ValueError(f"{tf.shape[0]} texel faces with {w.shape[0]} barycentrics")
+    if out is None:
+        o = torch.empty((num_texels, 3), dtype=torch.float32, device=dev)
+        d = torch.empty((num_texels, 3), dtype=torch.float32, device=dev)
+    else:
+        _require_cuda(*out)
+        o, d = out[0][:num_texels], out[1][:num_texels]
+        if o.shape != (num_texels, 3) or d.shape != (num_texels, 3) or not (o.is_contiguous() and d.is_contiguous()):
+            raise ValueError("out buffers must be contiguous fp32 [>= n, 3]")
+    L.check(L.load().fnr_chart_texel_rays(_ptr(v), _ptr(n), _ptr(f), int(f.shape[0]), _ptr(tf), _ptr(w), int(tf.shape[0]), float(raylen),
+                                          int(texel_start), int(num_texels), _ptr(o), _ptr(d), _stream(dev)))
+    return o, d

@@ -145,7 +145,9 @@ class ExportTSDFMesh(Exporter):
     """nerfstudio 0.3.2 ExportTSDFMesh: a surface mesh of the scene by TSDF fusion of rendered depth maps, plus the mesh of
     the fruit surfaces (faces whose vertices have a fused fruit probability >= 0.5).  Single GPU.  The PLYs carry vertex
     colours.  ``texture_method="nerf"`` with ``unwrap_method="custom"`` also writes both meshes as OBJs textured by the
-    NeRF, ``px_per_uv_triangle`` texels per face (DESIGN section 4.3p); the xatlas unwrap is not available.
+    NeRF, ``px_per_uv_triangle`` texels per face (DESIGN section 4.3p); with ``unwrap_method="charts"`` the texture is one
+    square atlas of ``num_pixels_per_side`` texels a side whose texel density follows surface area (DESIGN section 4.3r);
+    the xatlas unwrap is not available.
     ``target_num_faces`` decimates each textured mesh on the GPU first (DESIGN section 4.3q); unlike nerfstudio's 50 000
     its default is None, the full mesh."""
 
@@ -163,13 +165,14 @@ class ExportTSDFMesh(Exporter):
     unwrap_method: str = "xatlas"
     px_per_uv_triangle: int = 4
     target_num_faces: Optional[int] = None
+    num_pixels_per_side: int = 1024
 
     def validate(self) -> None:
         """Refuse what cannot run, before anything is loaded."""
         _validate_target_num_faces(self.texture_method, self.target_num_faces)
         if self.texture_method not in ("tsdf", "nerf"):
             raise ValueError(f"texture_method must be 'tsdf' or 'nerf', got {self.texture_method!r}")
-        _validate_nerf_texture(self.texture_method, self.unwrap_method, self.px_per_uv_triangle, "tsdf")
+        _validate_nerf_texture(self.texture_method, self.unwrap_method, self.px_per_uv_triangle, self.num_pixels_per_side, "tsdf")
         res = tuple(self.resolution) if isinstance(self.resolution, (list, tuple)) else (self.resolution,)
         if len(res) not in (1, 3) or min(int(r) for r in res) < 2:
             raise ValueError(f"resolution must be one or three integers >= 2, got {list(res)}")
@@ -199,7 +202,7 @@ class ExportTSDFMesh(Exporter):
                                refinement_epsilon=self.refinement_epsilon)
         if self.texture_method == "nerf":
             out["paths"].update(export_textured_meshes(pipeline, out, Path(self.output_dir), self.px_per_uv_triangle,
-                                                         self.target_num_faces))
+                                                         self.target_num_faces, self.unwrap_method, self.num_pixels_per_side))
         return out
 
 
@@ -209,7 +212,8 @@ class ExportPoissonMesh(Exporter):
     cloud, trimmed at the 0.1 quantile of vertex density, plus the mesh of the fruit surfaces (faces whose vertices have a
     fruit probability >= 0.5).  Single GPU.  The PLYs carry vertex colours.  ``texture_method="nerf"`` with
     ``unwrap_method="custom"`` also writes both meshes as OBJs textured by the NeRF, ``px_per_uv_triangle`` texels per
-    face (DESIGN section 4.3p); the xatlas unwrap is not available.  ``target_num_faces`` decimates each textured mesh on
+    face (DESIGN section 4.3p), or with ``unwrap_method="charts"`` in one ``num_pixels_per_side``-square chart atlas (DESIGN
+    section 4.3r); the xatlas unwrap is not available.  ``target_num_faces`` decimates each textured mesh on
     the GPU first (DESIGN section 4.3q); unlike nerfstudio's 50 000 its default is None, the full mesh.  ``depth`` (open3d's octree depth, here the dense grid's 2^depth cells per axis) is
     the one option upstream does not have."""
 
@@ -232,6 +236,7 @@ class ExportPoissonMesh(Exporter):
     unwrap_method: str = "xatlas"
     px_per_uv_triangle: int = 4
     target_num_faces: Optional[int] = None
+    num_pixels_per_side: int = 1024
 
     def validate(self) -> None:
         """Refuse what cannot run, before anything is loaded."""
@@ -240,7 +245,7 @@ class ExportPoissonMesh(Exporter):
         _validate_target_num_faces(self.texture_method, self.target_num_faces)
         if self.texture_method not in ("point_cloud", "nerf"):
             raise ValueError(f"texture_method must be 'point_cloud' or 'nerf', got {self.texture_method!r}")
-        _validate_nerf_texture(self.texture_method, self.unwrap_method, self.px_per_uv_triangle, "point_cloud")
+        _validate_nerf_texture(self.texture_method, self.unwrap_method, self.px_per_uv_triangle, self.num_pixels_per_side, "point_cloud")
         if self.normal_method not in ("open3d", "model_output"):
             raise ValueError(f"normal_method must be 'open3d' or 'model_output', got {self.normal_method!r}")
         poisson.check_depth(self.depth)
@@ -268,20 +273,25 @@ class ExportPoissonMesh(Exporter):
                                   bounding_box_max=self.bounding_box_max, std_ratio=self.std_ratio, depth=self.depth)
         if self.texture_method == "nerf":
             out["paths"].update(export_textured_meshes(pipeline, out, Path(self.output_dir), self.px_per_uv_triangle,
-                                                         self.target_num_faces))
+                                                         self.target_num_faces, self.unwrap_method, self.num_pixels_per_side))
         return out
 
 
-def _validate_nerf_texture(texture_method: str, unwrap_method: str, px_per_uv_triangle: int, vertex_colours: str) -> None:
-    """The options of NeRF texturing: only the per-face ("custom") unwrap is available, at >= 2 texels per triangle."""
-    from ..texture import check_px_per_uv_triangle
+def _validate_nerf_texture(texture_method: str, unwrap_method: str, px_per_uv_triangle: int, num_pixels_per_side: int,
+                           vertex_colours: str) -> None:
+    """The options of NeRF texturing: the per-face ("custom") unwrap at >= 2 texels per triangle, or the chart ("charts")
+    unwrap into a square atlas of num_pixels_per_side texels a side; xatlas is not available."""
+    from ..texture import check_num_pixels_per_side, check_px_per_uv_triangle
 
-    if unwrap_method not in ("xatlas", "custom"):
-        raise ValueError(f"unwrap_method must be 'xatlas' or 'custom', got {unwrap_method!r}")
+    if unwrap_method not in ("xatlas", "custom", "charts"):
+        raise ValueError(f"unwrap_method must be 'xatlas', 'custom' or 'charts', got {unwrap_method!r}")
     if texture_method == "nerf" and unwrap_method == "xatlas":
         raise ValueError(f"texture_method 'nerf' with the xatlas UV unwrap needs the xatlas package, which is not available; use "
-                         f"--unwrap-method custom (one atlas triangle per face) or texture_method '{vertex_colours}' (vertex colours)")
+                         f"--unwrap-method custom (one atlas triangle per face), --unwrap-method charts (area-proportional charts in "
+                         f"one square atlas) or texture_method '{vertex_colours}' (vertex colours)")
     check_px_per_uv_triangle(px_per_uv_triangle)
+    if unwrap_method == "charts":
+        check_num_pixels_per_side(num_pixels_per_side)
 
 
 def _validate_target_num_faces(texture_method: str, target_num_faces: Optional[int]) -> None:
@@ -357,8 +367,10 @@ def add_tsdf_parser(sub) -> argparse.ArgumentParser:
     p.add_argument("--texture-method", choices=("tsdf", "nerf"), default=d.texture_method)
     p.add_argument("--refine-mesh-using-initial-aabb-estimate", type=_flag, default=d.refine_mesh_using_initial_aabb_estimate)
     p.add_argument("--refinement-epsilon", type=float, default=d.refinement_epsilon)
-    p.add_argument("--unwrap-method", choices=("xatlas", "custom"), default=d.unwrap_method)
+    p.add_argument("--unwrap-method", choices=("xatlas", "custom", "charts"), default=d.unwrap_method)
     p.add_argument("--px-per-uv-triangle", type=int, default=d.px_per_uv_triangle)
+    p.add_argument("--num-pixels-per-side", type=int, default=d.num_pixels_per_side,
+                   help="side of the square texture atlas of --unwrap-method charts, in texels")
     p.add_argument("--target-num-faces", type=int, default=None,
                    help="decimate each textured mesh to this many faces on the GPU first (with --texture-method nerf); "
                         "default: no decimation, unlike nerfstudio's 50000, so the full mesh is textured")
@@ -386,8 +398,10 @@ def add_poisson_parser(sub) -> argparse.ArgumentParser:
     p.add_argument("--texture-method", choices=("point_cloud", "nerf"), default=d.texture_method)
     p.add_argument("--std-ratio", type=float, default=d.std_ratio)
     p.add_argument("--depth", type=int, default=d.depth)
-    p.add_argument("--unwrap-method", choices=("xatlas", "custom"), default=d.unwrap_method)
+    p.add_argument("--unwrap-method", choices=("xatlas", "custom", "charts"), default=d.unwrap_method)
     p.add_argument("--px-per-uv-triangle", type=int, default=d.px_per_uv_triangle)
+    p.add_argument("--num-pixels-per-side", type=int, default=d.num_pixels_per_side,
+                   help="side of the square texture atlas of --unwrap-method charts, in texels")
     p.add_argument("--target-num-faces", type=int, default=None,
                    help="decimate each textured mesh to this many faces on the GPU first (with --texture-method nerf); "
                         "default: no decimation, unlike nerfstudio's 50000, so the full mesh is textured")
@@ -401,7 +415,8 @@ def poisson_exporter_from_args(a) -> ExportPoissonMesh:
                              use_bounding_box=a.use_bounding_box, bounding_box_min=tuple(a.bounding_box_min),
                              bounding_box_max=tuple(a.bounding_box_max), num_rays_per_batch=a.num_rays_per_batch,
                              texture_method=a.texture_method, std_ratio=a.std_ratio, depth=a.depth, unwrap_method=a.unwrap_method,
-                             px_per_uv_triangle=a.px_per_uv_triangle, target_num_faces=a.target_num_faces)
+                             px_per_uv_triangle=a.px_per_uv_triangle, target_num_faces=a.target_num_faces,
+                             num_pixels_per_side=a.num_pixels_per_side)
 
 
 def _run_mesh_export(exp, parser):
@@ -435,7 +450,8 @@ def tsdf_exporter_from_args(a) -> ExportTSDFMesh:
                           bounding_box_max=tuple(a.bounding_box_max), texture_method=a.texture_method,
                           refine_mesh_using_initial_aabb_estimate=a.refine_mesh_using_initial_aabb_estimate,
                           refinement_epsilon=a.refinement_epsilon, unwrap_method=a.unwrap_method,
-                          px_per_uv_triangle=a.px_per_uv_triangle, target_num_faces=a.target_num_faces)
+                          px_per_uv_triangle=a.px_per_uv_triangle, target_num_faces=a.target_num_faces,
+                          num_pixels_per_side=a.num_pixels_per_side)
 
 
 def entrypoint(argv=None):

@@ -1,5 +1,6 @@
 """NeRF textures of the exported meshes (nerfstudio 0.3.2 texture_utils.export_textured_mesh with
-``unwrap_method="custom"``; DESIGN section 4.3p).
+``unwrap_method="custom"``; DESIGN section 4.3p), and the project's own ``charts`` unwrap (DESIGN section 4.3r, restated
+further down).
 
 Every face gets its own small triangle in a grid atlas, and every texel is coloured by one short ray through the model,
 cast from just outside the surface along the inverted normal.  This module owns the atlas layout (the kernel
@@ -34,7 +35,7 @@ MTL_LINES = ("# Generated with nerfstudio", "newmtl {name}", "Ka 1.00000000 1.00
 
 
 class AtlasTooLargeError(RuntimeError):
-    """The atlas of a mesh would have a side over MAX_SIDE texels."""
+    """The atlas of a mesh would have a side over MAX_SIDE texels, or its charts do not fit into the chosen atlas."""
 
 
 def check_px_per_uv_triangle(px_per_uv_triangle: int) -> int:
@@ -118,14 +119,21 @@ def texel_barycentrics(num_faces: int, px_per_uv_triangle: int, texel_start: int
 def restated_texel_rays(vertices, normals, faces, px_per_uv_triangle: int, width: int, height: int, raylen: float, texel_start: int = 0,
                         num_texels=None) -> Tuple[np.ndarray, np.ndarray]:
     """fnr_texel_rays in numpy fp32, bit for bit: (origins, directions) [n,3]."""
-    f32 = np.float32
-    v = np.asarray(vertices, f32).reshape(-1, 3)
-    nv = np.asarray(normals, f32).reshape(-1, 3)
     fc = np.asarray(faces, np.int64).reshape(-1, 3)
     if atlas_layout(len(fc), px_per_uv_triangle)[1:] != (width, height):
         raise ValueError(f"{width}x{height} is not the atlas of {len(fc)} faces at {px_per_uv_triangle} px per uv triangle")
     face, w = texel_barycentrics(len(fc), px_per_uv_triangle, texel_start, num_texels)
-    idx = fc[face]
+    return _texel_rays(vertices, normals, fc, face, w, raylen)
+
+
+def _texel_rays(vertices, normals, faces, face, w, raylen: float) -> Tuple[np.ndarray, np.ndarray]:
+    """The ray of each (face, fp32 barycentrics w [n,3]) in fp32 (the kernels' texel_ray): origins, directions [n,3]."""
+    f32 = np.float32
+    v = np.asarray(vertices, f32).reshape(-1, 3)
+    nv = np.asarray(normals, f32).reshape(-1, 3)
+    fc = np.asarray(faces, np.int64).reshape(-1, 3)
+    w = np.asarray(w, f32).reshape(-1, 3)
+    idx = fc[np.asarray(face, np.int64)]
     w0, w1, w2 = (w[:, k:k + 1] for k in range(3))
 
     def interp(a):
@@ -158,6 +166,278 @@ def restated_mean_edge(vertices, faces) -> float:
     fc = np.asarray(faces, np.int64).reshape(-1, 3)
     d = v[fc[:, 1]] - v[fc[:, 0]]
     return float(np.sqrt((d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1]) + d[:, 2] * d[:, 2]).sum() / len(fc))
+
+
+# ---- the `charts` unwrap (fnr_chart_unwrap; DESIGN section 4.3r) --------------------------------------------------------
+# Faces are grouped into connected charts of one dominant signed normal axis, every chart is projected onto its axis plane
+# at one scale s of texels per unit length (so texel density follows surface area), and the charts are packed by
+# next-fit shelves into one N x N atlas.  include/fruitnerf_b200.h writes out every step; this is its numpy restatement,
+# bit for bit, used on test-sized meshes.
+UNWRAP_MIN_SIDE = 16  # FNR_UNWRAP_MIN_SIDE
+UNWRAP_MARGIN = 3  # FNR_UNWRAP_MARGIN: texels around a chart's rectangle
+UNWRAP_GUTTER = 2  # FNR_UNWRAP_GUTTER: texels around a triangle that take its closest point
+UNWRAP_BISECTIONS = 40  # FNR_UNWRAP_BISECTIONS
+# (texel x, texel y) axes per label +x, -x, +y, -y, +z, -z: negative area in texel space, positive in vt space
+_CHART_AXES = np.array([[2, 1], [1, 2], [0, 2], [2, 0], [1, 0], [0, 1]], np.int64)
+_NO_OWNER = np.uint64(0xFFFFFFFFFFFFFFFF)
+_WORK_PER_PASS = 1 << 22
+
+
+def check_num_pixels_per_side(num_pixels_per_side: int) -> int:
+    n = int(num_pixels_per_side)
+    if n < UNWRAP_MIN_SIDE or n > MAX_SIDE:
+        raise ValueError(f"num_pixels_per_side must be an integer in [{UNWRAP_MIN_SIDE}, {MAX_SIDE}], got {num_pixels_per_side}")
+    return n
+
+
+def charts_too_many(num_charts: int, num_pixels_per_side: int) -> AtlasTooLargeError:
+    return AtlasTooLargeError(f"{num_charts} charts do not fit into a {num_pixels_per_side}x{num_pixels_per_side} atlas even at 7x7 texels each: "
+                              f"raise --num-pixels-per-side or decimate the mesh first with --target-num-faces")
+
+
+def chart_labels(vertices, faces) -> Tuple[np.ndarray, np.ndarray]:
+    """(labels [F] int32, projected corners [F,3,2] fp64): the dominant signed axis 2k + (n_k < 0) of each right-hand
+    normal, ties to the lower axis, and the two kept coordinates in the label's order."""
+    P = np.asarray(vertices, np.float32).reshape(-1, 3).astype(np.float64)[np.asarray(faces, np.int64).reshape(-1, 3)] + 0.0
+    e1, e2 = P[:, 1] - P[:, 0], P[:, 2] - P[:, 0]
+    n = np.stack([e1[:, 1] * e2[:, 2] - e1[:, 2] * e2[:, 1], e1[:, 2] * e2[:, 0] - e1[:, 0] * e2[:, 2],
+                  e1[:, 0] * e2[:, 1] - e1[:, 1] * e2[:, 0]], axis=1)
+    a = np.abs(n)
+    k = np.zeros(len(n), np.int64)
+    best = a[:, 0].copy()
+    for j in (1, 2):
+        m = a[:, j] > best
+        k[m], best[m] = j, a[m, j]
+    label = 2 * k + (n[np.arange(len(n)), k] < 0)
+    proj = np.take_along_axis(P, _CHART_AXES[label][:, None, :], axis=2)
+    return label.astype(np.int32), proj
+
+
+def _interior_edges(faces, num_vertices: int) -> Tuple[np.ndarray, np.ndarray]:
+    """The two faces of every edge held by exactly two half-edges (fnr_mesh_edges.cuh's keys, stably sorted)."""
+    fc = np.asarray(faces, np.int64).reshape(-1, 3)
+    a, b = fc, np.roll(fc, -1, axis=1)
+    key = (np.minimum(a, b) * int(num_vertices) + np.maximum(a, b)).reshape(-1)
+    order = np.argsort(key, kind="stable")
+    _, first, count = np.unique(key[order], return_index=True, return_counts=True)
+    i = first[count == 2]
+    return order[i] // 3, order[i + 1] // 3
+
+
+def chart_ids(labels, fa, fb, cut) -> Tuple[np.ndarray, int]:
+    """Chart of every face: components of the interior edges whose faces share a label and are not cut, numbered in
+    order of their smallest face."""
+    from scipy.sparse import coo_matrix
+    from scipy.sparse.csgraph import connected_components
+
+    F = len(labels)
+    join = (labels[fa] == labels[fb]) & ~cut[fa] & ~cut[fb]
+    g = coo_matrix((np.ones(int(join.sum()), np.int8), (fa[join], fb[join])), shape=(F, F))
+    C, comp = connected_components(g, directed=False)
+    _, first = np.unique(comp, return_index=True)  # component c's smallest face
+    rank = np.empty(C, np.int64)
+    rank[np.argsort(first)] = np.arange(C)
+    return rank[comp].astype(np.int32), int(C)
+
+
+def chart_extents(proj, charts, num_charts: int) -> Tuple[np.ndarray, np.ndarray]:
+    """(ext [C,2] = max - min, p_min [C,2]) of every chart's projected corners."""
+    o = np.argsort(charts, kind="stable")
+    starts = np.searchsorted(charts[o], np.arange(num_charts))
+    lo = np.minimum.reduceat(proj.min(axis=1)[o], starts, axis=0)
+    hi = np.maximum.reduceat(proj.max(axis=1)[o], starts, axis=0)
+    return hi - lo, lo
+
+
+def chart_order(ext) -> np.ndarray:
+    """The packing order: (ext_y desc, ext_x desc, id asc)."""
+    return np.lexsort((np.arange(len(ext)), -ext[:, 0], -ext[:, 1]))
+
+
+def pack_charts(ext, order, scale: float, num_pixels_per_side: int):
+    """Next-fit shelves of the charts' rectangles (floor(s ext) + 1 + 2 margin texels a side), taken in ``order``, into
+    N x N: offsets [C,2] int32 (top-left texel), or None when a rectangle does not fit."""
+    N, m2 = int(num_pixels_per_side), 2 * UNWRAP_MARGIN
+    s = float(scale)
+    ex, ey = ext[order, 0].tolist(), ext[order, 1].tolist()
+    out = np.empty((len(ext), 2), np.int32)
+    x = y = shelf = 0
+    for c, a, b in zip(order.tolist(), ex, ey):
+        w, h = math.floor(s * a) + 1 + m2, math.floor(s * b) + 1 + m2
+        if w > N:
+            return None
+        if x + w > N:
+            y, x, shelf = y + shelf, 0, 0
+        if y + h > N:
+            return None
+        out[c] = (x, y)
+        x += w
+        shelf = max(shelf, h)
+    return out
+
+
+def chart_scale(ext, num_pixels_per_side: int):
+    """(s, hi, offsets): the largest scale that packs after UNWRAP_BISECTIONS halvings of [0, N / largest extent], the
+    final upper bracket (which does not pack) and the offsets at s.  AtlasTooLargeError when s = 0 does not pack."""
+    N = int(num_pixels_per_side)
+    order = chart_order(ext)
+    if pack_charts(ext, order, 0.0, N) is None:
+        raise charts_too_many(len(ext), N)
+    emax = float(ext.max()) if ext.size else 0.0
+    if not emax > 0.0:
+        return 0.0, 0.0, pack_charts(ext, order, 0.0, N)
+    lo, hi = 0.0, N / emax
+    for _ in range(UNWRAP_BISECTIONS):
+        mid = (lo + hi) * 0.5
+        if pack_charts(ext, order, mid, N) is not None:
+            lo = mid
+        else:
+            hi = mid
+    return lo, hi, pack_charts(ext, order, lo, N)
+
+
+def chart_uv(proj, charts, offsets, pmin, scale: float) -> np.ndarray:
+    """[F,3,2] fp64 texel coordinates offset + margin + s (p - p_min) of every corner."""
+    c = np.asarray(charts, np.int64)
+    o = (offsets[c] + UNWRAP_MARGIN).astype(np.float64)[:, None, :]
+    return o + float(scale) * (proj - pmin[c][:, None, :])
+
+
+def chart_vt(uv, num_pixels_per_side: int) -> np.ndarray:
+    """OBJ vt of texel coordinates: (x / N, 1 - y / N)."""
+    uv = np.asarray(uv, np.float64)
+    N = float(num_pixels_per_side)
+    return np.stack([uv[..., 0] / N, 1.0 - uv[..., 1] / N], axis=-1)
+
+
+def _texel_boxes(uv, N: int):
+    """Per face: the first column and row and the size of its texel box grown by the gutter, clamped to the atlas."""
+    mn, mx = uv.min(axis=1), uv.max(axis=1)
+    lo = np.maximum(np.ceil(mn - (UNWRAP_GUTTER + 0.5)), 0).astype(np.int64)
+    hi = np.minimum(np.floor(mx + (UNWRAP_GUTTER - 0.5)), N - 1).astype(np.int64)
+    return lo, np.maximum(hi - lo + 1, 0)
+
+
+def _work_items(uv, N: int):
+    """(face, col, row) of every texel of every face's box, in face order, in passes of about _WORK_PER_PASS."""
+    lo, size = _texel_boxes(uv, N)
+    n = size[:, 0] * size[:, 1]
+    end = np.cumsum(n)
+    f0 = 0
+    while f0 < len(n):
+        base = end[f0] - n[f0]
+        f1 = max(int(np.searchsorted(end, base + _WORK_PER_PASS, side="right")), f0 + 1)
+        face = np.repeat(np.arange(f0, f1), n[f0:f1])
+        q = np.arange(base, end[f1 - 1]) - np.repeat(end[f0:f1] - n[f0:f1], n[f0:f1])
+        w = size[face, 0]
+        yield face, lo[face, 0] + q % w, lo[face, 1] + q // w
+        f0 = f1
+
+
+def _edge_fn(ax, ay, bx, by, cx, cy):
+    return (cx - ax) * (by - ay) - (cy - ay) * (bx - ax)
+
+
+def _edge_fns(uv, face, col, row):
+    t = uv[face]
+    x, y = t[:, :, 0], t[:, :, 1]
+    cx, cy = col + 0.5, row + 0.5
+    return (x, y, cx, cy, _edge_fn(x[:, 1], y[:, 1], x[:, 2], y[:, 2], cx, cy), _edge_fn(x[:, 2], y[:, 2], x[:, 0], y[:, 0], cx, cy),
+            _edge_fn(x[:, 0], y[:, 0], x[:, 1], y[:, 1], cx, cy))
+
+
+def chart_closest(uv, face, col, row) -> Tuple[np.ndarray, np.ndarray]:
+    """(d2 [n] fp64, barycentrics [n,3] fp32) of the closest point of face's UV triangle to each texel centre."""
+    f32 = np.float32
+    x, y, cx, cy, e0, e1, e2 = _edge_fns(uv, face, col, row)
+    total = (e0 + e1) + e2
+    inside = (e0 >= 0) & (e1 >= 0) & (e2 >= 0) & (total > 0)
+    best = bt = bk = None
+    for k in range(3):
+        k1 = (k + 1) % 3
+        dx, dy = x[:, k1] - x[:, k], y[:, k1] - y[:, k]
+        l2 = dx * dx + dy * dy
+        num = (cx - x[:, k]) * dx + (cy - y[:, k]) * dy
+        with np.errstate(divide="ignore", invalid="ignore"):
+            t = np.where(l2 > 0, np.minimum(np.maximum(num / np.where(l2 > 0, l2, 1.0), 0.0), 1.0), 0.0)
+        qx, qy = cx - (x[:, k] + t * dx), cy - (y[:, k] + t * dy)
+        d2 = qx * qx + qy * qy
+        if k == 0:
+            best, bt, bk = d2, t, np.zeros(len(d2), np.int64)
+        else:
+            m = d2 < best
+            best, bt, bk = np.where(m, d2, best), np.where(m, t, bt), np.where(m, k, bk)
+    w = np.zeros((len(best), 3), f32)
+    wt = bt.astype(f32)
+    r = np.arange(len(best))
+    w[r, bk] = f32(1) - wt
+    w[r, (bk + 1) % 3] = wt
+    with np.errstate(divide="ignore", invalid="ignore"):
+        w1, w2 = (e1 / total).astype(f32), (e2 / total).astype(f32)
+    w[inside] = np.stack([np.maximum((f32(1) - w1[inside]) - w2[inside], f32(0)), w1[inside], w2[inside]], axis=1)
+    w[~inside & ~(total > 0)] = f32([1, 0, 0])
+    return np.where(inside, 0.0, best), w
+
+
+def _conflict_faces(uv, N: int) -> np.ndarray:
+    """Faces strictly inside at a texel centre that another, smaller face is strictly inside too."""
+    texel, face = [], []
+    for f, col, row in _work_items(uv, N):
+        _, _, _, _, e0, e1, e2 = _edge_fns(uv, f, col, row)
+        m = (e0 > 0) & (e1 > 0) & (e2 > 0)
+        texel.append(row[m] * N + col[m])
+        face.append(f[m])
+    texel, face = np.concatenate(texel), np.concatenate(face)
+    hit = np.bincount(texel, minlength=N * N) >= 2
+    m = hit[texel]
+    texel, face = texel[m], face[m]
+    _, first, inv = np.unique(texel, return_index=True, return_inverse=True)  # items come in face order: the first is the smallest face
+    return np.unique(face[face != face[first][inv]])
+
+
+def restated_chart_unwrap(vertices, faces, num_pixels_per_side: int) -> Dict:
+    """fnr_chart_unwrap in numpy, bit for bit: {'labels', 'charts' [F] int32, 'offsets' [C,2] int32, 'uv' [F,3,2] fp64
+    texel coordinates, 'owner' [N*N] int32 (-1: none), 'texels', 'texel_faces' [n] int32 and 'barycentrics' [n,3] fp32
+    of the owned texels in texel order, 'rounds', 'num_charts', 'scale', 'scale_fails' (the last bisection bracket above
+    the scale, which does not pack)}.  AtlasTooLargeError when the charts do not fit at 7 x 7 texels each."""
+    N = check_num_pixels_per_side(num_pixels_per_side)
+    v = np.asarray(vertices, np.float32).reshape(-1, 3)
+    fc = np.asarray(faces, np.int64).reshape(-1, 3)
+    if len(fc) < 1:
+        raise ValueError("the mesh has no faces")
+    labels, proj = chart_labels(v, fc)
+    fa, fb = _interior_edges(fc, len(v))
+    cut = np.zeros(len(fc), bool)
+    rounds = 0
+    while True:
+        charts, C = chart_ids(labels, fa, fb, cut)
+        ext, pmin = chart_extents(proj, charts, C)
+        s, hi, offsets = chart_scale(ext, N)
+        uv = chart_uv(proj, charts, offsets, pmin, s)
+        split = _conflict_faces(uv, N)
+        split = split[~cut[split]]
+        if len(split) == 0:
+            break
+        cut[split] = True
+        rounds += 1
+    keys = np.full(N * N, _NO_OWNER, np.uint64)
+    for f, col, row in _work_items(uv, N):
+        d2, _ = chart_closest(uv, f, col, row)
+        m = d2 <= UNWRAP_GUTTER * UNWRAP_GUTTER
+        key = (d2[m].astype(np.float32).view(np.uint32).astype(np.uint64) << np.uint64(32)) | f[m].astype(np.uint64)
+        np.minimum.at(keys, row[m] * N + col[m], key)
+    texels = np.flatnonzero(keys != _NO_OWNER)
+    tf = (keys[texels] & np.uint64(0xFFFFFFFF)).astype(np.int64)
+    _, w = chart_closest(uv, tf, texels % N, texels // N)
+    owner = np.full(N * N, -1, np.int32)
+    owner[texels] = tf
+    return {"labels": labels, "charts": charts, "offsets": offsets, "uv": uv, "owner": owner, "texels": texels.astype(np.int32),
+            "texel_faces": tf.astype(np.int32), "barycentrics": w, "rounds": rounds, "num_charts": C, "scale": s, "scale_fails": hi}
+
+
+def restated_chart_texel_rays(vertices, normals, faces, texel_faces, barycentrics, raylen: float) -> Tuple[np.ndarray, np.ndarray]:
+    """fnr_chart_texel_rays in numpy fp32, bit for bit: (origins, directions) [n,3] of the owned texels."""
+    return _texel_rays(vertices, normals, faces, texel_faces, barycentrics, raylen)
 
 
 # ---- OBJ / MTL ---------------------------------------------------------------------------------------------------------

@@ -71,6 +71,9 @@
  *   fnr_mesh_decimate_scratch_bytes, fnr_mesh_decimate
  *                        quadric edge-collapse decimation of the meshes before NeRF texturing (nerfstudio
  *                        target_num_faces; pymeshlab meshing_decimation_quadric_edge_collapse)
+ *   fnr_chart_unwrap_scratch_bytes, fnr_chart_unwrap, fnr_chart_texel_rays
+ *                        the `charts` UV unwrap of NeRF texturing (the project's own, in place of nerfstudio's xatlas):
+ *                        area-proportional axis-projected charts packed into one square atlas, one ray per owned texel
  */
 #ifndef FRUITNERF_B200_H
 #define FRUITNERF_B200_H
@@ -765,6 +768,66 @@ int fnr_mesh_decimate_scratch_bytes(int64_t num_vertices, int64_t num_faces, siz
 int fnr_mesh_decimate(const double* vertices, const int64_t* faces, int64_t num_vertices, int64_t num_faces, int64_t target_num_faces,
                       void* scratch, size_t scratch_bytes, double* out_vertices, double* out_normals, int64_t* out_faces,
                       int64_t* out_num_vertices, int64_t* out_num_faces, int32_t* out_rounds, void* stream);
+
+/* ---- The `charts` UV unwrap (`--unwrap-method charts` of NeRF texturing; fnr_unwrap.cu, fnr_texture.cu; DESIGN section
+ * 4.3r) ----
+ * vertices: DEVICE [V,3] fp32, finite; faces: DEVICE [F,3] int64, every index in [0, V) (FNR_ERR_INVALID_ARGUMENT
+ * otherwise: a device check and one host read).  N = num_pixels_per_side in [FNR_UNWRAP_MIN_SIDE, FNR_TEXTURE_MAX_SIDE],
+ * V >= 1, F >= 1 and no NULL pointer (stage_ms aside), else FNR_ERR_INVALID_ARGUMENT before any CUDA call; V > 2^31 - 1
+ * or F > (2^31 - 1) / 3: FNR_ERR_UNSUPPORTED.  DEVICE scratch: fnr_chart_unwrap_scratch_bytes(V, F, N); nothing is
+ * allocated on the device.  Outputs, DEVICE: labels, charts [F] int32; offsets [F,2] int32 (the first C rows written);
+ * uv [F,3,2] fp64; owner [N*N] int32; texels, texel_faces [N*N] int32 and barycentrics [N*N,3] fp32 (the first
+ * *out_num_owned rows written).  HOST: *out_rounds, *out_num_charts (C), *out_scale (s), *out_num_owned; stage_ms, when
+ * not NULL, HOST double[FNR_UNWRAP_STAGES] of wall milliseconds (labels and edge sort, charts, packing, raster and
+ * conflicts, owners and compaction; the stream is drained at each stage boundary).
+ *
+ * In this order, every fp64 operation rounded where written (no FMA; texture.py restates it bit for bit):
+ *  1. Positions P = (double)v + 0.  Face f: e1 = P1 - P0, e2 = P2 - P0, n = e1 x e2 (each component a rounded difference
+ *     of rounded products).  Its label is 2k + (n_k < 0) for the axis k of the largest |n_k|, ties to the lower axis (a
+ *     zero normal gets +x, label 0).  Projected corner p = (P[a], P[b]) with (a, b) = (z, y), (y, z), (x, z), (z, x),
+ *     (y, x), (x, y) for the labels +x, -x, +y, -y, +z, -z: a face has negative area in texel space (x right, y down) and
+ *     positive area in vt space.
+ *  2. Charts.  The 3F half-edges (fnr_mesh_edges.cuh) sorted once; a run of exactly two half-edges joins their faces when
+ *     the labels are equal and neither face is cut.  Chart id = rank of the chart's smallest face index.
+ *  3. Extents per chart and axis: ext = max - min of its projected corners, p_min = min.
+ *  4. Packing, on the host: charts sorted by (ext_y desc, ext_x desc, id asc); at scale s a chart's rectangle is
+ *     floor(s ext_x) + 1 + 2 FNR_UNWRAP_MARGIN by floor(s ext_y) + 1 + 2 FNR_UNWRAP_MARGIN texels, placed by next-fit shelves
+ *     (a rectangle that overflows the row opens a shelf below the tallest of the row) into N x N; offsets = its top-left
+ *     texel.  When s = 0 does not pack, *out_scale = -1 and nothing after this step is written.  Otherwise, with E the
+ *     largest extent, s = 0 when E = 0, else lo = 0, hi = N / E and FNR_UNWRAP_BISECTIONS steps mid = (lo + hi) * 0.5,
+ *     lo = mid when it packs, else hi = mid; s = lo.
+ *  5. Texel coordinates of corner (f, k): x = (double)(offset_x + FNR_UNWRAP_MARGIN) + s * (p_x - p_min,x), likewise y.
+ *     vt = (x / N, 1 - y / N).  Texel (row, col) has its centre at (col + 0.5, row + 0.5).
+ *  6. Edge function of edge a -> b at c: (c_x - a_x) * (b_y - a_y) - (c_y - a_y) * (b_x - a_x); e_0, e_1, e_2 of the edges
+ *     1 -> 2, 2 -> 0, 0 -> 1.  A texel centre is strictly inside when all three are > 0.  A texel centre strictly inside two
+ *     triangles is a conflict: every face there but the smallest becomes cut (a chart of its own), and steps 2 to 6 run
+ *     again; *out_rounds counts the rounds that cut a face.
+ *  7. Owners.  Per face, every texel whose centre lies within FNR_UNWRAP_GUTTER of its texel box [min - g, max + g] per
+ *     axis, clamped to the atlas: the squared distance d2 to the triangle is 0 when e_0, e_1, e_2 >= 0 and
+ *     sum = (e_0 + e_1) + e_2 > 0, else the least over the edges k -> k + 1 (k = 0, 1, 2, ties to the lower k) of
+ *     |c - (a + t (b - a))|^2 (x^2 + y^2), t = clamp(((c_x - a_x) d_x + (c_y - a_y) d_y) / |d|^2, 0, 1) with d = b - a,
+ *     t = 0 when |d|^2 = 0.  When d2 <= g^2, atomicMin of (fp32(d2) bits << 32) | f: the winner owns the texel.
+ *     Barycentrics (fp32) of the owner's closest point: inside, w1 = fp32(e_1 / sum), w2 = fp32(e_2 / sum),
+ *     w0 = max((1 - w1) - w2, 0); on edge k, w_k = 1 - fp32(t), w_k+1 = fp32(t), the third 0; when sum <= 0 (a degenerate
+ *     triangle), (1, 0, 0).  owner = the face or -1; the owned texels are compacted in texel order.
+ *
+ * fnr_chart_texel_rays writes the rays of owned texels [texel_start, texel_start + num_texels) of num_owned (texel_faces,
+ * barycentrics as fnr_chart_unwrap wrote them) into origins, directions DEVICE [num_texels,3] fp32, with fnr_texel_rays'
+ * arithmetic after its barycentrics.  FNR_ERR_INVALID_ARGUMENT: a NULL pointer, F < 1, a range outside [0, num_owned), a
+ * raylen that is not finite and positive. */
+#define FNR_UNWRAP_MIN_SIDE 16
+#define FNR_UNWRAP_MARGIN 3
+#define FNR_UNWRAP_GUTTER 2
+#define FNR_UNWRAP_BISECTIONS 40
+#define FNR_UNWRAP_STAGES 5
+int fnr_chart_unwrap_scratch_bytes(int64_t num_vertices, int64_t num_faces, int32_t num_pixels_per_side, size_t* bytes);
+int fnr_chart_unwrap(const float* vertices, const int64_t* faces, int64_t num_vertices, int64_t num_faces, int32_t num_pixels_per_side,
+                     void* scratch, size_t scratch_bytes, int32_t* labels, int32_t* charts, int32_t* offsets, double* uv, int32_t* owner,
+                     int32_t* texels, int32_t* texel_faces, float* barycentrics, int32_t* out_rounds, int64_t* out_num_charts,
+                     double* out_scale, int64_t* out_num_owned, double* stage_ms, void* stream);
+int fnr_chart_texel_rays(const float* vertices, const float* normals, const int64_t* faces, int64_t num_faces, const int32_t* texel_faces,
+                         const float* barycentrics, int64_t num_owned, float raylen, int64_t texel_start, int32_t num_texels, float* origins,
+                         float* directions, void* stream);
 
 /* Hash-grid row indices (exact-integer parity hook): rows[N,L,8] in nerfstudio corner order for
  * the masked [0,1]^3 positions of the given samples; also writes positions[N,3] if non-NULL. */
