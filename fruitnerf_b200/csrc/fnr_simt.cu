@@ -244,18 +244,28 @@ constexpr int acc_off(int s) { return s == 0 ? 0 : acc_off(s - 1) + (acc_floats(
 constexpr int align128(int b) { return (b + 127) / 128 * 128; }
 }  // namespace resident
 
-// Warpgroups per CTA of the resident forward and export.  Two fit the kernels' registers as compiled (CTA of 256
-// threads, 128 KiB of dynamic shared memory); three need <= 168 registers and 160 KiB (DESIGN.md section 4.3 has the
-// measured choice).
-#ifndef FNR_FWD_GROUPS
-#define FNR_FWD_GROUPS 2
-#endif
-
-// Dynamic shared memory of the resident forward and export CTA: weight image | per-warpgroup step tiles.
+// The resident forward and export CTA: kGroups MMA warpgroups and one gather warpgroup (warpgroup kGroups).  The gather
+// warpgroup gathers the last kGatherLevels levels of the hash grid for the MMA warpgroups' points and hands them over
+// through a ring of kRing slots, each with a full and an empty mbarrier; the MMA warpgroups gather the other levels
+// themselves.  Registers: launched at 168 per thread (384 threads, 64 512 of the SM's 65 536), the gather warpgroup drops
+// to kGatherRegs and the MMA warpgroups rise to kMmaRegs.  The ring is kept small because the gather runs out of L1,
+// which gets what shared memory leaves: a 64 KiB cp.async stage and a ring of four slots were measured slower, as was
+// the gather warpgroup taking more than half of the levels (DESIGN.md section 4.3).
+// Dynamic shared memory: weight image | per-warpgroup step tiles | ring slots | ring barriers.
 struct ForwardPlan {
-  static constexpr int kGroups = FNR_FWD_GROUPS;
+  static constexpr int kGroups = 2;
+  static constexpr int kThreadsPerCta = (kGroups + 1) * kThreads;
+  static constexpr int kGatherRegs = 56, kMmaRegs = 224;
+  static_assert(kThreads * (kGatherRegs + kGroups * kMmaRegs) <= kThreadsPerCta * 168, "register split of the CTA");
+  static constexpr int kGatherLevels = 8;
+  static constexpr int kRing = 2;
+  static constexpr int kSlotFloats = kThreads * 2 * kGatherLevels;  // fp32, element (row, c) at (c / 4) * 512 + row * 4 + c % 4
   static constexpr int kStepOff = resident::kImageBytes;
-  static constexpr int kBytes = kStepOff + kGroups * wg::kResidentStepBytes;
+  static constexpr int kRingOff = kStepOff + kGroups * wg::kResidentStepBytes;
+  static constexpr int kBarOff = kRingOff + kRing * kSlotFloats * 4;
+  static constexpr int kBytes = kBarOff + 2 * kRing * 8;
+  // with the kernels' static shared memory (s_app, 128 B), within the 232 448 bytes an H100 CTA can have
+  static_assert(kBytes + 128 <= 232448, "forward shared-memory plan");
 };
 // Dynamic shared memory of the resident backward CTA: weight image | accumulators | locks | per-warpgroup step tiles |
 // per-warpgroup dW operand regions.
@@ -328,11 +338,38 @@ struct ResidentLayers {
     split_image<kCol0>(P);
     split_image<kCol1>(P);
   }
-  // Once per CTA, before the first tile: the weight image (forward and export).
+  // Once per CTA, before the first tile: the weight image and the ring's barriers (forward and export).
   static __device__ __forceinline__ void build_image(const KParams& P) {
     split_all(P);
+    if (threadIdx.x < Plan::kRing) {
+      wg::mbar_init(full(threadIdx.x), kThreads);
+      wg::mbar_init(empty(threadIdx.x), kThreads);
+    }
     wg::fence_proxy_async();
     __syncthreads();
+  }
+  // The forward's ring: slot s's encoding rows, and its full (the gather warpgroup's 128 threads arrive) and empty (the
+  // MMA warpgroup's 128 threads arrive) barriers.
+  static __device__ __forceinline__ float* slot(int s) { return reinterpret_cast<float*>(smem() + Plan::kRingOff) + s * Plan::kSlotFloats; }
+  static __device__ __forceinline__ uint64_t* full(int s) { return reinterpret_cast<uint64_t*>(smem() + Plan::kBarOff) + s; }
+  static __device__ __forceinline__ uint64_t* empty(int s) { return full(Plan::kRing) + s; }
+  // The encoding rows of this MMA warpgroup's k-th tile: ring item k * kGroups + group, in slot item % kRing at the
+  // slot's (item / kRing)-th use.  The slot is released as soon as the row is in registers.
+  static __device__ __forceinline__ void ring_read(long long k, float (&enc)[C::ENC]) {
+    const long long item = k * kGroups + wg::group();
+    const int s = (int)(item % Plan::kRing);
+    wg::mbar_wait(full(s), (uint32_t)(item / Plan::kRing) & 1u);
+    const float* row = slot(s) + 4 * wg::tid();
+    constexpr int e0 = 2 * (C::L - Plan::kGatherLevels);
+#pragma unroll
+    for (int i = 0; i < Plan::kGatherLevels / 2; ++i) {
+      const float4 v = *reinterpret_cast<const float4*>(row + i * wg::kRowsGroupStride);
+      enc[e0 + 4 * i] = v.x;
+      enc[e0 + 4 * i + 1] = v.y;
+      enc[e0 + 4 * i + 2] = v.z;
+      enc[e0 + 4 * i + 3] = v.w;
+    }
+    wg::mbar_arrive(empty(s));
   }
   // Once per CTA, before the first tile: the weight image, zero accumulators and free locks (backward).
   static __device__ __forceinline__ void prepare(const KParams& P) {
@@ -562,7 +599,13 @@ __device__ __forceinline__ void block_mean_embedding(const KParams& P, int num_i
 template <class C, bool TC>
 constexpr bool on_resident_image() { return TC && std::is_same<C, CfgSmall>::value; }
 template <class C, bool TC>
-constexpr int forward_threads() { return on_resident_image<C, TC>() ? ForwardPlan::kGroups * kThreads : kThreads; }
+constexpr int forward_groups() { return on_resident_image<C, TC>() ? ForwardPlan::kGroups : 1; }  // MMA warpgroups per CTA
+template <class C, bool TC>
+constexpr int forward_threads() { return on_resident_image<C, TC>() ? ForwardPlan::kThreadsPerCta : kThreads; }
+// The resident kernels name one CTA per SM, so that ptxas knows the registers at entry (168) and can apply setmaxnreg;
+// the others leave it unset, as before.
+template <class C, bool TC>
+constexpr int forward_min_ctas() { return on_resident_image<C, TC>() ? 1 : 0; }
 template <class C, bool TC>
 using ForwardLayers = std::conditional_t<on_resident_image<C, TC>(), ResidentForward, Layers<C, TC>>;
 // The warpgroup of this thread in a CTA of G warpgroups, and the thread's index in it (G = 1: the CTA's own indices, so
@@ -572,21 +615,112 @@ __device__ __forceinline__ int group_of() { return G == 1 ? 0 : wg::group(); }
 template <int G>
 __device__ __forceinline__ unsigned thread_of() { return G == 1 ? threadIdx.x : (unsigned)wg::tid(); }
 
+// The gather warpgroup of the resident forward and export.  It takes the tiles of the CTA's MMA warpgroups in the order
+// they run them (ring item j: the (j / kGroups)-th tile of warpgroup j % kGroups), one point per thread, a point past N
+// clamped to N - 1 as in the MMA warpgroups.  position(p) is the point's field_position.  Levels [L - kGatherLevels, L)
+// go through level_gather, two per step as in hash_encode, so the encoding has its bits.  They go into ring slot
+// j % kRing (and into the encoding stash, when there is one), and the slot's full barrier is arrived on.
+template <class Position>
+__device__ __forceinline__ void gather_encodings(const KField& F, const KParams& P, long long N, float* __restrict__ stash,
+                                                 Position position) {
+  using Plan = ForwardPlan;
+  using RF = ResidentForward;
+  constexpr int L = CfgSmall::L;
+#ifdef FNR_FWD_NO_GATHER
+  return;  // the MMA warpgroups make up their encodings (diagnostic build)
+#endif
+  const int t = wg::tid();
+  const float2* __restrict__ table = reinterpret_cast<const float2*>(P.hash_table);
+  for (long long j = 0;; ++j) {
+    const long long tile = ((long long)blockIdx.x + j / Plan::kGroups * gridDim.x) * Plan::kGroups + j % Plan::kGroups;
+    if (tile * kThreads >= N) break;
+    const int s = (int)(j % Plan::kRing);
+    const long long p = tile * kThreads + t;
+    const bool valid = p < N;
+    const Vec3 pos = position(valid ? p : N - 1);
+    wg::mbar_wait(RF::empty(s), ((uint32_t)(j / Plan::kRing) & 1u) ^ 1u);  // the slot's previous row has been read
+    float* row = RF::slot(s) + 4 * t;
+#pragma unroll 1
+    for (int cg = 0; cg < Plan::kGatherLevels / 2; ++cg) {  // column group of 4 floats = levels l0, l0 + 1
+      const int l0 = L - Plan::kGatherLevels + 2 * cg;
+      const float2 e0 = level_gather(table, pos, F.scalings[l0], l0, F.log2T);
+      const float2 e1 = level_gather(table, pos, F.scalings[l0 + 1], l0 + 1, F.log2T);
+      const float4 v = make_float4(e0.x, e0.y, e1.x, e1.y);
+      *reinterpret_cast<float4*>(row + cg * wg::kRowsGroupStride) = v;
+      if (stash && valid) reinterpret_cast<float4*>(stash + (size_t)p * CfgSmall::ENC)[l0 / 2] = v;
+    }
+    wg::mbar_arrive(RF::full(s));
+  }
+}
+
+// The resident kernels' split of the CTA into the gather warpgroup, which runs gather_encodings and returns false, and
+// the MMA warpgroups, which return true.
+template <class Position>
+__device__ __forceinline__ bool mma_warpgroup(const KField& F, const KParams& P, long long N, float* stash, Position position) {
+  ResidentForward::build_image(P);
+  if (wg::group() == ForwardPlan::kGroups) {
+    wg::setmaxnreg_dec<ForwardPlan::kGatherRegs>();
+    gather_encodings(F, P, N, stash, position);
+    return false;
+  }
+  wg::setmaxnreg_inc<ForwardPlan::kMmaRegs>();
+  return true;
+}
+
+// The encoding of an MMA warpgroup's k-th point: levels [0, L - kGatherLevels) gathered here with level_gather (four
+// levels per step) and stored to the stash, when there is one; the others from the ring.  With
+// -DFNR_FWD_NO_GATHER (a diagnostic build that times the MMA warpgroups alone) a made-up row.
+__device__ __forceinline__ void resident_encoding(const KField& F, const KParams& P, long long k, const Vec3& pos, float* stash_row,
+                                                  float (&enc)[CfgSmall::ENC]) {
+#ifdef FNR_FWD_NO_GATHER
+#pragma unroll
+  for (int l = 0; l < CfgSmall::L; ++l) {
+    enc[2 * l] = pos.x;
+    enc[2 * l + 1] = pos.y + pos.z;
+  }
+#else
+  constexpr int kOwn = CfgSmall::L - ForwardPlan::kGatherLevels;
+  const float2* __restrict__ table = reinterpret_cast<const float2*>(P.hash_table);
+#pragma unroll 2
+  for (int cg = 0; cg < kOwn / 2; ++cg) {
+    const float2 e0 = level_gather(table, pos, F.scalings[2 * cg], 2 * cg, F.log2T);
+    const float2 e1 = level_gather(table, pos, F.scalings[2 * cg + 1], 2 * cg + 1, F.log2T);
+    enc[4 * cg] = e0.x;
+    enc[4 * cg + 1] = e0.y;
+    enc[4 * cg + 2] = e1.x;
+    enc[4 * cg + 3] = e1.y;
+    if (stash_row) reinterpret_cast<float4*>(stash_row)[cg] = make_float4(e0.x, e0.y, e1.x, e1.y);
+  }
+  ResidentForward::ring_read(k, enc);
+#endif
+}
+
 // Every warpgroup takes whole 128-point tiles, tile g of CTA b then every (gridDim.x * warpgroups)-th one after it; threads
 // past N compute a clamped point and store nothing, so that the warpgroup-wide tensor-core layers see every thread.  A
 // warpgroup syncs on its own barrier only (wg::sync): the tile loop has no CTA-wide barrier, and a warpgroup without
 // tiles leaves at once.
 template <class C, bool TC>
-__global__ void __launch_bounds__(forward_threads<C, TC>()) simt_field_forward_kernel(KField F, KParams P, KRays Rr, KFieldOut O) {
-  constexpr int kGroups = forward_threads<C, TC>() / kThreads;
+__global__ void __launch_bounds__(forward_threads<C, TC>(), forward_min_ctas<C, TC>()) simt_field_forward_kernel(KField F, KParams P, KRays Rr, KFieldOut O) {
+  constexpr bool kResident = on_resident_image<C, TC>();
+  constexpr int kGroups = forward_groups<C, TC>();
   using Lin = ForwardLayers<C, TC>;
   __shared__ float s_app[C::APP];
   block_mean_embedding(P, F.num_images, C::APP, F.appearance_mode, s_app);
-  if constexpr (on_resident_image<C, TC>()) ResidentForward::build_image(P);
   const long long N = (long long)Rr.R * Rr.S;
+  if constexpr (kResident) {
+    const bool mma = mma_warpgroup(F, P, N, O.stash_encoding, [&](long long p) {
+      const int r = (int)(p / Rr.S);
+      bool sel;
+      return field_position(Rr.origins + 3 * (size_t)r, Rr.directions + 3 * (size_t)r, Rr.starts[p], Rr.ends[p], F.position_mode,
+                            F.aabb, sel);
+    });
+    if (!mma) return;
+  }
   const int g = group_of<kGroups>();
   const unsigned t = thread_of<kGroups>();
-  for (long long p0 = (long long)blockIdx.x * blockDim.x + g * kThreads; p0 < N; p0 += (long long)gridDim.x * blockDim.x) {
+  const unsigned span = kResident ? kGroups * kThreads : blockDim.x;  // points of a CTA's round of tiles
+  long long k = 0;  // the warpgroup's tile count
+  for (long long p0 = (long long)blockIdx.x * span + g * kThreads; p0 < N; p0 += (long long)gridDim.x * span, ++k) {
     const bool valid = p0 + t < N;
     const long long p = valid ? p0 + t : N - 1;
     const int r = (int)(p / Rr.S);
@@ -595,11 +729,15 @@ __global__ void __launch_bounds__(forward_threads<C, TC>()) simt_field_forward_k
     bool sel;
     const Vec3 pos = field_position(o, d, Rr.starts[p], Rr.ends[p], F.position_mode, F.aabb, sel);
     float enc[C::ENC];
-    hash_encode<C::L>(reinterpret_cast<const float2*>(P.hash_table), F.scalings, F.log2T, pos, enc);
-    if (O.stash_encoding && valid) {
-      float4* st = reinterpret_cast<float4*>(O.stash_encoding + (size_t)p * C::ENC);
+    if constexpr (kResident) {
+      resident_encoding(F, P, k, pos, O.stash_encoding && valid ? O.stash_encoding + (size_t)p * C::ENC : nullptr, enc);
+    } else {
+      hash_encode<C::L>(reinterpret_cast<const float2*>(P.hash_table), F.scalings, F.log2T, pos, enc);
+      if (O.stash_encoding && valid) {
+        float4* st = reinterpret_cast<float4*>(O.stash_encoding + (size_t)p * C::ENC);
 #pragma unroll
-      for (int i = 0; i < C::ENC / 4; ++i) st[i] = make_float4(enc[4 * i], enc[4 * i + 1], enc[4 * i + 2], enc[4 * i + 3]);
+        for (int i = 0; i < C::ENC / 4; ++i) st[i] = make_float4(enc[4 * i], enc[4 * i + 1], enc[4 * i + 2], enc[4 * i + 3]);
+      }
     }
     // not load_appearance: selecting the source row once compiles to ~130 fewer instructions in this kernel
     const float* app = (F.appearance_mode == FNR_APP_PER_CAMERA)
@@ -1114,34 +1252,49 @@ __device__ __forceinline__ int warp_claim(int* counter, bool pred, int lane, int
 }
 
 template <class C, bool TC>
-__global__ void __launch_bounds__(forward_threads<C, TC>()) simt_export_kernel(KField F, KParams P, KExport E) {
-  constexpr int kGroups = forward_threads<C, TC>() / kThreads;
+__global__ void __launch_bounds__(forward_threads<C, TC>(), forward_min_ctas<C, TC>()) simt_export_kernel(KField F, KParams P, KExport E) {
+  constexpr bool kResident = on_resident_image<C, TC>();
+  constexpr int kGroups = forward_groups<C, TC>();
   using Lin = ForwardLayers<C, TC>;
   __shared__ float s_app[C::APP];
   block_mean_embedding(P, F.num_images, C::APP, FNR_APP_MEAN, s_app);
-  if constexpr (on_resident_image<C, TC>()) ResidentForward::build_image(P);
   const int lane = threadIdx.x & 31;
   const long long N = (long long)E.B * E.S;
-  const int g = group_of<kGroups>();
-  const unsigned t = thread_of<kGroups>();
-  // whole 128-point tiles per warpgroup (see simt_field_forward_kernel): warp-converged row claims, warpgroup-wide MLP layers
-  for (long long p0 = (long long)blockIdx.x * blockDim.x + g * kThreads; p0 < N; p0 += (long long)gridDim.x * blockDim.x) {
-    const long long p = p0 + t;
-    const bool valid = p < N;
-    const long long pc = valid ? p : N - 1;
+  // UniformSamplerWithNoise (eval): bins = linspace(0,1,S+1) (made on the host, as the reference does:
+  // components/ray_samplers.py:75); t = bins*far + (1-bins)*near
+  auto position = [&](long long pc, bool& sel, Vec3& world) {
     const int r = (int)(pc / E.S), s = (int)(pc % E.S);
-    // UniformSamplerWithNoise (eval): bins = linspace(0,1,S+1) (made on the host, as the
-    // reference does: components/ray_samplers.py:75); t = bins*far + (1-bins)*near
     const float* bins = E.bins + (size_t)r * E.bins_ray_stride;  // per-ray jittered bins when the stride is S+1
     const float b0 = __ldg(bins + s), b1 = __ldg(bins + s + 1);
     const float t0 = __fadd_rn(__fmul_rn(b0, E.far_plane), __fmul_rn(__fsub_rn(1.0f, b0), E.near_plane));
     const float t1 = __fadd_rn(__fmul_rn(b1, E.far_plane), __fmul_rn(__fsub_rn(1.0f, b1), E.near_plane));
-    const float* o = E.origins + 3 * (size_t)r;
+    return field_position(E.origins + 3 * (size_t)r, E.normal, t0, t1, FNR_POS_AABB, F.aabb, sel, &world);
+  };
+  if constexpr (kResident) {
+    const bool mma = mma_warpgroup(F, P, N, nullptr, [&](long long pc) {
+      bool sel;
+      Vec3 world;
+      return position(pc, sel, world);
+    });
+    if (!mma) return;
+  }
+  const int g = group_of<kGroups>();
+  const unsigned t = thread_of<kGroups>();
+  const unsigned span = kResident ? kGroups * kThreads : blockDim.x;  // points of a CTA's round of tiles
+  long long k = 0;                                                    // the warpgroup's tile count
+  // whole 128-point tiles per warpgroup (see simt_field_forward_kernel): warp-converged row claims, warpgroup-wide MLP layers
+  for (long long p0 = (long long)blockIdx.x * span + g * kThreads; p0 < N; p0 += (long long)gridDim.x * span, ++k) {
+    const long long p = p0 + t;
+    const bool valid = p < N;
+    const long long pc = valid ? p : N - 1;
     bool sel;
     Vec3 world;
-    const Vec3 pos = field_position(o, E.normal, t0, t1, FNR_POS_AABB, F.aabb, sel, &world);
+    const Vec3 pos = position(pc, sel, world);
     float enc[C::ENC];
-    hash_encode<C::L>(reinterpret_cast<const float2*>(P.hash_table), F.scalings, F.log2T, pos, enc);
+    if constexpr (kResident)
+      resident_encoding(F, P, k, pos, nullptr, enc);
+    else
+      hash_encode<C::L>(reinterpret_cast<const float2*>(P.hash_table), F.scalings, F.log2T, pos, enc);
     float appv[C::APP];
     load_appearance(P, FNR_APP_MEAN, 0, s_app, appv);
     Acts<C> a;
@@ -1263,13 +1416,15 @@ static int launch_field_kernel(Kernel kernel, int smem, long long N, const char*
 }
 
 // One launch of a resident kernel (the small family's tensor-core forward, export and backward): one CTA of `threads`
-// per SM (its shared memory is most of the SM's), no more CTAs than the points need.
+// per SM (its shared memory is most of the SM's), no more CTAs than the points need (`groups` MMA warpgroups per CTA,
+// 128 points each).
 template <class Kernel, class... Args>
-static int launch_resident(Kernel kernel, int threads, int smem, long long N, const char* name, cudaStream_t st, const Args&... args) {
+static int launch_resident(Kernel kernel, int threads, int groups, int smem, long long N, const char* name, cudaStream_t st,
+                           const Args&... args) {
   if (N == 0) return FNR_OK;
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute");
-  kernel<<<grid_for(N, threads, sm_count()), threads, smem, st>>>(args...);
+  kernel<<<grid_for(N, groups * kThreads, sm_count()), threads, smem, st>>>(args...);
   return check_launch(name);
 }
 
@@ -1285,7 +1440,7 @@ int launch_field_forward(Family fam, bool tc, const KField& F, const KParams& P,
     using C = decltype(c);
     constexpr bool TC = decltype(t)::value;
     if constexpr (on_resident_image<C, TC>())
-      return launch_resident(simt_field_forward_kernel<C, TC>, forward_threads<C, TC>(), ForwardPlan::kBytes, (long long)Rr.R * Rr.S,
+      return launch_resident(simt_field_forward_kernel<C, TC>, forward_threads<C, TC>(), ForwardPlan::kGroups, ForwardPlan::kBytes, (long long)Rr.R * Rr.S,
                              "simt_field_forward_kernel<wgmma>", st, F, P, Rr, O);
     return launch_field_kernel(simt_field_forward_kernel<C, TC>, Layers<C, TC>::kFwdSmemBytes, (long long)Rr.R * Rr.S,
                                TC ? "simt_field_forward_kernel<wgmma>" : "simt_field_forward_kernel", st, F, P, Rr, O);
@@ -1298,7 +1453,7 @@ int launch_field_backward(Family fam, bool tc, const KField& F, const KParams& P
     using C = decltype(c);
     constexpr bool TC = decltype(t)::value;
     if constexpr (on_resident_image<C, TC>())
-      return launch_resident(simt_field_backward_kernel<C, TC>, backward_threads<C, TC>(), BackwardPlan::kBytes, (long long)Rr.R * Rr.S,
+      return launch_resident(simt_field_backward_kernel<C, TC>, backward_threads<C, TC>(), BackwardPlan::kGroups, BackwardPlan::kBytes, (long long)Rr.R * Rr.S,
                              "simt_field_backward_kernel<wgmma>", st, F, P, G, Rr, B);
     return launch_field_kernel(simt_field_backward_kernel<C, TC>, Layers<C, TC>::kBwdSmemBytes, (long long)Rr.R * Rr.S,
                                TC ? "simt_field_backward_kernel<wgmma>" : "simt_field_backward_kernel", st, F, P, G, Rr, B);
@@ -1327,7 +1482,7 @@ int launch_export(Family fam, bool tc, const KField& F, const KParams& P, const 
     using C = decltype(c);
     constexpr bool TC = decltype(t)::value;
     if constexpr (on_resident_image<C, TC>())
-      return launch_resident(simt_export_kernel<C, TC>, forward_threads<C, TC>(), ForwardPlan::kBytes, (long long)E.B * E.S,
+      return launch_resident(simt_export_kernel<C, TC>, forward_threads<C, TC>(), ForwardPlan::kGroups, ForwardPlan::kBytes, (long long)E.B * E.S,
                              "simt_export_kernel<wgmma>", st, F, P, E);
     return launch_field_kernel(simt_export_kernel<C, TC>, Layers<C, TC>::kFwdSmemBytes, (long long)E.B * E.S,
                                TC ? "simt_export_kernel<wgmma>" : "simt_export_kernel", st, F, P, E);

@@ -69,6 +69,32 @@ __device__ __forceinline__ void wait_all() { asm volatile("wgmma.wait_group.sync
 // generic-proxy shared-memory stores -> visible to the async proxy that wgmma reads operands through
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
+// mbarriers in shared memory (a ring between warpgroups of a CTA): init by one thread, then a CTA barrier before use;
+// arrive has release and a completed wait acquire semantics at CTA scope, so the generic-proxy stores before an arrive
+// are visible to the loads after the wait that sees its phase complete.
+__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+// Waits until the phase with parity `parity` of the barrier has completed.
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+  asm volatile(
+      "{\n\t.reg .pred done;\n"
+      "WAIT_%=:\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 done, [%0], %1;\n\t"
+      "@!done bra WAIT_%=;\n\t}" ::"r"(smem_u32(bar)),
+      "r"(parity)
+      : "memory");
+}
+// The registers per thread of the calling warpgroup (warpgroup-uniform; the CTA's sum must stay within what it was
+// launched with).
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+
 // D[64, N] (+)= A[64, 16] B[N, 16]^T, bf16 operands from shared memory, fp32 accumulators in registers.  TA / TB: the
 // operand is MN-major (the transpose bit).
 template <int N, int TA = 0, int TB = 0>

@@ -2,12 +2,16 @@
 (4096 rays x 192 samples, the bench.py field and batch), in training mode (the encoding stash written for the backward)
 and in inference mode.
 
-    python tools/bench_forward.py [--variant small|big] [--kernel auto|simt|tcgen05] [--steps 20] [--kernels] [--lib FILE] [--json FILE]
+    python tools/bench_forward.py [--variant small|big] [--kernel auto|simt|tcgen05] [--steps 20] [--kernels] [--lib FILE]
+                                  [--no-gather [--build-dir DIR]] [--json FILE]
 
 Each timed call is one `ops.render` (output allocation + the library call), CUDA events around it, the L2 flushed before
 every call as bench.py does.  `--kernels` then runs the same calls again under torch.profiler, in a run of their own after
 the timed one, and adds the device time of each kernel of the forward per call (field forward and compositing).  `--lib`
-times another build of the library (the C ABI is the same), such as one with -DFNR_FWD_GROUPS=3.
+times another build of the library (the C ABI is the same).  `--no-gather` builds the library with -DFNR_FWD_NO_GATHER into
+--build-dir (a temporary directory by default, never the package's own library) and times that: fruit_nerf's
+tensor-core forward and export then make up their encodings instead of gathering them from the hash table, so the
+difference to the normal build is the most that hiding the gather could save.  Its outputs are meaningless.
 """
 from __future__ import annotations
 
@@ -15,6 +19,7 @@ import argparse
 import json
 import statistics
 import sys
+import tempfile
 from pathlib import Path
 
 ROOT = Path(__file__).resolve().parent.parent
@@ -33,12 +38,20 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--kernels", action="store_true", help="device time per kernel from a torch.profiler run after the timed one")
     ap.add_argument("--lib", default=None, help="library to time (default: the package's)")
+    ap.add_argument("--no-gather", action="store_true", help="time a -DFNR_FWD_NO_GATHER build (diagnostic)")
+    ap.add_argument("--build-dir", default=None, help="where --no-gather builds its library (default: a temporary directory)")
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
 
     from fruitnerf_b200 import _lib as L
 
-    if args.lib:
+    tmp = None
+    if args.no_gather:
+        from fruitnerf_b200 import _build
+
+        out = args.build_dir or (tmp := tempfile.TemporaryDirectory(prefix="fnr_no_gather_")).name
+        L.LIB_PATH = _build.build(defines=["FNR_FWD_NO_GATHER"], out_dir=out)
+    elif args.lib:
         L.LIB_PATH = Path(args.lib).resolve()
     L.load()
 
@@ -93,6 +106,8 @@ def main():
     if args.json:
         Path(args.json).parent.mkdir(parents=True, exist_ok=True)
         Path(args.json).write_text(line + "\n")
+    if tmp is not None:
+        tmp.cleanup()
 
 
 if __name__ == "__main__":
