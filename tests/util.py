@@ -33,6 +33,10 @@ def assert_rel(actual, expected, rel=REL, floor=FLOOR, what=""):
 
 
 def variant(name: str):
+    """Field hyper-parameters of "small" (fruit_nerf), "big" (fruit_nerf_big) or "huge" (fruit_nerf_huge: the big network
+    on a max_res 8192 grid)."""
+    if name == "huge":
+        return dict(syn.BIG, max_res=8192)
     return dict(syn.SMALL if name == "small" else syn.BIG)
 
 
@@ -142,14 +146,26 @@ def coefficient_loss(coefs: dict, keys=UPSTREAM_KEYS):
     return loss
 
 
-def mse_bce_loss(image, mask):
-    """FruitModel's rgb MSE + semantic BCE (fruit_nerf.py:359-366), each ray weighted by w."""
+def mse_bce_loss(image, mask, batch_rays=None):
+    """FruitModel's rgb MSE + semantic BCE (fruit_nerf.py:359-366), each ray weighted by w.  The means are over
+    ``batch_rays`` rays (default: the rays given), so that the rays of a part of a batch get the whole batch's loss terms."""
     def loss(out, w):
         w = w.to(out["rgb"])
-        R = w.shape[0]
+        R = w.shape[0] if batch_rays is None else batch_rays
         bce = torch.nn.functional.binary_cross_entropy_with_logits(out["semantics"], mask.to(out["rgb"]).reshape(-1), reduction="none")
         return (w[:, None] * (image.to(out["rgb"]) - out["rgb"]) ** 2).sum() / (3 * R) + (w * bce).sum() / R
     return loss
+
+
+def ray_loss(kind: str, R: int, S: int, keys=UPSTREAM_KEYS):
+    """loss_of(rays=slice(None)) -> loss(out, w) of the rays ``rays`` (a slice or index tensor) of an R x S batch:
+    "mse_bce" (mse_bce_loss of syn.targets(R)) or the linear loss of upstream_coefficients(R, S) on ``keys``.  Both are sums
+    over rays, so the losses of disjoint sets of rays add up to the whole batch's."""
+    if kind == "mse_bce":
+        img, mask = syn.targets(R)
+        return lambda rays=slice(None): mse_bce_loss(img[rays], mask[rays], batch_rays=R)
+    coefs = upstream_coefficients(R, S)
+    return lambda rays=slice(None): coefficient_loss({k: c[rays] for k, c in coefs.items()}, keys)
 
 
 @dataclass
@@ -161,14 +177,21 @@ class OracleRun:
     loss: torch.Tensor
 
 
+def oracle_params(sd, dtype=torch.float64) -> dict:
+    """The parameters of a state dict as ``dtype`` leaves that require grad (the aabb and integer buffers as they are)."""
+    return {k: v.detach().to(dtype, copy=True).requires_grad_(True) if v.is_floating_point() and k != "aabb" else v
+            for k, v in sd.items()}
+
+
 def oracle_backward(sd, spec, rays, loss_fn, contraction=True, appearance="train", training=True, pass_semantic_gradients=False,
-                    dtype=torch.float64, ray_weights=None, mutate=None, min_rays=8) -> OracleRun:
+                    dtype=torch.float64, ray_weights=None, mutate=None, min_rays=8, params=None) -> OracleRun:
     """Autograd through the oracle with the parameters in ``dtype``.  Rays stay float32, so sample positions (and hash rows
     and trilinear offsets) are bit-equal to the kernels' (test_gpu_parity.py::test_hash_rows_bit_exact).  ``ray_weights``:
-    per-ray loss weights (default: this run's ReLU margins); ``mutate(out) -> out`` edits the outputs before the loss."""
+    per-ray loss weights (default: this run's ReLU margins); ``mutate(out) -> out`` edits the outputs before the loss.
+    ``params``: oracle_params(sd, dtype) to add this run's gradients to (default: fresh ones)."""
     o, d, s, e, cam = rays
-    params = {k: v.detach().to(dtype, copy=True).requires_grad_(True) if v.is_floating_point() and k != "aabb" else v
-              for k, v in sd.items()}
+    if params is None:
+        params = oracle_params(sd, dtype)
     sp = replace(spec, pass_semantic_gradients=pass_semantic_gradients)
     f = fr.field_forward(params, sp, o[:, None, :], d[:, None, :], s[..., None], e[..., None], cam, contraction=contraction,
                          appearance=appearance)
@@ -181,6 +204,59 @@ def oracle_backward(sd, spec, rays, loss_fn, contraction=True, appearance="train
     loss.backward()
     grads = {k: (p.grad if p.grad is not None else torch.zeros_like(p)).detach() for k, p in params.items() if p.requires_grad}
     return OracleRun(grads, f, out, ray_weights, loss.detach())
+
+
+def chunked_oracle_backward(sd, spec, rays, loss_of, chunk=512, contraction=True, appearance="train", training=True,
+                            pass_semantic_gradients=False, dtype=torch.float64, ray_weights=None, min_rays=8) -> OracleRun:
+    """oracle_backward of the loss ``loss_of()`` (see ray_loss) over chunks of ``chunk`` rays, the gradients of the chunks'
+    losses ``loss_of(chunk)`` summed: exact, since the loss is a sum over rays, and it bounds the autograd graph (at 4096 x 48
+    samples one graph in float64 takes several GB).  The default ray weights are the unchunked run's: safe_ray_weights of one
+    forward over the whole batch, whose ReLU margins are relative to the layer rms over field_forward's own sample chunks.
+    ``field`` and ``out`` hold the chunks' tensors concatenated, detached."""
+    R = rays[2].shape[0]
+    params = oracle_params(sd, dtype)
+    if ray_weights is None:
+        o, d, s, e, cam = rays
+        with torch.no_grad():
+            f = fr.field_forward(params, spec, o[:, None, :], d[:, None, :], s[..., None], e[..., None], cam, contraction=contraction,
+                                 appearance=appearance)
+        ray_weights = safe_ray_weights(f, min_rays)
+        del f
+    fields, outs, loss = [], [], 0.0
+    for a in range(0, R, chunk):
+        part = slice(a, min(R, a + chunk))
+        run = oracle_backward(sd, spec, tuple(t[part] for t in rays), loss_of(part), contraction=contraction, appearance=appearance,
+                              training=training, pass_semantic_gradients=pass_semantic_gradients, dtype=dtype,
+                              ray_weights=ray_weights[part], params=params)
+        fields.append({k: v.detach() for k, v in run.field.items()})
+        outs.append({k: v.detach() for k, v in run.out.items()})
+        loss = loss + run.loss
+    grads = {k: (p.grad if p.grad is not None else torch.zeros_like(p)).detach() for k, p in params.items() if p.requires_grad}
+    return OracleRun(grads, {k: torch.cat([f[k] for f in fields]) for k in fields[0]},
+                     {k: torch.cat([o[k] for o in outs]) for k in outs[0]}, ray_weights, loss)
+
+
+# ---- the field backward's tile schedule ---------------------------------------------------------------------------------------
+TILE_POINTS = 128  # points of one warpgroup tile of the field kernels
+RESIDENT_GROUPS = 2  # warpgroups per CTA of the small family's tensor-core backward
+
+
+def resident_backward_rounds(N: int, sms: int):
+    """([tiles] round of each tile, CTA count) of the small family's tensor-core backward over N points on a GPU of ``sms``
+    SMs (fnr_simt.cu: launch_resident, simt_field_backward_kernel): min(ceil(N / 256), sms) CTAs of two warpgroups;
+    warpgroup g of CTA b takes tile 2b + g, then every (2 * CTAs)-th tile after it, so tile t runs in round
+    t // (2 * CTAs).  A CTA keeps its weight gradients on chip over all its rounds and flushes them after the last."""
+    tiles = -(-N // TILE_POINTS)
+    grid = min(-(-N // (RESIDENT_GROUPS * TILE_POINTS)), sms)
+    return torch.arange(tiles) // (RESIDENT_GROUPS * grid), grid
+
+
+def live_rays_per_round(rounds: torch.Tensor, ray_weights: torch.Tensor, S: int) -> list:
+    """Per round, the number of rays of nonzero weight with a sample in one of the round's tiles."""
+    R = ray_weights.shape[0]
+    point_round = rounds.repeat_interleave(TILE_POINTS)[:R * S].view(R, S)
+    live = ray_weights > 0
+    return [int((live & (point_round == k).any(dim=1)).sum()) for k in range(int(rounds.max()) + 1)]
 
 
 def make_field(name: str, sd, spec, device, contraction=True, test_mode=None, **kw) -> FruitField:
