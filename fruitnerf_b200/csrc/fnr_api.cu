@@ -223,9 +223,9 @@ int fnr_render_backward_scratch_bytes(const fnr_field_desc* desc, int32_t num_ra
   }
   const size_t n = (size_t)num_rays * num_samples;
   *bytes = n * 5 * sizeof(float) + 256;  // per-point upstream gradients, 256-byte aligned
-  // the small family's tensor-core backward also keeps the encoding gradients, [L][N] float2, for the level-major
-  // scatter kernel
-  if (desc->impl != FNR_IMPL_SIMT && classify(desc) == kFamilySmall) *bytes += 256 + n * desc->num_levels * desc->features_per_level * sizeof(float);
+  // a backward that runs the level-major scatter kernel also keeps the encoding gradients, [L][N] float2
+  if (backward_uses_level_scatter(classify(desc), desc->impl != FNR_IMPL_SIMT))
+    *bytes += 256 + n * desc->num_levels * desc->features_per_level * sizeof(float);
   return FNR_OK;
 }
 
@@ -276,7 +276,7 @@ int fnr_render_backward(const fnr_field_desc* desc, const fnr_field_params* para
   if ((rc = launch_simt_composite_backward(Rr, B, st))) return rc;
   const bool tc = desc->impl != FNR_IMPL_SIMT;
   const uintptr_t denc_at = reinterpret_cast<uintptr_t>(point_grads + (size_t)Rr.R * Rr.S * 5);
-  float2* denc = tc && fam == kFamilySmall ? reinterpret_cast<float2*>((denc_at + 255) & ~(uintptr_t)255) : nullptr;
+  float2* denc = backward_uses_level_scatter(fam, tc) ? reinterpret_cast<float2*>((denc_at + 255) & ~(uintptr_t)255) : nullptr;
   const KFieldBwd FB{point_grads, saved->stash_encoding, denc};
   return launch_field_backward(fam, tc, F, P, G, Rr, FB, st);
 }

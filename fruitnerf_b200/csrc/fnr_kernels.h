@@ -226,8 +226,13 @@ inline int grid_for(long long work, int per_block, int max_blocks) {
 }
 
 // Field kernels of fnr_simt.cu for a shipped family: tc selects the tensor-core (wgmma, sm_90a) instantiation, otherwise
-// the exact-fp32 simt one.  The small family's tensor-core backward is two launches: the field backward stores the encoding
-// gradients to B.denc, and level_scatter_kernel adds them to the table gradient one level at a time.
+// the exact-fp32 simt one.  Each runs its layers on one layer type, which also gives its launch geometry: the small
+// family's tensor-core kernels are persistent CTAs on a resident weight image, the others one-warpgroup CTAs.
+// When backward_uses_level_scatter(fam, tc) (the small family's tensor-core backward), the backward is two launches: the
+// field backward stores the encoding gradients to B.denc ([L][N] float2, in the caller's scratch), and
+// level_scatter_kernel adds them to the table gradient one level at a time; otherwise the field backward adds them itself
+// and B.denc is NULL.
+bool backward_uses_level_scatter(Family fam, bool tc);
 int launch_field_forward(Family fam, bool tc, const KField& F, const KParams& P, const KRays& Rr, const KFieldOut& O, cudaStream_t st);
 int launch_field_backward(Family fam, bool tc, const KField& F, const KParams& P, const KParams& G, const KRays& Rr, const KFieldBwd& B,
                           cudaStream_t st);

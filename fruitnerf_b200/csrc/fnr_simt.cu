@@ -1,10 +1,13 @@
 // Kernels of the FruitNeRF hot path: one thread per sample point, per-ray compositing by one warp per ray.
 //
-// The field kernels (forward, export, backward) are instantiated twice through Layers<C, TC>.  TC = false is the "simt"
-// implementation, the exact-fp32 device path: MLP weights read straight from the torch parameter tensors through the
-// read-only path (warp-uniform addresses, float4 where the row alignment allows); it is the on-device fp32 reference
-// the tensor-core path is checked against at full size.  TC = true runs the MLP layers block-wide on the Hopper tensor
-// cores (fnr_wgmma.cuh).
+// The field kernels (forward, export, backward) are instantiated per family C (CfgSmall, CfgBig) and implementation TC,
+// and evaluate their Linear layers through a layer type (FieldLayers) that names each layer by its Slot.  TC = false is
+// the "simt" implementation on Layers<C, false>, the exact-fp32 device path: MLP weights read straight from the torch
+// parameter tensors through the read-only path (warp-uniform addresses, float4 where the row alignment allows); it is the
+// on-device fp32 reference the tensor-core path is checked against at full size.  TC = true runs the MLP layers
+// warpgroup-wide on the Hopper tensor cores (fnr_wgmma.cuh): the big family on Layers<CfgBig, true>, which stages each
+// layer's weights at every step, the small family on ResidentLayers<Plan>, persistent CTAs that hold the weights in
+// shared memory.  The layer type also gives its kernels' launch geometry.
 //
 // Reference semantics: fruit_nerf/fruit_field.py:168-301, fruit_nerf/fruit_nerf.py:251-269,316-357.
 #include <type_traits>
@@ -16,6 +19,10 @@ namespace fnr {
 
 constexpr int kThreads = 128;
 
+// The field's Linear layers.  The first six are the small family's tensor-core layers in the order of its resident
+// weight image; kSem2 exists in the big family only.
+enum Slot { kBase0, kBase1, kSem0, kSem1, kCol0, kCol1, kHead, kCol2, kSem2 };
+
 template <int GEO_, int SEM_LAYERS_, int SEM_H_>
 struct Cfg {
   static constexpr int L = 16, ENC = 32;
@@ -26,6 +33,15 @@ struct Cfg {
   static constexpr int APP = 32, SH = 16;
   static constexpr int COL_IN = SH + GEO_ + APP, COL_H = 64;
   static constexpr int MAXW = (SEM_H_ > COL_IN ? SEM_H_ : COL_IN) > 64 ? (SEM_H_ > COL_IN ? SEM_H_ : COL_IN) : 64;
+  // Shape of slot s's layer W [N][K]; 0 for a slot the family does not have
+  static constexpr int K(int s) {
+    return s == kBase0 ? ENC : s == kBase1 ? BASE_H : s == kSem0 ? GEO : s == kSem1 ? SEM_H : s == kSem2 ? (SEM_LAYERS == 3 ? SEM_H : 0)
+         : s == kCol0 ? COL_IN : s == kHead ? SEM_OUT : COL_H;
+  }
+  static constexpr int N(int s) {
+    return s == kBase0 ? BASE_H : s == kBase1 ? BASE_OUT : s == kSem0 ? SEM_H : s == kSem1 ? (SEM_LAYERS == 3 ? SEM_H : SEM_OUT)
+         : s == kSem2 ? (SEM_LAYERS == 3 ? SEM_OUT : 0) : s == kHead ? 1 : s == kCol2 ? 3 : COL_H;
+  }
 };
 using CfgSmall = Cfg<15, 2, 64>;
 using CfgBig = Cfg<30, 3, 128>;
@@ -143,22 +159,45 @@ __device__ __forceinline__ void tile_weight_grad(float* __restrict__ sX, float* 
 
 constexpr int cmax(int a, int b) { return a > b ? a : b; }
 
-// The field's Linear layers.  The first six are the small family's tensor-core layers in the order of its resident
-// weight image; kSem2 exists in the big family only.
-enum Slot { kBase0, kBase1, kSem0, kSem1, kCol0, kCol1, kHead, kCol2, kSem2 };
+// Slot s's weight W [N][K] and bias [N] in a parameter set: the parameters P, or the gradients G they are added into
+__device__ __forceinline__ float* weight(const KParams& P, int s) {
+  return s == kBase0 ? P.base_w[0] : s == kBase1 ? P.base_w[1] : s == kSem0 ? P.sem_w[0] : s == kSem1 ? P.sem_w[1] : s == kSem2 ? P.sem_w[2]
+       : s == kCol0 ? P.col_w[0] : s == kCol1 ? P.col_w[1] : s == kHead ? P.head_w : P.col_w[2];
+}
+__device__ __forceinline__ float* bias(const KParams& P, int s) {
+  return s == kBase0 ? P.base_b[0] : s == kBase1 ? P.base_b[1] : s == kSem0 ? P.sem_b[0] : s == kSem1 ? P.sem_b[1] : s == kSem2 ? P.sem_b[2]
+       : s == kCol0 ? P.col_b[0] : s == kCol1 ? P.col_b[1] : s == kHead ? P.head_b : P.col_b[2];
+}
 
-// How the field kernels evaluate a Linear layer W [N][K] (SLOT: which one): forward y = act(W x + b), input gradient
-// dx = W^T dy and weight gradient dW = dY^T X over the tile.  TC = false: per thread in fp32 on the CUDA cores (the exact
+// The field kernels evaluate their Linear layers through a layer type (Layers<C, TC> or ResidentLayers<Plan>).  Both
+// have the same calls, each naming its layer by SLOT, whose shape the register arrays must have:
+//   fwd<SLOT, RELU>(P, x, y)           y = act(W x + b)
+//   fwd2<S0, S1, RELU1>(P, x, m, y)    m = relu(W0 x + b0), y = act(W1 m + b1)
+//   dx<SLOT>(P, dy, dxv)               dxv = W^T dy
+//   dw<SLOT>(G, x, dy)                 dW = dY^T X and db over the warpgroup's 128-point tile, added to G
+//   grad<SLOT>(P, G, x, dy, dxv)       dx and dw
+//   grad_relu<SLOT>(P, G, x, dy, dxv)  grad of a layer whose input x is a ReLU's output, dxv masked by that ReLU (x > 0)
+// and the same launch geometry of their kernels:
+//   kGroups                            MMA warpgroups per CTA (each takes its own 128-point tiles)
+//   kThreadsPerCta, kMinCtas           the kernels' __launch_bounds__ (kMinCtas = 0: none given)
+//   kFwdSmemBytes, kBwdSmemBytes       dynamic shared memory of the forward and export, and of the backward
+//   kResident                          one persistent CTA per SM on the resident weight image (the small family's
+//                                      tensor-core kernels); otherwise as many CTAs as fit on the SMs
+// Layers<C, TC> evaluates a layer in CTAs of one warpgroup.  TC = false: per thread in fp32 on the CUDA cores (the exact
 // device reference).  TC = true: warpgroup-wide on the tensor cores with the weight tile staged from global memory at
-// every step (fnr_wgmma.cuh; every thread of the 128-thread CTA must take part): the big family's tensor-core path.  The
-// small family's runs on ResidentLayers below.
+// every step (fnr_wgmma.cuh; every thread of the 128-thread CTA must take part): the big family's tensor-core path.
 template <class C, bool TC>
 struct Layers {
+  static constexpr int kGroups = 1;
+  static constexpr int kThreadsPerCta = kThreads;
+  static constexpr int kMinCtas = 0;
+  static constexpr bool kResident = false;
   // the 1- and 3-wide output heads (64 MACs per point) stay in exact fp32 on the CUDA cores on both paths
   static constexpr bool tensor(int n) { return TC && n >= 8; }
   // dynamic shared memory: the sX / sY tiles of tile_weight_grad, and the wgmma operand plans (the backward's heads
   // still use tile_weight_grad, so its tensor-core plan holds that tile too)
-  static constexpr int kTileBytes = 2 * kThreads * (((C::MAXW + 3) & ~3) + 4) * 4;
+  static constexpr int kTileFloats = ((C::MAXW + 3) & ~3) + 4;  // padded row stride of sX / sY
+  static constexpr int kTileBytes = 2 * kThreads * kTileFloats * 4;
   static constexpr int kFwdSmemBytes = TC ? wg::Smem<C::MAXW, C::MAXW>::kBytes : 0;
   static constexpr int kBwdSmemBytes =
       TC ? cmax(cmax(wg::Smem<C::MAXW, C::MAXW>::kBytes, wg::DwSmem<C::MAXW, C::MAXW>::kBytes), kTileBytes) : kTileBytes;
@@ -167,50 +206,77 @@ struct Layers {
     extern __shared__ __align__(128) uint8_t wg_smem[];
     return wg_smem;
   }
-  template <int SLOT, int K, int N, bool RELU>
-  static __device__ __forceinline__ void fwd(const float* __restrict__ W, const float* __restrict__ b, const float (&x)[K], float (&y)[N]) {
-    if constexpr (tensor(N))
-      wg::linear<C::MAXW, C::MAXW, K, N, RELU>(dyn_smem(), W, b, x, y);
+  static __device__ __forceinline__ float* sX() { return reinterpret_cast<float*>(dyn_smem()); }
+  static __device__ __forceinline__ float* sY() { return sX() + kThreads * kTileFloats; }
+
+  // The layer arithmetic on the slot's pointers.  Each call below reads all of its pointers before any arithmetic (fwd2:
+  // both layers'), where the call sites read them when they passed the pointers.  This is a codegen guard, not a
+  // semantic requirement: the position of the parameter loads steers ptxas's register allocation, and reading them
+  // later changed the SASS of the backward kernels.
+  template <bool RELU, int Kv, int Nv>
+  static __device__ __forceinline__ void linear(const float* __restrict__ W, const float* __restrict__ b, const float (&x)[Kv],
+                                                float (&y)[Nv]) {
+    if constexpr (tensor(Nv))
+      wg::linear<C::MAXW, C::MAXW, Kv, Nv, RELU>(dyn_smem(), W, b, x, y);
     else
-      linear_fwd<K, N, RELU>(W, b, x, y);
+      linear_fwd<Kv, Nv, RELU>(W, b, x, y);
   }
-  // m = relu(W0 x + b0), y = act(W1 m + b1): two steps
-  template <int S0, int S1, int K0, int N0, int N1, bool RELU1>
-  static __device__ __forceinline__ void fwd2(const float* __restrict__ W0, const float* __restrict__ b0, const float* __restrict__ W1,
-                                              const float* __restrict__ b1, const float (&x)[K0], float (&m)[N0], float (&y)[N1]) {
-    fwd<S0, K0, N0, true>(W0, b0, x, m);
-    fwd<S1, N0, N1, RELU1>(W1, b1, m, y);
-  }
-  template <int SLOT, int K, int N>
-  static __device__ __forceinline__ void dx(const float* __restrict__ W, const float (&dy)[N], float (&dxv)[K]) {
-    if constexpr (tensor(N))
-      wg::linear_dx<C::MAXW, C::MAXW, K, N>(dyn_smem(), W, dy, dxv);
+  template <int Kv, int Nv>
+  static __device__ __forceinline__ void input_grad(const float* __restrict__ W, const float (&dy)[Nv], float (&dxv)[Kv]) {
+    if constexpr (tensor(Nv))
+      wg::linear_dx<C::MAXW, C::MAXW, Kv, Nv>(dyn_smem(), W, dy, dxv);
     else
-      linear_bwd_input<K, N>(W, dy, dxv);
+      linear_bwd_input<Kv, Nv>(W, dy, dxv);
     FNR_PHASE(kPhDx);
   }
-  template <int SLOT, int K, int N>
-  static __device__ __forceinline__ void dw(float* sX, float* sY, const float (&x)[K], const float (&dy)[N], float* gW, float* gb) {
-    if constexpr (tensor(N))
-      wg::weight_grad<K, N>(dyn_smem(), x, dy, gW, gb);
+  template <int Kv, int Nv>
+  static __device__ __forceinline__ void weight_grad(const float (&x)[Kv], const float (&dy)[Nv], float* gW, float* gb) {
+    if constexpr (tensor(Nv))
+      wg::weight_grad<Kv, Nv>(dyn_smem(), x, dy, gW, gb);
     else
-      tile_weight_grad<K, N>(sX, sY, x, dy, gW, gb);
+      tile_weight_grad<Kv, Nv>(sX(), sY(), x, dy, gW, gb);
     FNR_PHASE(kPhDw);
   }
-  // Both gradients of one layer: dxv = W^T dy, then dW / db from (x, dy).
-  template <int SLOT, int K, int N>
-  static __device__ __forceinline__ void grad(const float* __restrict__ W, float* sX, float* sY, const float (&x)[K], const float (&dy)[N],
-                                              float (&dxv)[K], float* gW, float* gb) {
-    dx<SLOT, K, N>(W, dy, dxv);
-    dw<SLOT, K, N>(sX, sY, x, dy, gW, gb);
+
+  template <int SLOT, bool RELU, int Kv, int Nv>
+  static __device__ __forceinline__ void fwd(const KParams& P, const float (&x)[Kv], float (&y)[Nv]) {
+    static_assert(C::K(SLOT) == Kv && C::N(SLOT) == Nv, "slot shape");
+    linear<RELU>(weight(P, SLOT), bias(P, SLOT), x, y);
   }
-  // grad of a layer whose input x is a ReLU's output, with dxv masked by that ReLU (x > 0)
-  template <int SLOT, int K, int N>
-  static __device__ __forceinline__ void grad_relu(const float* __restrict__ W, float* sX, float* sY, const float (&x)[K],
-                                                   const float (&dy)[N], float (&dxv)[K], float* gW, float* gb) {
-    grad<SLOT, K, N>(W, sX, sY, x, dy, dxv, gW, gb);
+  // two steps
+  template <int S0, int S1, bool RELU1, int K0, int N0, int N1>
+  static __device__ __forceinline__ void fwd2(const KParams& P, const float (&x)[K0], float (&m)[N0], float (&y)[N1]) {
+    static_assert(C::K(S0) == K0 && C::N(S0) == N0 && C::K(S1) == N0 && C::N(S1) == N1, "slot shapes");
+    const float *W0 = weight(P, S0), *b0 = bias(P, S0), *W1 = weight(P, S1), *b1 = bias(P, S1);
+    linear<true>(W0, b0, x, m);
+    linear<RELU1>(W1, b1, m, y);
+  }
+  template <int SLOT, int Kv, int Nv>
+  static __device__ __forceinline__ void dx(const KParams& P, const float (&dy)[Nv], float (&dxv)[Kv]) {
+    static_assert(C::K(SLOT) == Kv && C::N(SLOT) == Nv, "slot shape");
+    input_grad(weight(P, SLOT), dy, dxv);
+  }
+  template <int SLOT, int Kv, int Nv>
+  static __device__ __forceinline__ void dw(const KParams& G, const float (&x)[Kv], const float (&dy)[Nv]) {
+    static_assert(C::K(SLOT) == Kv && C::N(SLOT) == Nv, "slot shape");
+    weight_grad(x, dy, weight(G, SLOT), bias(G, SLOT));
+  }
+  // dx, then dw
+  template <int SLOT, int Kv, int Nv>
+  static __device__ __forceinline__ void grad(const KParams& P, const KParams& G, const float (&x)[Kv], const float (&dy)[Nv],
+                                              float (&dxv)[Kv]) {
+    static_assert(C::K(SLOT) == Kv && C::N(SLOT) == Nv, "slot shape");
+    const float* W = weight(P, SLOT);
+    float *gW = weight(G, SLOT), *gb = bias(G, SLOT);
+    input_grad(W, dy, dxv);
+    weight_grad(x, dy, gW, gb);
+  }
+  template <int SLOT, int Kv, int Nv>
+  static __device__ __forceinline__ void grad_relu(const KParams& P, const KParams& G, const float (&x)[Kv], const float (&dy)[Nv],
+                                                   float (&dxv)[Kv]) {
+    grad<SLOT>(P, G, x, dy, dxv);
 #pragma unroll
-    for (int k = 0; k < K; ++k) dxv[k] = x[k] > 0.f ? dxv[k] : 0.f;
+    for (int k = 0; k < Kv; ++k) dxv[k] = x[k] > 0.f ? dxv[k] : 0.f;
   }
 };
 
@@ -226,20 +292,14 @@ using C = CfgSmall;
 static_assert(C::SEM_LAYERS == 2, "resident plan of the two-layer semantic MLP");
 constexpr int kSlots = 8;  // kBase0 .. kCol2
 constexpr int kImageSlots = 6;
-constexpr int K(int s) {
-  return s == kBase0 ? C::ENC : s == kBase1 ? C::BASE_H : s == kSem0 ? C::GEO : s == kSem1 ? C::SEM_H : s == kCol0 ? C::COL_IN
-                                                                                                      : s == kHead ? C::SEM_OUT : C::COL_H;
-}
-constexpr int N(int s) {
-  return s == kBase0 ? C::BASE_H : s == kBase1 ? C::BASE_OUT : s == kSem0 ? C::SEM_H : s == kSem1 ? C::SEM_OUT : s == kHead ? 1
-                                                                                                      : s == kCol2 ? 3 : C::COL_H;
-}
 constexpr bool tensor(int n) { return n >= 8; }
-constexpr int img_bytes(int s) { return 2 * wg::padn(N(s)) * wg::pad16(K(s)) * 2; }
+constexpr int img_bytes(int s) { return 2 * wg::padn(C::N(s)) * wg::pad16(C::K(s)) * 2; }
 constexpr int img_off(int s) { return s == 0 ? 0 : img_off(s - 1) + img_bytes(s - 1); }
 constexpr int kImageBytes = img_off(kImageSlots);
 static_assert(kImageBytes == 64 * 1024, "16384 split weights");
-constexpr int acc_floats(int s) { return tensor(N(s)) ? (N(s) + 15) / 16 * 32 * (wg::padn(K(s)) / 2) + N(s) : N(s) * K(s) + N(s); }
+constexpr int acc_floats(int s) {
+  return tensor(C::N(s)) ? (C::N(s) + 15) / 16 * 32 * (wg::padn(C::K(s)) / 2) + C::N(s) : C::N(s) * C::K(s) + C::N(s);
+}
 constexpr int acc_off(int s) { return s == 0 ? 0 : acc_off(s - 1) + (acc_floats(s - 1) + 3) / 4 * 4; }  // float4-aligned
 constexpr int align128(int b) { return (b + 127) / 128 * 128; }
 }  // namespace resident
@@ -255,6 +315,8 @@ constexpr int align128(int b) { return (b + 127) / 128 * 128; }
 struct ForwardPlan {
   static constexpr int kGroups = 2;
   static constexpr int kThreadsPerCta = (kGroups + 1) * kThreads;
+  // one CTA per SM named in __launch_bounds__, so that ptxas knows the registers at entry (168) and can apply setmaxnreg
+  static constexpr int kMinCtas = 1;
   static constexpr int kGatherRegs = 56, kMmaRegs = 224;
   static_assert(kThreads * (kGatherRegs + kGroups * kMmaRegs) <= kThreadsPerCta * 168, "register split of the CTA");
   static constexpr int kGatherLevels = 8;
@@ -271,6 +333,8 @@ struct ForwardPlan {
 // per-warpgroup dW operand regions.
 struct BackwardPlan {
   static constexpr int kGroups = 2;
+  static constexpr int kThreadsPerCta = kGroups * kThreads;
+  static constexpr int kMinCtas = 0;
   static constexpr int kAccOff = resident::kImageBytes;
   static constexpr int kLockOff = kAccOff + resident::acc_off(resident::kSlots) * 4;
   static constexpr int kStepOff = resident::align128(kLockOff + resident::kSlots * 4);
@@ -283,14 +347,16 @@ struct BackwardPlan {
 
 // The layers of the small family's tensor-core kernels on the resident image (Plan: the kernel's shared-memory plan).
 // fwd and fwd2 are the same code in the forward, the export and the backward's recompute; acc / lock / part, prepare, flush, dx
-// and dw exist in the backward's plan only.
+// and dw exist in the backward's plan only.  One plan per kernel, so both shared-memory sizes are the plan's.
 template <class Plan>
 struct ResidentLayers {
   using C = CfgSmall;
   static constexpr int kGroups = Plan::kGroups;
+  static constexpr int kThreadsPerCta = Plan::kThreadsPerCta;
+  static constexpr int kMinCtas = Plan::kMinCtas;
+  static constexpr int kFwdSmemBytes = Plan::kBytes, kBwdSmemBytes = Plan::kBytes;
+  static constexpr bool kResident = true;
   static constexpr int kSlots = resident::kSlots;
-  static constexpr int K(int s) { return resident::K(s); }
-  static constexpr int N(int s) { return resident::N(s); }
   static constexpr bool tensor(int n) { return resident::tensor(n); }
   static constexpr int img_off(int s) { return resident::img_off(s); }
   static constexpr int acc_off(int s) { return resident::acc_off(s); }
@@ -307,26 +373,18 @@ struct ResidentLayers {
     return reinterpret_cast<float*>(smem() + Plan::kAccOff) + off;
   }
   static __device__ __forceinline__ int* lock(int s) { return reinterpret_cast<int*>(smem() + Plan::kLockOff) + s; }
-  static __device__ __forceinline__ const float* weight(const KParams& P, int s) {
-    return s == kBase0 ? P.base_w[0] : s == kBase1 ? P.base_w[1] : s == kSem0 ? P.sem_w[0] : s == kSem1 ? P.sem_w[1]
-         : s == kCol0 ? P.col_w[0] : s == kCol1 ? P.col_w[1] : s == kHead ? P.head_w : P.col_w[2];
-  }
-  static __device__ __forceinline__ const float* bias(const KParams& P, int s) {
-    return s == kBase0 ? P.base_b[0] : s == kBase1 ? P.base_b[1] : s == kSem0 ? P.sem_b[0] : s == kSem1 ? P.sem_b[1]
-         : s == kCol0 ? P.col_b[0] : s == kCol1 ? P.col_b[1] : s == kHead ? P.head_b : P.col_b[2];
-  }
 
   // Split slot S's weights into the image exactly as rowgemm stages them (getw(n, k) = W[n][k], zero padding).
   template <int S>
   static __device__ __forceinline__ void split_image(const KParams& P) {
-    constexpr int NP = wg::padn(N(S)), KP = wg::pad16(K(S)), kChunks = NP * KP / 8;
+    constexpr int NP = wg::padn(C::N(S)), KP = wg::pad16(C::K(S)), kChunks = NP * KP / 8;
     const float* __restrict__ W = weight(P, S);
     uint8_t* hi = smem() + img_off(S);
     for (int i = threadIdx.x; i < kChunks; i += blockDim.x) {
       const int n = i % NP, kc = i / NP;
       float v[8];
 #pragma unroll
-      for (int j = 0; j < 8; ++j) v[j] = (n < N(S) && 8 * kc + j < K(S)) ? __ldg(W + (size_t)n * K(S) + 8 * kc + j) : 0.f;
+      for (int j = 0; j < 8; ++j) v[j] = (n < C::N(S) && 8 * kc + j < C::K(S)) ? __ldg(W + (size_t)n * C::K(S) + 8 * kc + j) : 0.f;
       wg::split_store8(hi, hi + NP * KP * 2, kc * (NP * 16) + n * 16, v);
     }
   }
@@ -384,9 +442,9 @@ struct ResidentLayers {
   // Slot S's accumulator added to the global gradient (reds: G may be a buffer other GPUs add into); after a CTA barrier.
   template <int S>
   static __device__ __forceinline__ void flush(const KParams& G) {
-    constexpr int Kv = K(S), Nv = N(S);
-    float* gW = const_cast<float*>(weight(G, S));
-    float* gb = const_cast<float*>(bias(G, S));
+    constexpr int Kv = C::K(S), Nv = C::N(S);
+    float* gW = weight(G, S);
+    float* gb = bias(G, S);
     const float* a = acc<S>();
     constexpr int kW = tensor(Nv) ? wg::DwAcc<Kv, Nv>::kW : Nv * Kv;
     for (int e = threadIdx.x; e < kW; e += blockDim.x) {
@@ -410,19 +468,20 @@ struct ResidentLayers {
   }
 
   // The fp32 heads only: every tensor-core layer runs in a chained pair (fwd2).
-  template <int SLOT, int Kv, int Nv, bool RELU>
-  static __device__ __forceinline__ void fwd(const float* __restrict__ W, const float* __restrict__ b, const float (&x)[Kv], float (&y)[Nv]) {
-    static_assert(K(SLOT) == Kv && N(SLOT) == Nv && !tensor(Nv), "slot shape");
-    linear_fwd<Kv, Nv, RELU>(W, b, x, y);
+  template <int SLOT, bool RELU, int Kv, int Nv>
+  static __device__ __forceinline__ void fwd(const KParams& P, const float (&x)[Kv], float (&y)[Nv]) {
+    static_assert(C::K(SLOT) == Kv && C::N(SLOT) == Nv && !tensor(Nv), "slot shape");
+    linear_fwd<Kv, Nv, RELU>(weight(P, SLOT), bias(P, SLOT), x, y);
   }
-  // Two tensor-core layers chained (wg::resident_chain), m = relu(W0 x + b0), y = act(W1 m + b1).  In the forward and
-  // the export, m goes from the first layer's accumulators to the second layer's operand tile without a round trip
-  // through rows, and is left unset.  The backward, whose weight gradients and ReLU masks read m, gets it as rows.  The
-  // bias and ReLU are the same fp32 operations either way, so m and y have the same bits.
-  template <int S0, int S1, int K0, int N0, int N1, bool RELU1>
-  static __device__ __forceinline__ void fwd2(const float* __restrict__, const float* __restrict__ b0, const float* __restrict__,
-                                              const float* __restrict__ b1, const float (&x)[K0], float (&m)[N0], float (&y)[N1]) {
-    static_assert(K(S0) == K0 && N(S0) == N0 && K(S1) == N0 && N(S1) == N1 && tensor(N0) && tensor(N1), "slot shapes");
+  // Two tensor-core layers chained (wg::resident_chain).  In the forward and the export, m goes from the first layer's
+  // accumulators to the second layer's operand tile without a round trip through rows, and is left unset.  The backward,
+  // whose weight gradients and ReLU masks read m, gets it as rows.  The bias and ReLU are the same fp32 operations either
+  // way, so m and y have the same bits.
+  template <int S0, int S1, bool RELU1, int K0, int N0, int N1>
+  static __device__ __forceinline__ void fwd2(const KParams& P, const float (&x)[K0], float (&m)[N0], float (&y)[N1]) {
+    static_assert(C::K(S0) == K0 && C::N(S0) == N0 && C::K(S1) == N0 && C::N(S1) == N1 && tensor(N0) && tensor(N1), "slot shapes");
+    const float* __restrict__ b0 = bias(P, S0);
+    const float* __restrict__ b1 = bias(P, S1);
     wg::resident_chain<wg::padn(N0), wg::pad16(K0), wg::padn(N1), std::is_same<Plan, BackwardPlan>::value>(
         step(), smem() + img_off(S0), smem() + img_off(S1), x, m, y, [&](int c, float v) { return fmaxf(v + __ldg(b0 + c), 0.f); });
 #pragma unroll
@@ -432,17 +491,18 @@ struct ResidentLayers {
     }
   }
   template <int SLOT, int Kv, int Nv>
-  static __device__ __forceinline__ void dx(const float* __restrict__ W, const float (&dy)[Nv], float (&dxv)[Kv]) {
-    static_assert(K(SLOT) == Kv && N(SLOT) == Nv, "slot shape");
+  static __device__ __forceinline__ void dx(const KParams& P, const float (&dy)[Nv], float (&dxv)[Kv]) {
+    static_assert(C::K(SLOT) == Kv && C::N(SLOT) == Nv, "slot shape");
     if constexpr (tensor(Nv))
       wg::resident_rowgemm_t<wg::padn(Nv), wg::pad16(Kv)>(step(), smem() + img_off(SLOT), dy, dxv);
     else
-      linear_bwd_input<Kv, Nv>(W, dy, dxv);
+      linear_bwd_input<Kv, Nv>(weight(P, SLOT), dy, dxv);
     FNR_PHASE(kPhDx);
   }
+  // dW / db into the CTA's accumulators, which flush adds to G
   template <int SLOT, int Kv, int Nv>
-  static __device__ __forceinline__ void dw(float*, float*, const float (&x)[Kv], const float (&dy)[Nv], float*, float*) {
-    static_assert(K(SLOT) == Kv && N(SLOT) == Nv, "slot shape");
+  static __device__ __forceinline__ void dw(const KParams&, const float (&x)[Kv], const float (&dy)[Nv]) {
+    static_assert(C::K(SLOT) == Kv && C::N(SLOT) == Nv, "slot shape");
     if constexpr (tensor(Nv))
       wg::weight_grad_acc<Kv, Nv>(step(), dw_region(), x, dy, acc<SLOT>(), lock(SLOT));
     else
@@ -454,43 +514,52 @@ struct ResidentLayers {
   // to dxv (for a 64-wide layer, 64 registers at the backward's peak; DESIGN.md section 4.3).
   // RELU (grad_relu): x is a ReLU's output and dxv is masked by it.  Once dW has read x, only its signs are needed, so
   // they are kept as one bit per input (bit k % 32 of word k / 32) and the floats are dead before dx runs.
-  template <int SLOT, int Kv, int Nv, bool RELU = false>
-  static __device__ __forceinline__ void grad(const float* __restrict__ W, float* sX, float* sY, const float (&x)[Kv],
-                                              const float (&dy)[Nv], float (&dxv)[Kv], float* gW, float* gb) {
-    dw<SLOT, Kv, Nv>(sX, sY, x, dy, gW, gb);
+  // A head's W is read before dw runs, where the call sites read it when they passed it.  This is a codegen guard, not a
+  // semantic requirement: reading it in dx moves the load and changes the backward kernel's register allocation; read
+  // here, the kernel compiles to the SASS it had before the slot interface.
+  template <int SLOT, bool RELU = false, int Kv, int Nv>
+  static __device__ __forceinline__ void grad(const KParams& P, const KParams& G, const float (&x)[Kv], const float (&dy)[Nv],
+                                              float (&dxv)[Kv]) {
+    [[maybe_unused]] const float* W = weight(P, SLOT);
+    dw<SLOT>(G, x, dy);
     uint32_t live[RELU ? (Kv + 31) / 32 : 1] = {};
     if constexpr (RELU) {
 #pragma unroll
       for (int k = 0; k < Kv; ++k) live[k / 32] |= (x[k] > 0.f ? 1u : 0u) << (k % 32);
     }
-    if constexpr (tensor(Nv)) {
+    if constexpr (tensor(Nv))
       wg::resident_rowgemm_t_staged<wg::padn(Nv), wg::pad16(Kv), Nv>(step(), smem() + img_off(SLOT), dxv);
-      FNR_PHASE(kPhDx);
-    } else {
-      dx<SLOT, Kv, Nv>(W, dy, dxv);
-    }
+    else
+      linear_bwd_input<Kv, Nv>(W, dy, dxv);
+    FNR_PHASE(kPhDx);
     if constexpr (RELU) {
 #pragma unroll
       for (int k = 0; k < Kv; ++k) dxv[k] = (live[k / 32] >> (k % 32)) & 1u ? dxv[k] : 0.f;
     }
   }
   template <int SLOT, int Kv, int Nv>
-  static __device__ __forceinline__ void grad_relu(const float* __restrict__ W, float* sX, float* sY, const float (&x)[Kv],
-                                                   const float (&dy)[Nv], float (&dxv)[Kv], float* gW, float* gb) {
-    grad<SLOT, Kv, Nv, true>(W, sX, sY, x, dy, dxv, gW, gb);
+  static __device__ __forceinline__ void grad_relu(const KParams& P, const KParams& G, const float (&x)[Kv], const float (&dy)[Nv],
+                                                   float (&dxv)[Kv]) {
+    grad<SLOT, true>(P, G, x, dy, dxv);
   }
   // m = relu(W x + b) of a chained pair's first layer on its own, by the backward's row path of fwd2: the same tile
   // bytes, MMAs and fp32 bias and ReLU, so m has the bits fwd2 gives.  The backward recomputes the base MLP's h1 with it.
   template <int SLOT, int Kv, int Nv>
-  static __device__ __forceinline__ void fwd_relu(const float* __restrict__ b, const float (&x)[Kv], float (&m)[Nv]) {
-    static_assert(K(SLOT) == Kv && N(SLOT) == Nv && tensor(Nv), "slot shape");
+  static __device__ __forceinline__ void fwd_relu(const KParams& P, const float (&x)[Kv], float (&m)[Nv]) {
+    static_assert(C::K(SLOT) == Kv && C::N(SLOT) == Nv && tensor(Nv), "slot shape");
+    const float* __restrict__ b = bias(P, SLOT);
     wg::resident_rowgemm<wg::padn(Nv), wg::pad16(Kv)>(step(), smem() + img_off(SLOT), x, m);
 #pragma unroll
     for (int n = 0; n < Nv; ++n) m[n] = fmaxf(m[n] + __ldg(b + n), 0.f);
   }
 };
 using ResidentForward = ResidentLayers<ForwardPlan>;
-using ResidentBackward = ResidentLayers<BackwardPlan>;
+
+// The layers of family C's field kernels in implementation TC (Plan: ForwardPlan for the forward and the export,
+// BackwardPlan for the backward): the small family's tensor-core kernels run on the resident image, the others on
+// Layers<C, TC>.
+template <class C, bool TC, class Plan>
+using FieldLayers = std::conditional_t<TC && std::is_same<C, CfgSmall>::value, ResidentLayers<Plan>, Layers<C, TC>>;
 
 template <class C>
 struct Acts {
@@ -508,14 +577,13 @@ struct Acts {
 // The field's branch forwards.  field_mlps and the backward's recompute both run these, so the recompute gives the
 // forward's pre-activations bit for bit and its ReLU masks agree with the forward that ran.
 //
-// Lin: how the layers are evaluated (Layers<C, TC> or ResidentLayers<Plan>).
+// Lin: the layer type (FieldLayers).
 //
 // base MLP: enc -> [h0, geo...]; geo = out[1:]
 template <class C, class Lin>
 __device__ __forceinline__ void base_fwd(const KParams& P, const float (&enc)[C::ENC], float (&h1)[C::BASE_H],
                                          float (&out)[C::BASE_OUT], float (&geo)[C::GEO]) {
-  Lin::template fwd2<kBase0, kBase1, C::ENC, C::BASE_H, C::BASE_OUT, false>(P.base_w[0], P.base_b[0], P.base_w[1], P.base_b[1], enc,
-                                                                            h1, out);
+  Lin::template fwd2<kBase0, kBase1, false>(P, enc, h1, out);
 #pragma unroll
   for (int i = 0; i < C::GEO; ++i) geo[i] = out[1 + i];
 }
@@ -525,11 +593,11 @@ template <class C, class Lin>
 __device__ __forceinline__ void semantic_fwd(const KParams& P, const float (&geo)[C::GEO], float (&z1)[C::SEM_H],
                                              float (&z2)[C::SEM_LAYERS == 3 ? C::SEM_H : 1], float (&zo)[C::SEM_OUT]) {
   if constexpr (C::SEM_LAYERS == 3) {
-    Lin::template fwd<kSem0, C::GEO, C::SEM_H, true>(P.sem_w[0], P.sem_b[0], geo, z1);
-    Lin::template fwd<kSem1, C::SEM_H, C::SEM_H, true>(P.sem_w[1], P.sem_b[1], z1, z2);
-    Lin::template fwd<kSem2, C::SEM_H, C::SEM_OUT, false>(P.sem_w[2], P.sem_b[2], z2, zo);
+    Lin::template fwd<kSem0, true>(P, geo, z1);
+    Lin::template fwd<kSem1, true>(P, z1, z2);
+    Lin::template fwd<kSem2, false>(P, z2, zo);
   } else {
-    Lin::template fwd2<kSem0, kSem1, C::GEO, C::SEM_H, C::SEM_OUT, false>(P.sem_w[0], P.sem_b[0], P.sem_w[1], P.sem_b[1], geo, z1, zo);
+    Lin::template fwd2<kSem0, kSem1, false>(P, geo, z1, zo);
   }
 }
 
@@ -550,8 +618,8 @@ __device__ __forceinline__ void colour_fwd(const KParams& P, const float* __rest
                                            const float (&app)[C::APP], float (&cin)[C::COL_IN], float (&c1)[C::COL_H],
                                            float (&c2)[C::COL_H], float (&o3)[3]) {
   colour_input<C>(dir, geo, app, cin);
-  Lin::template fwd2<kCol0, kCol1, C::COL_IN, C::COL_H, C::COL_H, true>(P.col_w[0], P.col_b[0], P.col_w[1], P.col_b[1], cin, c1, c2);
-  Lin::template fwd<kCol2, C::COL_H, 3, false>(P.col_w[2], P.col_b[2], c2, o3);
+  Lin::template fwd2<kCol0, kCol1, true>(P, cin, c1, c2);
+  Lin::template fwd<kCol2, false>(P, c2, o3);
 }
 
 template <class C, class Lin>
@@ -561,7 +629,7 @@ __device__ __forceinline__ void field_mlps(const KParams& P, const float (&enc)[
   base_fwd<C, Lin>(P, enc, a.h1, a.out, geo);
   semantic_fwd<C, Lin>(P, geo, a.z1, a.z2, a.zo);
   float lg[1];
-  Lin::template fwd<kHead, C::SEM_OUT, 1, false>(P.head_w, P.head_b, a.zo, lg);
+  Lin::template fwd<kHead, false>(P, a.zo, lg);
   a.logit = lg[0];
   float o3[3];
   colour_fwd<C, Lin>(P, dir, geo, app, a.cin, a.c1, a.c2, o3);
@@ -596,20 +664,9 @@ __device__ __forceinline__ void block_mean_embedding(const KParams& P, int num_i
 // ------------------------------------------------------------------------------------------
 // The small family's tensor-core forward and export run on the resident weight image (ResidentForward); the other
 // instantiations stage the weights at every layer step (Layers<C, TC>) in CTAs of one warpgroup.
-template <class C, bool TC>
-constexpr bool on_resident_image() { return TC && std::is_same<C, CfgSmall>::value; }
-template <class C, bool TC>
-constexpr int forward_groups() { return on_resident_image<C, TC>() ? ForwardPlan::kGroups : 1; }  // MMA warpgroups per CTA
-template <class C, bool TC>
-constexpr int forward_threads() { return on_resident_image<C, TC>() ? ForwardPlan::kThreadsPerCta : kThreads; }
-// The resident kernels name one CTA per SM, so that ptxas knows the registers at entry (168) and can apply setmaxnreg;
-// the others leave it unset, as before.
-template <class C, bool TC>
-constexpr int forward_min_ctas() { return on_resident_image<C, TC>() ? 1 : 0; }
-template <class C, bool TC>
-using ForwardLayers = std::conditional_t<on_resident_image<C, TC>(), ResidentForward, Layers<C, TC>>;
-// The warpgroup of this thread in a CTA of G warpgroups, and the thread's index in it (G = 1: the CTA's own indices, so
-// that the one-warpgroup kernels compile as they did before there were several)
+//
+// The warpgroup of this thread in a CTA of G = Lin::kGroups MMA warpgroups, and the thread's index in it (G = 1: the
+// CTA's own indices, so that the one-warpgroup kernels compile as they did before there were several)
 template <int G>
 __device__ __forceinline__ int group_of() { return G == 1 ? 0 : wg::group(); }
 template <int G>
@@ -700,10 +757,11 @@ __device__ __forceinline__ void resident_encoding(const KField& F, const KParams
 // warpgroup syncs on its own barrier only (wg::sync): the tile loop has no CTA-wide barrier, and a warpgroup without
 // tiles leaves at once.
 template <class C, bool TC>
-__global__ void __launch_bounds__(forward_threads<C, TC>(), forward_min_ctas<C, TC>()) simt_field_forward_kernel(KField F, KParams P, KRays Rr, KFieldOut O) {
-  constexpr bool kResident = on_resident_image<C, TC>();
-  constexpr int kGroups = forward_groups<C, TC>();
-  using Lin = ForwardLayers<C, TC>;
+__global__ void __launch_bounds__(FieldLayers<C, TC, ForwardPlan>::kThreadsPerCta, FieldLayers<C, TC, ForwardPlan>::kMinCtas)
+    simt_field_forward_kernel(KField F, KParams P, KRays Rr, KFieldOut O) {
+  using Lin = FieldLayers<C, TC, ForwardPlan>;
+  constexpr bool kResident = Lin::kResident;
+  constexpr int kGroups = Lin::kGroups;
   __shared__ float s_app[C::APP];
   block_mean_embedding(P, F.num_images, C::APP, F.appearance_mode, s_app);
   const long long N = (long long)Rr.R * Rr.S;
@@ -927,7 +985,7 @@ __global__ void __launch_bounds__(kThreads) simt_composite_backward_kernel(KRays
 // layer the tile's inputs X[128,K] and output grads dY[128,N] go to shared memory.  simt: each thread
 // reduces a 4x4 block of dW = dY^T X over the tile, then adds it to the global gradient.  Tensor cores:
 // the tile's dW is one MMA, added to the global gradient per tile (Layers<C, true>) or to accumulators in
-// shared memory that the CTA flushes once (ResidentBackward, small family).
+// shared memory that the CTA flushes once (ResidentLayers<BackwardPlan>, small family).
 // ------------------------------------------------------------------------------------------
 template <int K, int N>
 __device__ __forceinline__ void tile_weight_grad(float* __restrict__ sX, float* __restrict__ sY, const float (&x)[K],
@@ -979,21 +1037,14 @@ __device__ unsigned long long g_bwd_phase_cycles[kBwdPhases];
 #endif
 
 template <class C, bool TC>
-constexpr int backward_threads() { return on_resident_image<C, TC>() ? ResidentBackward::kGroups * kThreads : kThreads; }
-
-template <class C, bool TC>
-__global__ void __launch_bounds__(backward_threads<C, TC>()) simt_field_backward_kernel(KField F, KParams P, KParams G, KRays Rr,
-                                                                                       KFieldBwd B) {
-  constexpr bool kResident = on_resident_image<C, TC>();
-  constexpr int kGroups = backward_threads<C, TC>() / kThreads;  // warpgroups (tiles in flight) per CTA
-  using Lin = std::conditional_t<kResident, ResidentBackward, Layers<C, TC>>;
-  extern __shared__ __align__(16) float smem[];
-  constexpr int TP = ((C::MAXW + 3) & ~3) + 4;
-  float* sX = smem;
-  float* sY = smem + kThreads * TP;
+__global__ void __launch_bounds__(FieldLayers<C, TC, BackwardPlan>::kThreadsPerCta, FieldLayers<C, TC, BackwardPlan>::kMinCtas)
+    simt_field_backward_kernel(KField F, KParams P, KParams G, KRays Rr, KFieldBwd B) {
+  using Lin = FieldLayers<C, TC, BackwardPlan>;
+  constexpr bool kResident = Lin::kResident;
+  constexpr int kGroups = Lin::kGroups;  // warpgroups (tiles in flight) per CTA
   __shared__ float s_app[C::APP];
   block_mean_embedding(P, F.num_images, C::APP, F.appearance_mode, s_app);
-  if constexpr (kResident) ResidentBackward::prepare(P);
+  if constexpr (kResident) Lin::prepare(P);
 #ifdef FNR_BWD_PHASE_TIMERS
   if (threadIdx.x < 2 * kBwdPhases) phase::cycles[threadIdx.x / kBwdPhases][threadIdx.x % kBwdPhases] = 0;
   if (wg::tid() == 0) phase::last[wg::group()] = clock64();
@@ -1064,19 +1115,19 @@ __global__ void __launch_bounds__(backward_threads<C, TC>()) simt_field_backward
       FNR_PHASE(kPhRecompute);
       float dlg[1] = {d_logit};
       float dzo[C::SEM_OUT];
-      Lin::template grad<kHead, C::SEM_OUT, 1>(P.head_w, sX, sY, zo, dlg, dzo, G.head_w, G.head_b);
+      Lin::template grad<kHead>(P, G, zo, dlg, dzo);
       float dz1[C::SEM_H];
       if constexpr (C::SEM_LAYERS == 3) {
         float dz2[C::SEM_H];
-        Lin::template grad_relu<kSem2, C::SEM_H, C::SEM_OUT>(P.sem_w[2], sX, sY, z2, dzo, dz2, G.sem_w[2], G.sem_b[2]);
-        Lin::template grad_relu<kSem1, C::SEM_H, C::SEM_H>(P.sem_w[1], sX, sY, z1, dz2, dz1, G.sem_w[1], G.sem_b[1]);
+        Lin::template grad_relu<kSem2>(P, G, z2, dzo, dz2);
+        Lin::template grad_relu<kSem1>(P, G, z1, dz2, dz1);
       } else {
-        Lin::template grad_relu<kSem1, C::SEM_H, C::SEM_OUT>(P.sem_w[1], sX, sY, z1, dzo, dz1, G.sem_w[1], G.sem_b[1]);
+        Lin::template grad_relu<kSem1>(P, G, z1, dzo, dz1);
       }
-      Lin::template dw<kSem0, C::GEO, C::SEM_H>(sX, sY, geo, dz1, G.sem_w[0], G.sem_b[0]);
+      Lin::template dw<kSem0>(G, geo, dz1);
       if (F.pass_semantic_gradients) {
         float dg[C::GEO];
-        Lin::template dx<kSem0, C::GEO, C::SEM_H>(P.sem_w[0], dz1, dg);
+        Lin::template dx<kSem0>(P, dz1, dg);
 #pragma unroll
         for (int i = 0; i < C::GEO; ++i) d_geo[i] += dg[i];
       }
@@ -1096,14 +1147,14 @@ __global__ void __launch_bounds__(backward_threads<C, TC>()) simt_field_backward
         do3[i] = d_rgb[i] * rgb * (1.0f - rgb);
       }
       float dc2[C::COL_H], dc1[C::COL_H], dcin[C::COL_IN];
-      Lin::template grad_relu<kCol2, C::COL_H, 3>(P.col_w[2], sX, sY, c2, do3, dc2, G.col_w[2], G.col_b[2]);
-      Lin::template grad_relu<kCol1, C::COL_H, C::COL_H>(P.col_w[1], sX, sY, c1, dc2, dc1, G.col_w[1], G.col_b[1]);
+      Lin::template grad_relu<kCol2>(P, G, c2, do3, dc2);
+      Lin::template grad_relu<kCol1>(P, G, c1, dc2, dc1);
       if constexpr (kResident) {
         // cin again, from what built it, rather than carried through the col2 and col1 gradients
         load_appearance(P, F.appearance_mode, cam, s_app, appv);
         colour_input<C>(d, geo, appv, cin);
       }
-      Lin::template grad<kCol0, C::COL_IN, C::COL_H>(P.col_w[0], sX, sY, cin, dc1, dcin, G.col_w[0], G.col_b[0]);
+      Lin::template grad<kCol0>(P, G, cin, dc1, dcin);
 #pragma unroll
       for (int i = 0; i < C::GEO; ++i) d_geo[i] += dcin[C::SH + i];
       // appearance-embedding gradient (only the per-camera rows are parameters of the graph;
@@ -1144,12 +1195,12 @@ __global__ void __launch_bounds__(backward_threads<C, TC>()) simt_field_backward
           bool s;
           return field_position(o, d, Rr.starts[pc], Rr.ends[pc], F.position_mode, F.aabb, s);
         });
-        Lin::template fwd_relu<kBase0, C::ENC, C::BASE_H>(P.base_b[0], enc, h1);
+        Lin::template fwd_relu<kBase0>(P, enc, h1);
         FNR_PHASE(kPhRecompute);
       }
       float dh1[C::BASE_H];
-      Lin::template grad_relu<kBase1, C::BASE_H, C::BASE_OUT>(P.base_w[1], sX, sY, h1, dout, dh1, G.base_w[1], G.base_b[1]);
-      Lin::template grad<kBase0, C::ENC, C::BASE_H>(P.base_w[0], sX, sY, enc, dh1, denc, G.base_w[0], G.base_b[0]);
+      Lin::template grad_relu<kBase1>(P, G, h1, dout, dh1);
+      Lin::template grad<kBase0>(P, G, enc, dh1, denc);
     }
     // ---- hash-table gradient -----------------------------------------------------------------
     if constexpr (kResident) {
@@ -1177,7 +1228,7 @@ __global__ void __launch_bounds__(backward_threads<C, TC>()) simt_field_backward
 #ifdef FNR_BWD_PHASE_TIMERS
     const long long f0 = clock64();
 #endif
-    ResidentBackward::flush_all(G);
+    Lin::flush_all(G);
 #ifdef FNR_BWD_PHASE_TIMERS
     __syncthreads();
     if (threadIdx.x == 0) phase::cycles[0][kPhDwFlush] += (unsigned long long)(clock64() - f0);
@@ -1252,10 +1303,11 @@ __device__ __forceinline__ int warp_claim(int* counter, bool pred, int lane, int
 }
 
 template <class C, bool TC>
-__global__ void __launch_bounds__(forward_threads<C, TC>(), forward_min_ctas<C, TC>()) simt_export_kernel(KField F, KParams P, KExport E) {
-  constexpr bool kResident = on_resident_image<C, TC>();
-  constexpr int kGroups = forward_groups<C, TC>();
-  using Lin = ForwardLayers<C, TC>;
+__global__ void __launch_bounds__(FieldLayers<C, TC, ForwardPlan>::kThreadsPerCta, FieldLayers<C, TC, ForwardPlan>::kMinCtas)
+    simt_export_kernel(KField F, KParams P, KExport E) {
+  using Lin = FieldLayers<C, TC, ForwardPlan>;
+  constexpr bool kResident = Lin::kResident;
+  constexpr int kGroups = Lin::kGroups;
   __shared__ float s_app[C::APP];
   block_mean_embedding(P, F.num_images, C::APP, FNR_APP_MEAN, s_app);
   const int lane = threadIdx.x & 31;
@@ -1397,40 +1449,31 @@ int launch_simt_composite_backward(const KRays& Rr, const KCompositeBwd& B, cuda
   return check_launch("simt_composite_backward_kernel");
 }
 
-// One launch of a field kernel over N points.  Kernels with dynamic shared memory (the backward and every tensor-core
-// instantiation) opt in to it and run as many CTAs as fit on the SMs; the simt forward and export run 16 CTAs per SM.
-template <class Kernel, class... Args>
-static int launch_field_kernel(Kernel kernel, int smem, long long N, const char* name, cudaStream_t st, const Args&... args) {
+// One launch of a field kernel over N points on layer type Lin, with `smem` bytes of dynamic shared memory.  Resident
+// kernels run one CTA per SM (their shared memory is most of the SM's); the others with dynamic shared memory (the
+// backward and every tensor-core instantiation) opt in to it and run as many CTAs as fit on the SMs, and the simt forward
+// and export run 16 CTAs per SM.  No more CTAs than the points need (Lin::kGroups warpgroups per CTA, 128 points each).
+template <class Lin, class Kernel, class... Args>
+static int launch_field(Kernel kernel, int smem, long long N, const char* name, cudaStream_t st, const Args&... args) {
   if (N == 0) return FNR_OK;
-  int per_sm = 16;
+  int per_sm = Lin::kResident ? 1 : 16;
   if (smem > 0) {
     // per device: set on every call (cheap), so that a process driving several GPUs opts in on each of them
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute");
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, smem);
-    if (e != cudaSuccess) return check_cuda(e, "cudaOccupancyMaxActiveBlocksPerMultiprocessor");
-    if (per_sm < 1) per_sm = 1;
+    if (!Lin::kResident) {
+      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, Lin::kThreadsPerCta, smem);
+      if (e != cudaSuccess) return check_cuda(e, "cudaOccupancyMaxActiveBlocksPerMultiprocessor");
+      if (per_sm < 1) per_sm = 1;
+    }
   }
-  kernel<<<grid_for(N, kThreads, sm_count() * per_sm), kThreads, smem, st>>>(args...);
+  kernel<<<grid_for(N, Lin::kGroups * kThreads, sm_count() * per_sm), Lin::kThreadsPerCta, smem, st>>>(args...);
   return check_launch(name);
 }
 
-// One launch of a resident kernel (the small family's tensor-core forward, export and backward): one CTA of `threads`
-// per SM (its shared memory is most of the SM's), no more CTAs than the points need (`groups` MMA warpgroups per CTA,
-// 128 points each).
-template <class Kernel, class... Args>
-static int launch_resident(Kernel kernel, int threads, int groups, int smem, long long N, const char* name, cudaStream_t st,
-                           const Args&... args) {
-  if (N == 0) return FNR_OK;
-  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute");
-  kernel<<<grid_for(N, groups * kThreads, sm_count()), threads, smem, st>>>(args...);
-  return check_launch(name);
-}
-
-// Calls launch(C{}, std::bool_constant<TC>{}) with the family's config C and the implementation TC as types.
+// Returns launch(C{}, std::bool_constant<TC>{}) with the family's config C and the implementation TC as types.
 template <class Launch>
-static int with_layers(Family fam, bool tc, Launch launch) {
+static auto with_layers(Family fam, bool tc, Launch launch) {
   if (fam == kFamilySmall) return tc ? launch(CfgSmall{}, std::true_type{}) : launch(CfgSmall{}, std::false_type{});
   return tc ? launch(CfgBig{}, std::true_type{}) : launch(CfgBig{}, std::false_type{});
 }
@@ -1439,12 +1482,14 @@ int launch_field_forward(Family fam, bool tc, const KField& F, const KParams& P,
   return with_layers(fam, tc, [&](auto c, auto t) {
     using C = decltype(c);
     constexpr bool TC = decltype(t)::value;
-    if constexpr (on_resident_image<C, TC>())
-      return launch_resident(simt_field_forward_kernel<C, TC>, forward_threads<C, TC>(), ForwardPlan::kGroups, ForwardPlan::kBytes, (long long)Rr.R * Rr.S,
-                             "simt_field_forward_kernel<wgmma>", st, F, P, Rr, O);
-    return launch_field_kernel(simt_field_forward_kernel<C, TC>, Layers<C, TC>::kFwdSmemBytes, (long long)Rr.R * Rr.S,
-                               TC ? "simt_field_forward_kernel<wgmma>" : "simt_field_forward_kernel", st, F, P, Rr, O);
+    using Lin = FieldLayers<C, TC, ForwardPlan>;
+    return launch_field<Lin>(simt_field_forward_kernel<C, TC>, Lin::kFwdSmemBytes, (long long)Rr.R * Rr.S,
+                             TC ? "simt_field_forward_kernel<wgmma>" : "simt_field_forward_kernel", st, F, P, Rr, O);
   });
+}
+
+bool backward_uses_level_scatter(Family fam, bool tc) {
+  return with_layers(fam, tc, [](auto c, auto t) { return FieldLayers<decltype(c), decltype(t)::value, BackwardPlan>::kResident; });
 }
 
 int launch_field_backward(Family fam, bool tc, const KField& F, const KParams& P, const KParams& G, const KRays& Rr, const KFieldBwd& B,
@@ -1452,13 +1497,11 @@ int launch_field_backward(Family fam, bool tc, const KField& F, const KParams& P
   const int rc = with_layers(fam, tc, [&](auto c, auto t) {
     using C = decltype(c);
     constexpr bool TC = decltype(t)::value;
-    if constexpr (on_resident_image<C, TC>())
-      return launch_resident(simt_field_backward_kernel<C, TC>, backward_threads<C, TC>(), BackwardPlan::kGroups, BackwardPlan::kBytes, (long long)Rr.R * Rr.S,
-                             "simt_field_backward_kernel<wgmma>", st, F, P, G, Rr, B);
-    return launch_field_kernel(simt_field_backward_kernel<C, TC>, Layers<C, TC>::kBwdSmemBytes, (long long)Rr.R * Rr.S,
-                               TC ? "simt_field_backward_kernel<wgmma>" : "simt_field_backward_kernel", st, F, P, G, Rr, B);
+    using Lin = FieldLayers<C, TC, BackwardPlan>;
+    return launch_field<Lin>(simt_field_backward_kernel<C, TC>, Lin::kBwdSmemBytes, (long long)Rr.R * Rr.S,
+                             TC ? "simt_field_backward_kernel<wgmma>" : "simt_field_backward_kernel", st, F, P, G, Rr, B);
   });
-  if (rc || !(tc && fam == kFamilySmall)) return rc;
+  if (rc || !backward_uses_level_scatter(fam, tc)) return rc;
   return launch_level_scatter(F, Rr, B.denc, reinterpret_cast<float2*>(G.hash_table), st);
 }
 
@@ -1481,11 +1524,9 @@ int launch_export(Family fam, bool tc, const KField& F, const KParams& P, const 
   return with_layers(fam, tc, [&](auto c, auto t) {
     using C = decltype(c);
     constexpr bool TC = decltype(t)::value;
-    if constexpr (on_resident_image<C, TC>())
-      return launch_resident(simt_export_kernel<C, TC>, forward_threads<C, TC>(), ForwardPlan::kGroups, ForwardPlan::kBytes, (long long)E.B * E.S,
-                             "simt_export_kernel<wgmma>", st, F, P, E);
-    return launch_field_kernel(simt_export_kernel<C, TC>, Layers<C, TC>::kFwdSmemBytes, (long long)E.B * E.S,
-                               TC ? "simt_export_kernel<wgmma>" : "simt_export_kernel", st, F, P, E);
+    using Lin = FieldLayers<C, TC, ForwardPlan>;
+    return launch_field<Lin>(simt_export_kernel<C, TC>, Lin::kFwdSmemBytes, (long long)E.B * E.S,
+                             TC ? "simt_export_kernel<wgmma>" : "simt_export_kernel", st, F, P, E);
   });
 }
 

@@ -243,7 +243,7 @@ RESIDENT_GROUPS = 2  # warpgroups per CTA of the small family's tensor-core back
 
 def resident_backward_rounds(N: int, sms: int):
     """([tiles] round of each tile, CTA count) of the small family's tensor-core backward over N points on a GPU of ``sms``
-    SMs (fnr_simt.cu: launch_resident, simt_field_backward_kernel): min(ceil(N / 256), sms) CTAs of two warpgroups;
+    SMs (fnr_simt.cu: launch_field, simt_field_backward_kernel): min(ceil(N / 256), sms) CTAs of two warpgroups;
     warpgroup g of CTA b takes tile 2b + g, then every (2 * CTAs)-th tile after it, so tile t runs in round
     t // (2 * CTAs).  A CTA keeps its weight gradients on chip over all its rounds and flushes them after the last."""
     tiles = -(-N // TILE_POINTS)
