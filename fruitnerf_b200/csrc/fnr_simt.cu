@@ -1107,77 +1107,85 @@ __global__ void __launch_bounds__(FieldLayers<C, TC, BackwardPlan>::kThreadsPerC
 #pragma unroll
     for (int i = 0; i < C::GEO; ++i) d_geo[i] = 0.f;
 
-    // ---- semantic branch (its logit head is not needed: d_logit is the upstream gradient) ------------------------
-    {
-      float z1[C::SEM_H], zo[C::SEM_OUT];
-      float z2[C::SEM_LAYERS == 3 ? C::SEM_H : 1];
-      semantic_fwd<C, Lin>(P, geo, z1, z2, zo);
-      FNR_PHASE(kPhRecompute);
-      float dlg[1] = {d_logit};
-      float dzo[C::SEM_OUT];
-      Lin::template grad<kHead>(P, G, zo, dlg, dzo);
-      float dz1[C::SEM_H];
-      if constexpr (C::SEM_LAYERS == 3) {
-        float dz2[C::SEM_H];
-        Lin::template grad_relu<kSem2>(P, G, z2, dzo, dz2);
-        Lin::template grad_relu<kSem1>(P, G, z1, dz2, dz1);
-      } else {
-        Lin::template grad_relu<kSem1>(P, G, z1, dzo, dz1);
-      }
-      Lin::template dw<kSem0>(G, geo, dz1);
-      if (F.pass_semantic_gradients) {
-        float dg[C::GEO];
-        Lin::template dx<kSem0>(P, dz1, dg);
+    // Warpgroup 1 of the resident kernel runs the colour branch first, so that the CTA's two warpgroups run different
+    // layers rather than the same layers in step (DESIGN.md section 4.3); d_geo then adds the branches' terms in the
+    // other order.  The resident kernel runs both iterations, the semantic branch in iteration `sem` and the colour
+    // branch in the other, one copy of each in its code.  The other kernels run one iteration with both branches.
+    const int sem = kResident ? wg::group() : 0;
+#pragma unroll 1
+    for (int br = 0; br < (kResident ? 2 : 1); ++br) {
+      if (!kResident || br == sem) {
+        // ---- semantic branch (its logit head is not needed: d_logit is the upstream gradient) ----------------------
+        float z1[C::SEM_H], zo[C::SEM_OUT];
+        float z2[C::SEM_LAYERS == 3 ? C::SEM_H : 1];
+        semantic_fwd<C, Lin>(P, geo, z1, z2, zo);
+        FNR_PHASE(kPhRecompute);
+        float dlg[1] = {d_logit};
+        float dzo[C::SEM_OUT];
+        Lin::template grad<kHead>(P, G, zo, dlg, dzo);
+        float dz1[C::SEM_H];
+        if constexpr (C::SEM_LAYERS == 3) {
+          float dz2[C::SEM_H];
+          Lin::template grad_relu<kSem2>(P, G, z2, dzo, dz2);
+          Lin::template grad_relu<kSem1>(P, G, z1, dz2, dz1);
+        } else {
+          Lin::template grad_relu<kSem1>(P, G, z1, dzo, dz1);
+        }
+        Lin::template dw<kSem0>(G, geo, dz1);
+        if (F.pass_semantic_gradients) {
+          float dg[C::GEO];
+          Lin::template dx<kSem0>(P, dz1, dg);
 #pragma unroll
-        for (int i = 0; i < C::GEO; ++i) d_geo[i] += dg[i];
+          for (int i = 0; i < C::GEO; ++i) d_geo[i] += dg[i];
+        }
       }
-    }
-    // ---- colour branch ---------------------------------------------------------------------
-    {
-      float cin[C::COL_IN], c1[C::COL_H], c2[C::COL_H], o3[3];
-      // the resident kernel loads it here rather than with the point's inputs, so that it is not live through the base
-      // and semantic branches (fewer spills, DESIGN.md section 4.3)
-      if constexpr (kResident) load_appearance(P, F.appearance_mode, cam, s_app, appv);
-      colour_fwd<C, Lin>(P, d, geo, appv, cin, c1, c2, o3);
-      FNR_PHASE(kPhRecompute);
-      float do3[3];
+      if (!kResident || br != sem) {
+        // ---- colour branch -------------------------------------------------------------------
+        float cin[C::COL_IN], c1[C::COL_H], c2[C::COL_H], o3[3];
+        // the resident kernel loads it here rather than with the point's inputs, so that it is not live through the base
+        // and semantic branches (fewer spills, DESIGN.md section 4.3)
+        if constexpr (kResident) load_appearance(P, F.appearance_mode, cam, s_app, appv);
+        colour_fwd<C, Lin>(P, d, geo, appv, cin, c1, c2, o3);
+        FNR_PHASE(kPhRecompute);
+        float do3[3];
 #pragma unroll
-      for (int i = 0; i < 3; ++i) {
-        const float rgb = sigmoidf_(o3[i]);
-        do3[i] = d_rgb[i] * rgb * (1.0f - rgb);
-      }
-      float dc2[C::COL_H], dc1[C::COL_H], dcin[C::COL_IN];
-      Lin::template grad_relu<kCol2>(P, G, c2, do3, dc2);
-      Lin::template grad_relu<kCol1>(P, G, c1, dc2, dc1);
-      if constexpr (kResident) {
-        // cin again, from what built it, rather than carried through the col2 and col1 gradients
-        load_appearance(P, F.appearance_mode, cam, s_app, appv);
-        colour_input<C>(d, geo, appv, cin);
-      }
-      Lin::template grad<kCol0>(P, G, cin, dc1, dcin);
+        for (int i = 0; i < 3; ++i) {
+          const float rgb = sigmoidf_(o3[i]);
+          do3[i] = d_rgb[i] * rgb * (1.0f - rgb);
+        }
+        float dc2[C::COL_H], dc1[C::COL_H], dcin[C::COL_IN];
+        Lin::template grad_relu<kCol2>(P, G, c2, do3, dc2);
+        Lin::template grad_relu<kCol1>(P, G, c1, dc2, dc1);
+        if constexpr (kResident) {
+          // cin again, from what built it, rather than carried through the col2 and col1 gradients
+          load_appearance(P, F.appearance_mode, cam, s_app, appv);
+          colour_input<C>(d, geo, appv, cin);
+        }
+        Lin::template grad<kCol0>(P, G, cin, dc1, dcin);
 #pragma unroll
-      for (int i = 0; i < C::GEO; ++i) d_geo[i] += dcin[C::SH + i];
-      // appearance-embedding gradient (only the per-camera rows are parameters of the graph;
-      // the mean embedding spreads 1/num_images to every row)
-      if (F.appearance_mode == FNR_APP_PER_CAMERA) {
-        const bool uniform = __all_sync(kFull, cam == __shfl_sync(kFull, cam, 0));
-        if (uniform) {
+        for (int i = 0; i < C::GEO; ++i) d_geo[i] += dcin[C::SH + i];
+        // appearance-embedding gradient (only the per-camera rows are parameters of the graph;
+        // the mean embedding spreads 1/num_images to every row)
+        if (F.appearance_mode == FNR_APP_PER_CAMERA) {
+          const bool uniform = __all_sync(kFull, cam == __shfl_sync(kFull, cam, 0));
+          if (uniform) {
+#pragma unroll
+            for (int i = 0; i < C::APP; ++i) {
+              const float s = warp_sum(dcin[C::SH + C::GEO + i]);
+              if (lane == 0 && s != 0.f) atomicAdd(G.app_embedding + (size_t)cam * C::APP + i, s);
+            }
+          } else {
+#pragma unroll
+            for (int i = 0; i < C::APP; ++i)
+              if (dcin[C::SH + C::GEO + i] != 0.f) atomicAdd(G.app_embedding + (size_t)cam * C::APP + i, dcin[C::SH + C::GEO + i]);
+          }
+        } else if (F.appearance_mode == FNR_APP_MEAN) {
 #pragma unroll
           for (int i = 0; i < C::APP; ++i) {
-            const float s = warp_sum(dcin[C::SH + C::GEO + i]);
-            if (lane == 0 && s != 0.f) atomicAdd(G.app_embedding + (size_t)cam * C::APP + i, s);
+            const float s = warp_sum(dcin[C::SH + C::GEO + i]) / (float)F.num_images;
+            if (s != 0.f)
+              for (int row = lane; row < F.num_images; row += 32) atomicAdd(G.app_embedding + (size_t)row * C::APP + i, s);
           }
-        } else {
-#pragma unroll
-          for (int i = 0; i < C::APP; ++i)
-            if (dcin[C::SH + C::GEO + i] != 0.f) atomicAdd(G.app_embedding + (size_t)cam * C::APP + i, dcin[C::SH + C::GEO + i]);
-        }
-      } else if (F.appearance_mode == FNR_APP_MEAN) {
-#pragma unroll
-        for (int i = 0; i < C::APP; ++i) {
-          const float s = warp_sum(dcin[C::SH + C::GEO + i]) / (float)F.num_images;
-          if (s != 0.f)
-            for (int row = lane; row < F.num_images; row += 32) atomicAdd(G.app_embedding + (size_t)row * C::APP + i, s);
         }
       }
     }
